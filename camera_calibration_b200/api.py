@@ -160,6 +160,19 @@ class BundleAdjuster:
         _check(self.lib.b200ba_build_system(self._h, C.byref(opt), n, _dp(H), _dp(b), C.byref(cost)), self._h)
         return H, b, cost.value
 
+    def calibration_report(self, with_errors: bool = False):
+        """CreateCalibrationReport's numbers (calibration_report.cc:83-98) for every camera on the device-resident
+        state (``b200ba_calibration_report``). Returns (reports, errors, device_ms): one ``cabi.CameraReport``
+        per camera, and with ``with_errors`` the [n_obs, 2] array pixel - xy in the problem's observation order
+        (NaN where Project failed), else None. The state, last_projection and the Jacobians of the last
+        evaluation are left as they were."""
+        reports = (cabi.CameraReport * self.problem.n_cameras)()
+        errors = np.zeros((self.problem.n_obs, 2)) if with_errors else None
+        ms = C.c_double(0)
+        _check(self.lib.b200ba_calibration_report(self._h, reports, None if errors is None else _dp(errors), C.byref(ms)),
+               self._h)
+        return list(reports), errors, ms.value
+
     def timings(self) -> cabi.Timings:
         t = cabi.Timings()
         _check(self.lib.b200ba_get_timings(self._h, C.byref(t)), self._h)
@@ -897,3 +910,32 @@ def dataset_from_flat(problem: FlatProblem, state: FlatState) -> Tuple[Dataset, 
         m.set_flat_intrinsics(intr)
         st.intrinsics.append(m)
     return ds, st
+
+
+def _report_context(dataset: Dataset, state: BAState):
+    """Cached device context with the state of (dataset, state) uploaded."""
+    ctx, fs = _prepare(dataset, state)
+    ctx.adjuster.set_state(fs)
+    return ctx
+
+
+def CalibrationReports(dataset: Dataset, state: BAState, with_errors: bool = False):
+    """CreateCalibrationReport's numbers for every camera of (dataset, state) on the device:
+    ``BundleAdjuster.calibration_report`` through the cached ``_Context``. Returns (reports, errors, ctx)."""
+    ctx = _report_context(dataset, state)
+    reports, errors, _ = ctx.adjuster.calibration_report(with_errors)
+    return reports, errors, ctx
+
+
+def ComputeAllReprojectionErrors(camera_index: int, dataset: Dataset, state: BAState):
+    """APP/calibration_report.cc:101-148: every feature of one camera in the used imagesets, in dataset
+    order, re-projected with Project (no warm start). Returns (count, sum, max, errors [count, 2],
+    features [count, 2] float32) over the successful projections; count / sum / max come from the
+    device's fixed-order reduction."""
+    reports, errors, ctx = CalibrationReports(dataset, state, with_errors=True)
+    sel = ctx.problem.obs_camera == camera_index
+    e = errors[sel]
+    ok = ~np.isnan(e[:, 0])
+    r = reports[camera_index]
+    return (int(r.reprojection_error_count), float(r.reprojection_error_sum), float(r.reprojection_error_max), e[ok],
+            np.asarray(ctx.problem.obs_xy)[sel][ok])

@@ -198,6 +198,24 @@ class Timings(C.Structure):
     ]
 
 
+REPORT_HIST = 50
+
+
+class CameraReport(C.Structure):
+    """b200ba_camera_report: CreateCalibrationReport's numbers for one camera."""
+    _fields_ = [
+        ("reprojection_error_count", C.c_int64),
+        ("reprojection_error_sum", C.c_double),
+        ("reprojection_error_max", C.c_double),
+        ("reprojection_error_median", C.c_double),
+        ("biasedness", C.c_double),
+        ("biasedness_cells", C.c_int32),
+        ("horizontal_fov", C.c_double),
+        ("vertical_fov", C.c_double),
+        ("histogram", C.c_int32 * (REPORT_HIST * REPORT_HIST)),
+    ]
+
+
 class FitReport(C.Structure):
     """b200ba_fit_report."""
     _fields_ = [
@@ -370,6 +388,7 @@ SYMBOLS = {
                                              C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double)]),
     "b200ba_run_bundle_adjustment": (C.c_int, [C.c_void_p, C.POINTER(Options), C.c_int32, C.c_double, C.POINTER(BAReport),
                                               ON_ITERATION, C.c_void_p]),
+    "b200ba_calibration_report": (C.c_int, [C.c_void_p, C.POINTER(CameraReport), _D, _D]),
     "b200ba_snapshot_state": (C.c_int, [C.c_void_p]),
     "b200ba_restore_state": (C.c_int, [C.c_void_p]),
     "b200ba_version": (C.c_char_p, []),

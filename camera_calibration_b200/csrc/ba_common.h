@@ -107,6 +107,32 @@ struct SystemDev {
   double* scalars;  // [8]: cost, n_valid, ...
 };
 
+// Calibration report (b200ba_calibration_report): per-camera results and scratch of the radix select.
+constexpr int kReportBiasCells = 50;  // kBiasCellCount of ComputeBiasedness (calibration_report.cc:222)
+struct ReportCam {
+  long long count;
+  double sum, max, median;
+  double biasedness;
+  int biasedness_cells;
+  double hfov, vfov;
+  unsigned long long select_prefix;  // bits of the median chosen so far
+  long long select_rank;             // rank of the median among the values sharing that prefix
+};
+// Report-owned device buffers (allocated on the first report; none of them is read by the LM path).
+struct ReportDev {
+  double2* err;          // [n_obs] pixel - xy, device order; NaN where Project failed
+  double* mag;           // [n_obs] |err|, NaN where Project failed
+  int64_t* cam_off;      // [n_cameras + 1] range of each camera in the device order
+  int* cell_off;         // [n_cameras * 2500 + 1] range of each (camera, bias cell) in cell_order
+  uint32_t* cell_order;  // [n_obs] device positions by (camera, bias cell), caller's order inside a cell
+  double* Q;             // [64] the normalised 8 x 8 Gaussian table, y-major
+  double* partial;       // report_partial_size(n_cameras)
+  unsigned int* select_hist;  // [n_cameras * 256]
+  int* hist;             // [n_cameras * 2500] error histogram, [hy * 50 + hx]
+  double* kl;            // [n_cameras * 2500] KL divergence per bias cell, NaN if skipped
+  ReportCam* cams;       // [n_cameras]
+};
+
 // Up to four ranges [lo, hi) of global unknown indices held fixed (debug_fix_* of OptimizeJointly).
 struct FixedRanges {
   int n;

@@ -166,6 +166,11 @@ struct b200ba_handle {
   int force_grouped = -1;                 // B200BA_GROUPED=0|1 overrides the cost model
   bool compact_j = true;                  // B200BA_COMPACT_J=0: expanded Jacobian buffer also for central-generic cameras
 
+  // calibration report: allocated by the first b200ba_calibration_report
+  ReportDev rep{};
+  double2* d_rep_stage = nullptr;  // errors in the caller's order (D2H staging)
+  bool have_report = false;
+
   // multi-GPU
   void* comm = nullptr;
   int rank = 0, n_ranks = 1;
@@ -1138,6 +1143,9 @@ void free_handle_buffers(b200ba_handle* h) {
   if (h->h_count) cudaFreeHost(h->h_count);
   h->h_count = nullptr;
   F(h->d_partial); F(h->d_scal); F(h->d_rot);
+  F(h->rep.err); F(h->rep.mag); F(h->rep.cam_off); F(h->rep.cell_off); F(h->rep.cell_order); F(h->rep.Q);
+  F(h->rep.partial); F(h->rep.select_hist); F(h->rep.hist); F(h->rep.kl); F(h->rep.cams); F(h->d_rep_stage);
+  h->have_report = false;
   F(h->dn.Lpack); F(h->dn.tmp); F(h->dn.d_panel_off); F(h->dn.d_panel_h); F(h->d_ident_cols); F(h->d_gemv_partial);
   h->dn.S = nullptr;
   h->dense_planned_n = -1;
@@ -1145,6 +1153,68 @@ void free_handle_buffers(b200ba_handle* h) {
   if (h->h_flags) cudaFreeHost(h->h_flags);
   h->h_scal = nullptr;
   h->h_flags = nullptr;
+}
+
+// First b200ba_calibration_report: allocates the report's buffers and uploads what depends on the problem
+// only -- the camera ranges of the device order, the ordering by (camera, bias cell) and the Gaussian table
+// of ComputeBiasedness (calibration_report.cc:241-258, computed here with std::exp).
+int setup_report(b200ba_handle* h) {
+  if (h->have_report) return 0;
+  const int64_t n = h->n_obs;
+  const int nc = h->n_cameras;
+  constexpr int kCells = kReportBiasCells * kReportBiasCells;
+  // the device order is sorted by camera first (b200ba_create): each camera is one range
+  std::vector<int64_t> cam_off(nc + 1, 0);
+  for (int64_t o = 0; o < n; ++o) ++cam_off[h->h_obs_camera[o] + 1];
+  for (int c = 0; c < nc; ++c) cam_off[c + 1] += cam_off[c];
+  // bias cell of every observation (:225-235): step = (max - min) / 50.0 + 1e-7; the subtraction
+  // xy - min is float - int in float, the division is in double, the conversion truncates
+  std::vector<uint32_t> key(n);
+  std::vector<int> cell_off(static_cast<size_t>(nc) * kCells + 1, 0);
+  for (int64_t o = 0; o < n; ++o) {
+    const uint32_t cam = h->h_obs_camera[o];
+    const b200ba_camera& c = h->cams_host[cam];
+    const double step_u = static_cast<double>(c.calibration_max_x - c.calibration_min_x) / kReportBiasCells + 1e-7;
+    const double step_v = static_cast<double>(c.calibration_max_y - c.calibration_min_y) / kReportBiasCells + 1e-7;
+    const float dx = h->h_obs_xy[2 * o] - static_cast<float>(c.calibration_min_x);
+    const float dy = h->h_obs_xy[2 * o + 1] - static_cast<float>(c.calibration_min_y);
+    const int cx = std::min(kReportBiasCells - 1, std::max(0, static_cast<int>(dx / step_u)));
+    const int cy = std::min(kReportBiasCells - 1, std::max(0, static_cast<int>(dy / step_v)));
+    key[o] = cam * kCells + cy * kReportBiasCells + cx;
+    ++cell_off[key[o] + 1];
+  }
+  for (size_t k = 0; k + 1 < cell_off.size(); ++k) cell_off[k + 1] += cell_off[k];
+  // stable counting sort by key: the caller's order inside each cell; entries are device positions
+  std::vector<uint32_t> pos(n), order(n);
+  for (int64_t i = 0; i < n; ++i) pos[h->perm[i]] = static_cast<uint32_t>(i);
+  {
+    std::vector<int> fill(cell_off.begin(), cell_off.end() - 1);
+    for (int64_t o = 0; o < n; ++o) order[fill[key[o]]++] = pos[o];
+  }
+  // Q(x, y) = exp(-0.5 (dx^2 + dy^2)), dx = (2.5 / (0.5 * 8)) * (0.5 * 8 - (x + 0.5)), normalised; y-major
+  double Q[64], q_sum = 0;
+  for (int y = 0; y < 8; ++y)
+    for (int x = 0; x < 8; ++x) {
+      const double dx = (2.5 / (0.5 * 8)) * (0.5 * 8 - (x + 0.5));
+      const double dy = (2.5 / (0.5 * 8)) * (0.5 * 8 - (y + 0.5));
+      const double p = std::exp(-0.5 * (dx * dx + dy * dy));
+      Q[y * 8 + x] = p;
+      q_sum += p;
+    }
+  for (double& q : Q) q /= q_sum;
+  ReportDev& r = h->rep;
+  if (dev_alloc(h, &r.err, n) || dev_alloc(h, &r.mag, n) || dev_alloc(h, &r.cam_off, nc + 1) ||
+      dev_alloc(h, &r.cell_off, cell_off.size()) || dev_alloc(h, &r.cell_order, n) || dev_alloc(h, &r.Q, 64) ||
+      dev_alloc(h, &r.partial, report_partial_size(nc)) || dev_alloc(h, &r.select_hist, 256 * nc) ||
+      dev_alloc(h, &r.hist, static_cast<size_t>(nc) * B200BA_REPORT_HIST * B200BA_REPORT_HIST) ||
+      dev_alloc(h, &r.kl, static_cast<size_t>(nc) * kCells) || dev_alloc(h, &r.cams, nc) || dev_alloc(h, &h->d_rep_stage, n))
+    return 1;
+  CUDA_TRY(h, cudaMemcpy(r.cam_off, cam_off.data(), cam_off.size() * sizeof(int64_t), cudaMemcpyHostToDevice));
+  CUDA_TRY(h, cudaMemcpy(r.cell_off, cell_off.data(), cell_off.size() * sizeof(int), cudaMemcpyHostToDevice));
+  if (n > 0) CUDA_TRY(h, cudaMemcpy(r.cell_order, order.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice));
+  CUDA_TRY(h, cudaMemcpy(r.Q, Q, sizeof(Q), cudaMemcpyHostToDevice));
+  h->have_report = true;
+  return 0;
 }
 
 }  // namespace
@@ -1482,6 +1552,65 @@ int b200ba_restore_state(b200ba_handle* h) {
   }
   CUDA_TRY(h, cudaSetDevice(h->device));
   return copy_state_dev(h, h->snap, h->d_snap_lp, h->st[h->cur], h->d_last_projection);
+}
+
+int b200ba_calibration_report(b200ba_handle* h, b200ba_camera_report* reports, double* errors, double* report_ms) {
+  if (!h) return 1;
+  if (!reports) {
+    h->error = "reports is NULL";
+    return 2;
+  }
+  if (h->comm || h->n_ranks > 1) {
+    h->error = "b200ba_calibration_report: the handle is joined to a communicator and holds one shard of the "
+               "observations; the report needs all of them (use a single-rank handle)";
+    return 2;
+  }
+  if (!h->have_state) {
+    h->error = "no state: call b200ba_set_state first";
+    return 2;
+  }
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  if (setup_report(h)) return 1;
+  const int nc = h->n_cameras;
+  // prepare_state only refreshes the derived image_tr_global / tangents caches of the current state
+  Layout L{};
+  L.n_points = h->n_points;
+  L.n_imagesets = h->n_imagesets;
+  L.n_cameras = nc;
+  cudaEvent_t a = get_event(h), b = get_event(h);
+  cudaEventRecord(a, h->stream);
+  launch_prepare_state(h->pb, L, h->st[h->cur], h->n_control_total, h->stream);
+  launch_calibration_report(h->pb, nc, h->st[h->cur], h->rep, h->stream);
+  cudaEventRecord(b, h->stream);
+  CUDA_TRY(h, cudaGetLastError());
+  constexpr int kBins = B200BA_REPORT_HIST * B200BA_REPORT_HIST;
+  std::vector<ReportCam> rc(nc);
+  std::vector<int32_t> hist(static_cast<size_t>(nc) * kBins);
+  CUDA_TRY(h, cudaMemcpyAsync(rc.data(), h->rep.cams, nc * sizeof(ReportCam), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(hist.data(), h->rep.hist, hist.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
+  if (errors && h->n_obs > 0) {
+    launch_permute_double2(h->n_obs, h->d_perm, h->rep.err, h->d_rep_stage, /*scatter=*/true, h->stream);
+    CUDA_TRY(h, cudaMemcpyAsync(errors, h->d_rep_stage, 2 * sizeof(double) * h->n_obs, cudaMemcpyDeviceToHost, h->stream));
+  }
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  float ms = 0;
+  CUDA_TRY(h, cudaEventElapsedTime(&ms, a, b));
+  h->event_pool.push_back(a);
+  h->event_pool.push_back(b);
+  if (report_ms) *report_ms = ms;
+  for (int c = 0; c < nc; ++c) {
+    b200ba_camera_report& r = reports[c];
+    r.reprojection_error_count = rc[c].count;
+    r.reprojection_error_sum = rc[c].sum;
+    r.reprojection_error_max = rc[c].max;
+    r.reprojection_error_median = rc[c].median;
+    r.biasedness = rc[c].biasedness;
+    r.biasedness_cells = rc[c].biasedness_cells;
+    r.horizontal_fov = rc[c].hfov;
+    r.vertical_fov = rc[c].vfov;
+    memcpy(r.histogram, hist.data() + static_cast<size_t>(c) * kBins, kBins * sizeof(int32_t));
+  }
+  return 0;
 }
 
 int32_t b200ba_degrees_of_freedom(const b200ba_handle* h, const b200ba_options* opt) {

@@ -1737,6 +1737,344 @@ void launch_unproject_pixels(const CamDev& c, const double* intr, int64_t n, con
   unproject_pixels_kernel<<<static_cast<unsigned>((n + 127) / 128), 128, 0, s>>>(c, intr, n, px, dirs, origins, ok);
 }
 
+// ------------------------------------------------------------------------------------------
+// calibration report (APP/calibration_report.cc:83-98, per camera :713-817)
+// ------------------------------------------------------------------------------------------
+// Everything below works on the device (cell-major) observation order, in which every camera is
+// one contiguous range [cam_off[c], cam_off[c + 1]). Bin and cell indices depend on the last bit
+// of the values they are computed from, so those expressions use __dmul_rn / __dadd_rn (no FMA
+// contraction) and evaluate in the reference's order; the CPU side is compiled with
+// -ffp-contract=off for the same reason.
+
+// static_cast<int>(double) as x86-64 executes it (cvttsd2si): truncation toward zero, and INT_MIN
+// for NaN and for values outside the int range, where CUDA's conversion would saturate instead.
+__device__ __forceinline__ int report_trunc(double v) {
+  return (v > -2147483649.0 && v < 2147483648.0) ? static_cast<int>(v) : INT_MIN;
+}
+
+// Eigen's Vector2d::norm(): sqrt(x * x + y * y) with no fused multiply-add
+__device__ __forceinline__ double report_norm(double x, double y) {
+  return sqrt(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y)));
+}
+
+// ComputeAllReprojectionErrors (:101-148): local point from the image_tr_global cache, Project()
+// (start at CenterOfCalibratedArea, no warm start; central_grid.h:79-97, noncentral_generic.h:88-93)
+// with the projection code of the residual kernel. err = pixel - xy, NaN where Project fails.
+__global__ void report_errors_kernel(ProblemDev pb, int n_cameras, StateDev st, double2* __restrict__ err,
+                                     double* __restrict__ mag) {
+  const int64_t o = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (o >= pb.n_obs) return;
+  const int iset = static_cast<int>(pb.obs_imageset[o]);
+  const int cam = static_cast<int>(pb.obs_camera[o]);
+  const CamDev& c = pb.cams[cam];
+  const double* T = st.image_tr_global + 12 * (static_cast<int64_t>(iset) * n_cameras + cam);
+  double R[9];
+#pragma unroll
+  for (int i = 0; i < 9; ++i) R[i] = __ldg(T + i);
+  const d3 lp = rot_apply(R, ld3(st.points + 3 * static_cast<int64_t>(pb.obs_point[o]))) +
+                mk3(__ldg(T + 9), __ldg(T + 10), __ldg(T + 11));
+  const double* intr = st.intrinsics + c.intr_off;
+  double px = c.center_x, py = c.center_y;
+  bool ok;
+  if (c.model_type == B200BA_MODEL_CENTRAL_GENERIC) {
+    CentralEval e;
+    int ne = 0;
+    ok = central_project(c, intr, rsqrt(dot3(lp, lp)) * lp, px, py, e, ne, kUnlimitedEvals) == kProjOk;
+  } else if (c.model_type == B200BA_MODEL_NONCENTRAL_GENERIC) {
+    NoncentralEval e;
+    d3 t1, t2;
+    double Rn[2][2];
+    int ne = 0;
+    ok = noncentral_project(c, intr, intr + 3 * static_cast<int64_t>(c.gw) * c.gh, lp, px, py, e, t1, t2, Rn, ne,
+                            kUnlimitedEvals) == kProjOk;
+  } else {
+    ok = opencv_project(c, intr, lp, px, py);
+  }
+  if (!ok) {
+    err[o] = make_double2(nan(""), nan(""));
+    mag[o] = nan("");
+    return;
+  }
+  const float2 xy = pb.obs_xy[o];
+  const double ex = px - static_cast<double>(xy.x), ey = py - static_cast<double>(xy.y);
+  err[o] = make_double2(ex, ey);
+  mag[o] = report_norm(ex, ey);
+}
+
+// count, sum and max of |e| per camera: two stages with a compile-time grid, like cost_reduce_stage1/2,
+// so that the sum is the same on every GPU.
+constexpr int kReportBlocks = 132;
+constexpr int kReportThreads = 256;
+__global__ void __launch_bounds__(kReportThreads)
+    report_reduce_stage1(const int64_t* __restrict__ cam_off, const double* __restrict__ mag, double* __restrict__ partial) {
+  const int cam = blockIdx.y;
+  double cnt = 0, sum = 0, mx = 0;
+  for (int64_t o = cam_off[cam] + blockIdx.x * static_cast<int64_t>(kReportThreads) + threadIdx.x; o < cam_off[cam + 1];
+       o += static_cast<int64_t>(kReportBlocks) * kReportThreads) {
+    const double m = mag[o];
+    if (!isnan(m)) {
+      cnt += 1;
+      sum += m;
+      mx = fmax(mx, m);
+    }
+  }
+  __shared__ double sh[3][kReportThreads];
+  sh[0][threadIdx.x] = cnt;
+  sh[1][threadIdx.x] = sum;
+  sh[2][threadIdx.x] = mx;
+  __syncthreads();
+  for (int s = kReportThreads / 2; s > 0; s >>= 1) {
+    if (threadIdx.x < s) {
+      sh[0][threadIdx.x] += sh[0][threadIdx.x + s];
+      sh[1][threadIdx.x] += sh[1][threadIdx.x + s];
+      sh[2][threadIdx.x] = fmax(sh[2][threadIdx.x], sh[2][threadIdx.x + s]);
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x < 3) partial[(static_cast<int64_t>(cam) * kReportBlocks + blockIdx.x) * 3 + threadIdx.x] = sh[threadIdx.x][0];
+}
+__global__ void report_reduce_stage2(int n_cameras, const double* __restrict__ partial, ReportCam* __restrict__ rc) {
+  const int cam = threadIdx.x;
+  if (cam >= n_cameras) return;
+  double cnt = 0, sum = 0, mx = 0;
+  for (int b = 0; b < kReportBlocks; ++b) {
+    const double* p = partial + (static_cast<int64_t>(cam) * kReportBlocks + b) * 3;
+    cnt += p[0];
+    sum += p[1];
+    mx = fmax(mx, p[2]);
+  }
+  ReportCam& r = rc[cam];
+  r.count = static_cast<long long>(cnt);
+  r.sum = sum;
+  r.max = mx;
+  r.select_prefix = 0;
+  r.select_rank = r.count / 2;
+}
+
+// Median (WriteReportInfoFile, :685-693: sorted(|e|)[count / 2]) by radix select on the bit patterns:
+// non-negative doubles order like their uint64 patterns. 8 passes of 8 bits; pass p histograms digit
+// 7 - p of the values whose higher digits equal the prefix chosen so far.
+constexpr int kSelectBlocks = 132;
+__global__ void __launch_bounds__(kReportThreads)
+    report_select_hist_kernel(int pass, const int64_t* __restrict__ cam_off, const double* __restrict__ mag,
+                              const ReportCam* __restrict__ rc, unsigned int* __restrict__ hist) {
+  const int cam = blockIdx.y;
+  __shared__ unsigned int h[256];
+  h[threadIdx.x] = 0;
+  __syncthreads();
+  const int shift = 56 - 8 * pass;
+  const unsigned long long prefix = rc[cam].select_prefix;
+  for (int64_t o = cam_off[cam] + blockIdx.x * static_cast<int64_t>(kReportThreads) + threadIdx.x; o < cam_off[cam + 1];
+       o += static_cast<int64_t>(kSelectBlocks) * kReportThreads) {
+    const double m = mag[o];
+    if (isnan(m)) continue;
+    const unsigned long long bits = static_cast<unsigned long long>(__double_as_longlong(m));
+    if (pass > 0 && ((bits ^ prefix) >> (shift + 8)) != 0) continue;
+    atomicAdd(&h[(bits >> shift) & 255], 1u);
+  }
+  __syncthreads();
+  if (h[threadIdx.x]) atomicAdd(&hist[cam * 256 + threadIdx.x], h[threadIdx.x]);
+}
+__global__ void report_select_scan_kernel(int pass, int n_cameras, unsigned int* __restrict__ hist,
+                                          ReportCam* __restrict__ rc) {
+  const int cam = threadIdx.x;
+  if (cam >= n_cameras) return;
+  ReportCam& r = rc[cam];
+  unsigned int* h = hist + cam * 256;
+  long long k = r.select_rank;
+  int digit = 255;
+  for (int d = 0; d < 256; ++d) {
+    if (k < static_cast<long long>(h[d])) {
+      digit = d;
+      break;
+    }
+    k -= h[d];
+  }
+  for (int d = 0; d < 256; ++d) h[d] = 0;
+  r.select_rank = k;
+  r.select_prefix |= static_cast<unsigned long long>(digit) << (56 - 8 * pass);
+  if (pass == 7) r.median = r.count > 0 ? __longlong_as_double(static_cast<long long>(r.select_prefix)) : nan("");
+}
+
+// ComputeReprojectionErrorHistogram (:151-168) with kHistResolution = 50, kHistExtent = 0.2f (:739-743):
+// hx_f = (50 * 0.5f) * (e.x / extent + 1.f), hx = int(hx_f) - (hx_f < 0 ? 1.f : 0.f) (a float subtraction)
+__device__ __forceinline__ int report_hist_bin(double e) {
+  const double extent = static_cast<double>(0.2f);
+  const double f = __dmul_rn(25.0, __dadd_rn(e / extent, 1.0));
+  const int i = report_trunc(f);
+  return f < 0 ? report_trunc(static_cast<double>(static_cast<float>(i) - 1.f)) : i;
+}
+constexpr int kHistBlocks = 66;
+__global__ void __launch_bounds__(kReportThreads)
+    report_hist_kernel(const int64_t* __restrict__ cam_off, const double2* __restrict__ err, int* __restrict__ hist) {
+  const int cam = blockIdx.y;
+  constexpr int kBins = B200BA_REPORT_HIST * B200BA_REPORT_HIST;
+  __shared__ int h[kBins];
+  for (int i = threadIdx.x; i < kBins; i += kReportThreads) h[i] = 0;
+  __syncthreads();
+  for (int64_t o = cam_off[cam] + blockIdx.x * static_cast<int64_t>(kReportThreads) + threadIdx.x; o < cam_off[cam + 1];
+       o += static_cast<int64_t>(kHistBlocks) * kReportThreads) {
+    const double2 e = err[o];
+    if (isnan(e.x)) continue;
+    const int hx = report_hist_bin(e.x), hy = report_hist_bin(e.y);
+    if (hx >= 0 && hy >= 0 && hx < B200BA_REPORT_HIST && hy < B200BA_REPORT_HIST) atomicAdd(&h[hy * B200BA_REPORT_HIST + hx], 1);
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < kBins; i += kReportThreads)
+    if (h[i]) atomicAdd(&hist[cam * kBins + i], h[i]);
+}
+
+// ComputeBiasedness (:171-351), one warp per (camera, bias cell). order lists the device positions of
+// the cell's observations in the caller's order (cell_off: [n_cameras * 2500 + 1]). Lane 0 takes the
+// Welford mean of |e| (libvis statistics.h:55-63) in that order; cells with fewer than 5 errors are
+// skipped (kl = NaN). The lanes bin e * (1.25331 / mean) into the 8 x 8 table (:284-296), lane 0 sums
+// P log(P / Q) over the non-empty bins in y-then-x order (:328-337).
+__device__ __forceinline__ int report_bias_bin(double n) {
+  // -1 * (n * (0.5 * 8) / 2.5 - 0.5 * 8), truncated, clamped to [0, 7]
+  const double v = -__dadd_rn(__dmul_rn(n, 4.0) / 2.5, -4.0);
+  return min(7, max(0, report_trunc(v)));
+}
+__global__ void __launch_bounds__(256)
+    report_bias_kernel(int n_cells, const int* __restrict__ cell_off, const uint32_t* __restrict__ order,
+                       const double2* __restrict__ err, const double* __restrict__ mag, const double* __restrict__ Q,
+                       double* __restrict__ kl) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int cell = blockIdx.x * 8 + warp;
+  __shared__ int bins[8][64];
+  if (cell >= n_cells) return;
+  const int a = cell_off[cell], b = cell_off[cell + 1];
+  double mean = 0;
+  unsigned int count = 0;
+  if (lane == 0) {
+    for (int i = a; i < b; ++i) {
+      const double m = mag[order[i]];
+      if (isnan(m)) continue;
+      ++count;
+      const double delta = m - mean;
+      mean = __dadd_rn(mean, delta / static_cast<double>(count));
+    }
+  }
+  count = __shfl_sync(0xffffffffu, count, 0);
+  mean = __shfl_sync(0xffffffffu, mean, 0);
+  if (count < 5) {
+    if (lane == 0) kl[cell] = nan("");
+    return;
+  }
+  bins[warp][lane] = 0;
+  bins[warp][lane + 32] = 0;
+  __syncwarp();
+  const double s = 1.25331 / mean;
+  for (int i = a + lane; i < b; i += 32) {
+    const double2 e = err[order[i]];
+    if (isnan(e.x)) continue;
+    atomicAdd(&bins[warp][report_bias_bin(__dmul_rn(e.y, s)) * 8 + report_bias_bin(__dmul_rn(e.x, s))], 1);
+  }
+  __syncwarp();
+  if (lane == 0) {
+    const double total = static_cast<double>(count);
+    double d = 0;
+    for (int k = 0; k < 64; ++k) {
+      const int c = bins[warp][k];
+      if (c == 0) continue;
+      const double P = c / total;
+      d = __dadd_rn(d, __dmul_rn(P, log(P / Q[k])));
+    }
+    kl[cell] = d;
+  }
+}
+
+// Biasedness = sorted(KL)[size / 2] over the cells that were not skipped: one block per camera sorts its
+// (at most 2 500) values with a bitonic network in shared memory.
+constexpr int kBiasSortN = 4096;
+__global__ void __launch_bounds__(1024) report_bias_median_kernel(const double* __restrict__ kl, ReportCam* __restrict__ rc) {
+  constexpr int kCells = kReportBiasCells * kReportBiasCells;
+  const int cam = blockIdx.x;
+  __shared__ double v[kBiasSortN];
+  int valid = 0;
+  for (int i = threadIdx.x; i < kBiasSortN; i += blockDim.x) {
+    const double x = i < kCells ? kl[cam * kCells + i] : nan("");
+    v[i] = isnan(x) ? INFINITY : x;
+    valid += isnan(x) ? 0 : 1;
+  }
+  __shared__ int n_valid;
+  if (threadIdx.x == 0) n_valid = 0;
+  __syncthreads();
+  atomicAdd(&n_valid, valid);
+  for (int k = 2; k <= kBiasSortN; k <<= 1) {
+    for (int j = k >> 1; j > 0; j >>= 1) {
+      __syncthreads();
+      for (int i = threadIdx.x; i < kBiasSortN; i += blockDim.x) {
+        const int p = i ^ j;
+        if (p > i) {
+          const bool up = (i & k) == 0;
+          const double x = v[i], y = v[p];
+          if ((x > y) == up) {
+            v[i] = y;
+            v[p] = x;
+          }
+        }
+      }
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    rc[cam].biasedness_cells = n_valid;
+    rc[cam].biasedness = n_valid > 0 ? v[n_valid / 2] : nan("");
+  }
+}
+
+// ComputeApproximateFOV (:609-645) for central-generic cameras: Unproject at
+// (min_x + 0.5f, 0.5f * height) and (max_x + 0.5f, 0.5f * height), angle between the normalised
+// directions times width / (max_x - min_x) (a float ratio); vertically alike. -1 where an
+// un-projection fails, for non-central cameras (as in the reference) and for OpenCV cameras (the model's
+// iterative undistortion has no device code).
+__device__ __forceinline__ bool report_unproject(const CamDev& c, const double* intr, float x, float y, d3& d) {
+  if (!in_area(c, x, y)) return false;
+  CentralEval e;
+  central_eval(c, intr, x, y, e);
+  d = rsqrt(dot3(e.u, e.u)) * e.u;
+  return true;
+}
+__global__ void report_fov_kernel(ProblemDev pb, int n_cameras, StateDev st, ReportCam* __restrict__ rc) {
+  const int cam = threadIdx.x;
+  if (cam >= n_cameras) return;
+  const CamDev& c = pb.cams[cam];
+  double hfov = -1, vfov = -1;
+  if (c.model_type == B200BA_MODEL_CENTRAL_GENERIC) {
+    const double* intr = st.intrinsics + c.intr_off;
+    d3 a, b;
+    const float min_x = c.min_x + 0.5f, max_x = c.max_x + 0.5f, y = 0.5f * c.height;
+    if (report_unproject(c, intr, min_x, y, a) && report_unproject(c, intr, max_x, y, b))
+      hfov = acos(dot3(a, b)) * static_cast<double>(c.width / (max_x - min_x));
+    const float min_y = c.min_y + 0.5f, max_y = c.max_y + 0.5f, x = 0.5f * c.width;
+    if (report_unproject(c, intr, x, min_y, a) && report_unproject(c, intr, x, max_y, b))
+      vfov = acos(dot3(a, b)) * static_cast<double>(c.height / (max_y - min_y));
+  }
+  rc[cam].hfov = hfov;
+  rc[cam].vfov = vfov;
+}
+
+void launch_calibration_report(const ProblemDev& pb, int n_cameras, const StateDev& st, const ReportDev& r,
+                               cudaStream_t s) {
+  const int64_t n = pb.n_obs;
+  if (n > 0) report_errors_kernel<<<static_cast<unsigned>((n + 127) / 128), 128, 0, s>>>(pb, n_cameras, st, r.err, r.mag);
+  report_reduce_stage1<<<dim3(kReportBlocks, n_cameras), kReportThreads, 0, s>>>(r.cam_off, r.mag, r.partial);
+  report_reduce_stage2<<<1, 32, 0, s>>>(n_cameras, r.partial, r.cams);
+  cudaMemsetAsync(r.select_hist, 0, sizeof(unsigned int) * 256 * n_cameras, s);
+  for (int pass = 0; pass < 8; ++pass) {
+    report_select_hist_kernel<<<dim3(kSelectBlocks, n_cameras), kReportThreads, 0, s>>>(pass, r.cam_off, r.mag, r.cams,
+                                                                                        r.select_hist);
+    report_select_scan_kernel<<<1, 32, 0, s>>>(pass, n_cameras, r.select_hist, r.cams);
+  }
+  cudaMemsetAsync(r.hist, 0, sizeof(int) * n_cameras * B200BA_REPORT_HIST * B200BA_REPORT_HIST, s);
+  report_hist_kernel<<<dim3(kHistBlocks, n_cameras), kReportThreads, 0, s>>>(r.cam_off, r.err, r.hist);
+  const int n_cells = n_cameras * kReportBiasCells * kReportBiasCells;
+  report_bias_kernel<<<(n_cells + 7) / 8, 256, 0, s>>>(n_cells, r.cell_off, r.cell_order, r.err, r.mag, r.Q, r.kl);
+  report_bias_median_kernel<<<n_cameras, 1024, 0, s>>>(r.kl, r.cams);
+  report_fov_kernel<<<1, 32, 0, s>>>(pb, n_cameras, st, r.cams);
+}
+int report_partial_size(int n_cameras) { return n_cameras * kReportBlocks * 3; }
+
 // Generic small-block Schur preparation for b200ba_schur_solve (block size <= 6, arbitrary
 // symmetric blocks like the reference's known-answer test): D^-1 by Gauss-Jordan with partial
 // pivoting on the symmetrised block; DinvB = D^-1 B, Dinvb = D^-1 b1.

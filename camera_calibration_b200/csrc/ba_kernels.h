@@ -51,6 +51,10 @@ void launch_project_points(const CamDev& c, const double* intr, int64_t n, const
                            cudaStream_t s);
 void launch_unproject_pixels(const CamDev& c, const double* intr, int64_t n, const double* px, double* dirs,
                              double* origins, int32_t* ok, cudaStream_t s);
+// every statistic of the calibration report from the state st (its image_tr_global cache must be current)
+void launch_calibration_report(const ProblemDev& pb, int n_cameras, const StateDev& st, const ReportDev& r,
+                               cudaStream_t s);
+int report_partial_size(int n_cameras);
 void launch_generic_block_inverse(int bs, int nb, int nd, const double* D, const double* B, const double* b1,
                                   double* DinvB, double* Dinvb, cudaStream_t s);
 void launch_symmetrize(int n, double* M, cudaStream_t s);

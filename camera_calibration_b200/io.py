@@ -438,3 +438,43 @@ def LoadColmapProblem(model: CameraModel, model_input_directory: str):
     st.feature_id_to_points_index = {k: i for i, k in enumerate(ids)}
     st.ComputeFeatureIdToPointsIndex(ds)
     return ds, st
+
+
+# ---------------------------------------------------------------------------------------
+# calibration report
+# ---------------------------------------------------------------------------------------
+REPORT_HIST_EXTENT = float(np.float32(0.2))  # kHistExtent (calibration_report.cc:740): the float 0.2f
+REPORT_MAX_ERROR = 0.5  # max_error_in_px (:777)
+
+
+def WriteReportInfoFile(path: str, cam: CameraModel, horizontal_fov: float, vertical_fov: float, imageset_count: int,
+                        num_localized_images: int, reprojection_error_count: int, reprojection_error_sum: float,
+                        reprojection_error_max: float, reprojection_error_median: float, biasedness: float,
+                        histogram_extent_in_px: float = REPORT_HIST_EXTENT,
+                        max_error_in_px: float = REPORT_MAX_ERROR) -> bool:
+    """``<base>_info.txt`` (APP/calibration_report.cc:648-710). The reference takes the error vector and
+    sorts it for the median; here the median comes in (it is computed on the device) and its line is
+    written when there is at least one error. The average is sum / count (NaN for no errors). NaN is
+    written as ``nan`` whatever its sign bit, so that the C++ writer (b200ba_pipeline.hpp) produces the
+    same bytes."""
+    count = int(reprojection_error_count)
+    lines = [f"resolution : {cam.width()} x {cam.height()}"]
+    if horizontal_fov >= 0:
+        lines.append(f"horizontal_fov : {_g(180.0 / np.pi * horizontal_fov)}")
+    if vertical_fov >= 0:
+        lines.append(f"vertical_fov : {_g(180.0 / np.pi * vertical_fov)}")
+    lines += ["", f"num_localized_imagesets : {int(num_localized_images)}", f"num_total_imagesets : {int(imageset_count)}",
+              "", f"reprojection_error_count : {count}"]
+    if count > 0:
+        lines.append(f"reprojection_error_median : {_g(reprojection_error_median)}")
+    average = float(reprojection_error_sum) / count if count > 0 else float("nan")
+    lines += [f"reprojection_error_average : {_g(average)}", f"reprojection_error_maximum : {_g(reprojection_error_max)}",
+              f"median_kl_divergence : {_g(biasedness)}", "",
+              f"reprojection_error_histogram_visualization_half_extent_in_pixels : {_g(histogram_extent_in_px)}",
+              f"maximum_error_visualization_maximum_error_in_pixels : {_g(max_error_in_px)}"]
+    try:
+        with open(path, "w") as f:
+            f.write("\n".join(lines) + "\n")
+    except OSError:
+        return False
+    return True

@@ -217,6 +217,29 @@ B200BA_API int b200ba_run_bundle_adjustment(b200ba_handle* h, const b200ba_optio
                                             int (*on_iteration)(void* user, int32_t iteration, double cost),
                                             void* user);
 
+/* ---- calibration report ---------------------------------------------------- */
+/* The numbers of CreateCalibrationReport (calibration_report.cc:83-98, per camera :713-817) for every
+ * camera: every observation re-projected with Project (start at the centre of the calibrated area, no
+ * warm start), then per camera the count / sum / max / median of |pixel - xy| over the successful
+ * projections, the 50 x 50 error histogram (half extent 0.2f px), the biasedness (median KL divergence
+ * of the per-cell error distributions from a Gaussian, 50 x 50 cells, cells with < 5 errors skipped)
+ * and the approximate field of view. */
+#define B200BA_REPORT_HIST 50
+typedef struct b200ba_camera_report {
+  int64_t reprojection_error_count;
+  double reprojection_error_sum, reprojection_error_max, reprojection_error_median; /* median NaN if count == 0 */
+  double biasedness;                 /* median KL divergence; NaN if no cell has >= 5 errors */
+  int32_t biasedness_cells;          /* cells that entered the median */
+  double horizontal_fov, vertical_fov; /* radians; -1 if not computed (non-central and OpenCV cameras) */
+  int32_t histogram[B200BA_REPORT_HIST * B200BA_REPORT_HIST]; /* [hy * 50 + hx] */
+} b200ba_camera_report;
+/* CreateCalibrationReport's numbers (calibration_report.cc) for every camera, on the state held by the handle.
+ * errors (nullable): [2*n_obs] pixel - xy in caller order, NaN where Project failed. Reads the state, writes none
+ * of it (nor last_projection, nor what b200ba_get_jacobians reads). report_ms (nullable): device time. The
+ * report's buffers are allocated on the first call. Single-rank handles only. */
+B200BA_API int b200ba_calibration_report(b200ba_handle* h, b200ba_camera_report* reports /* [n_cameras] */,
+                                         double* errors, double* report_ms);
+
 /* ---- building blocks, exposed for parity tests and profiling -------------- */
 /* One pass of JointOptimizationCostFunction::Compute<compute_jacobians>
  * (joint_optimization.cc:240-306) at the current state.

@@ -1,6 +1,6 @@
 // b200ba_pipeline.hpp -- C++ host logic of the callers either side of the hot path (SURVEY.md 8f-3 / 8f-4):
-// the outlier deletion between bundle-adjustment rounds, the metric rescaling and the pyramid resampling of the generic
-// models, over the containers of
+// the outlier deletion between bundle-adjustment rounds, the metric rescaling, the pyramid resampling of the generic
+// models and the calibration report's info files, over the containers of
 // b200ba_shim.hpp. (RunBundleAdjustment itself -- 8f-2 -- is in b200ba_shim.hpp and runs device-resident in the
 // library.) The Python mirror is camera_calibration_b200/pipeline.py.
 //
@@ -10,8 +10,12 @@
 
 #include <algorithm>
 #include <cmath>
+#include <filesystem>
+#include <fstream>
 #include <functional>
+#include <iomanip>
 #include <map>
+#include <sstream>
 
 #include "b200ba_shim.hpp"
 
@@ -388,6 +392,90 @@ inline int ResampleModelsIfNecessary(const Dataset& dataset, BAState* state, Cam
     }
   }
   return count;
+}
+
+// ---- calibration report --------------------------------------------------------------------------------------
+namespace detail {
+// std::ostream << double with setprecision(14), except that NaN is always written "nan" (glibc writes "-nan"
+// when the sign bit is set, e.g. for 0.0 / 0), so that the Python writer (io.py) produces the same bytes
+inline std::string report_number(double v) {
+  if (v != v) return "nan";
+  std::ostringstream s;
+  s << std::setprecision(14) << v;
+  return s.str();
+}
+}  // namespace detail
+
+// calibration_report.cc:648-710 -- <base>_info.txt. The reference takes the error vector and sorts it for the
+// median; here the median comes in (b200ba_calibration_report computes it) and its line is written when there is
+// at least one error. The average is sum / count (NaN without errors). Returns false if the file cannot be opened.
+inline bool WriteReportInfoFile(const std::string& path, const CameraModel& cam, double horizontal_fov, double vertical_fov,
+                                int imageset_count, int num_localized_images, int64_t reprojection_error_count,
+                                double reprojection_error_sum, double reprojection_error_max, double reprojection_error_median,
+                                double biasedness, double histogram_extent_in_px = 0.2f, double max_error_in_px = 0.5) {
+  std::ofstream stream(path, std::ios::out);
+  if (!stream) return false;
+  using detail::report_number;
+  stream << "resolution : " << cam.width() << " x " << cam.height() << "\n";
+  if (horizontal_fov >= 0) stream << "horizontal_fov : " << report_number(180.f / M_PI * horizontal_fov) << "\n";
+  if (vertical_fov >= 0) stream << "vertical_fov : " << report_number(180.f / M_PI * vertical_fov) << "\n";
+  stream << "\n";
+  stream << "num_localized_imagesets : " << num_localized_images << "\n";
+  stream << "num_total_imagesets : " << imageset_count << "\n";
+  stream << "\n";
+  stream << "reprojection_error_count : " << reprojection_error_count << "\n";
+  if (reprojection_error_count > 0) stream << "reprojection_error_median : " << report_number(reprojection_error_median) << "\n";
+  const double average = reprojection_error_count > 0 ? reprojection_error_sum / static_cast<double>(reprojection_error_count) : std::nan("");
+  stream << "reprojection_error_average : " << report_number(average) << "\n";
+  stream << "reprojection_error_maximum : " << report_number(reprojection_error_max) << "\n";
+  stream << "median_kl_divergence : " << report_number(biasedness) << "\n";
+  stream << "\n";
+  stream << "reprojection_error_histogram_visualization_half_extent_in_pixels : " << report_number(histogram_extent_in_px) << "\n";
+  stream << "maximum_error_visualization_maximum_error_in_pixels : " << report_number(max_error_in_px) << "\n";
+  return static_cast<bool>(stream);
+}
+
+// calibration_report.cc:83-98 without the visualisations: the numbers of CreateCalibrationReportForCamera
+// (:713-817) for every camera, computed in the library (b200ba_calibration_report) on the flattening that
+// OptimizeJointly uses, and written to <report_base_path>_camera<i>_info.txt. Neither argument is modified.
+// Returns the per-camera numbers; throws on a library error.
+inline std::vector<b200ba_camera_report> CreateCalibrationReport(const Dataset& dataset, const BAState& state,
+                                                                 const std::string& report_base_path) {
+  detail::Flat f;
+  // flatten() only reads; it takes mutable references because flat_intrinsics() hands out the model's storage
+  detail::flatten(const_cast<Dataset&>(dataset), const_cast<BAState*>(&state), &f);
+  b200ba_problem pb{};
+  pb.n_cameras = static_cast<int32_t>(f.cams.size());
+  pb.cameras = f.cams.data();
+  pb.n_imagesets = static_cast<int32_t>(f.used.size());
+  pb.n_points = static_cast<int32_t>(state.points.size());
+  pb.n_obs = static_cast<int64_t>(f.oi.size());
+  pb.obs_imageset = f.oi.data();
+  pb.obs_camera = f.oc.data();
+  pb.obs_point = f.op.data();
+  pb.obs_xy = f.oxy.data();
+  b200ba_handle* h = nullptr;
+  if (b200ba_create(&pb, -1, &h) != 0) throw std::runtime_error(std::string("b200ba_create: ") + b200ba_last_error(nullptr));
+  b200ba_state st{f.points.data(), f.rtg.data(), f.ctr.data(), f.intr.data(), nullptr};
+  std::vector<b200ba_camera_report> reports(f.cams.size());
+  int rc = b200ba_set_state(h, &st);
+  if (rc == 0) rc = b200ba_calibration_report(h, reports.data(), nullptr, nullptr);
+  const std::string err = rc ? b200ba_last_error(h) : "";
+  b200ba_destroy(h);
+  if (rc) throw std::runtime_error("b200ba_calibration_report: " + err);
+  int num_localized = 0;
+  for (bool used : state.image_used) num_localized += used ? 1 : 0;
+  for (size_t c = 0; c < reports.size(); ++c) {
+    const b200ba_camera_report& r = reports[c];
+    const std::string path = report_base_path + "_camera" + std::to_string(c) + "_info.txt";
+    const std::filesystem::path parent = std::filesystem::path(path).parent_path();
+    if (!parent.empty()) std::filesystem::create_directories(parent);  // the reference's mkpath (:720-721)
+    if (!WriteReportInfoFile(path, *state.intrinsics[c], r.horizontal_fov, r.vertical_fov, dataset.ImagesetCount(), num_localized,
+                             r.reprojection_error_count, r.reprojection_error_sum, r.reprojection_error_max,
+                             r.reprojection_error_median, r.biasedness))
+      throw std::runtime_error("CreateCalibrationReport: cannot write " + path);
+  }
+  return reports;
 }
 
 }  // namespace b200ba_shim

@@ -939,3 +939,24 @@ def ComputeAllReprojectionErrors(camera_index: int, dataset: Dataset, state: BAS
     r = reports[camera_index]
     return (int(r.reprojection_error_count), float(r.reprojection_error_sum), float(r.reprojection_error_max), e[ok],
             np.asarray(ctx.problem.obs_xy)[sel][ok])
+
+
+def CompareModels(model_a: CameraModel, model_b: CameraModel, with_errors: bool = False, device: int = -1):
+    """CreateFittingErrorReport(base = model_a, fitted = model_b, Identity) (APP/fitting_report.h:55-203)
+    on the device (``b200ba_compare_models``). Returns (report, direction_errors, reprojection_errors,
+    device_ms): a ``cabi.FittingReport``; with ``with_errors`` the [h, w, 3] array dir_b - dir_a (NaN where
+    model_a does not un-project the pixel, +inf where model_b does not) and the [h, w, 2] array pixel -
+    model_b.Project(dir_a) (NaN where model_a or the projection fails), else None for both."""
+    lib = cabi.load_library()
+    ca, cb = model_a.c_camera(), model_b.c_camera()
+    ia = np.ascontiguousarray(model_a.flat_intrinsics(), dtype=np.float64)
+    ib = np.ascontiguousarray(model_b.flat_intrinsics(), dtype=np.float64)
+    h, w = model_a.height(), model_a.width()
+    dir_err = np.empty((h, w, 3)) if with_errors else None
+    rep_err = np.empty((h, w, 2)) if with_errors else None
+    report = cabi.FittingReport()
+    ms = C.c_double(0)
+    _check(lib.b200ba_compare_models(device, C.byref(ca), _dp(ia), C.byref(cb), _dp(ib), C.byref(report),
+                                     None if dir_err is None else _dp(dir_err),
+                                     None if rep_err is None else _dp(rep_err), C.byref(ms)))
+    return report, dir_err, rep_err, ms.value

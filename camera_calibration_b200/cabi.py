@@ -216,6 +216,18 @@ class CameraReport(C.Structure):
     ]
 
 
+class FittingReport(C.Structure):
+    """b200ba_fitting_report: CreateFittingErrorReport's numbers for two models of one camera."""
+    _fields_ = [
+        ("reprojection_error_count", C.c_int64),
+        ("reprojection_error_sum", C.c_double),
+        ("reprojection_error_max", C.c_double),
+        ("reprojection_error_median", C.c_double),
+        ("max_error_norm", C.c_double),
+        ("max_error_component", C.c_double),
+    ]
+
+
 class FitReport(C.Structure):
     """b200ba_fit_report."""
     _fields_ = [
@@ -381,6 +393,8 @@ SYMBOLS = {
     "b200ba_unproject": (C.c_int, [C.c_int, C.POINTER(Camera), _D, C.c_int64, _D, _D, _D, _I32]),
     "b200ba_fit_directions": (C.c_int, [C.c_int, C.c_int32, C.c_int32, _D, C.c_int64, _D, _D, C.c_int32,
                                         C.POINTER(FitReport)]),
+    "b200ba_compare_models": (C.c_int, [C.c_int, C.POINTER(Camera), _D, C.POINTER(Camera), _D, C.POINTER(FittingReport),
+                                        _D, _D, _D]),
     "b200ba_nccl_unique_id": (C.c_int, [C.POINTER(C.c_uint8)]),
     "b200ba_comm_init": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint8), C.c_int, C.c_int]),
     "b200ba_get_timings": (C.c_int, [C.c_void_p, C.POINTER(Timings)]),

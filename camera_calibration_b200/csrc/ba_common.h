@@ -133,6 +133,18 @@ struct ReportDev {
   ReportCam* cams;       // [n_cameras]
 };
 
+// Model comparison (b200ba_compare_models): device buffers of one call.
+struct CompareDev {
+  double* mag;                  // [w * h] |re-projection error|, NaN where A's un-projection or B's Project fails
+  double* dir_err;              // [3 * w * h] dir_B - dir_A, or NULL
+  double* rep_err;              // [2 * w * h] pixel - B.Project(dir_A), or NULL
+  unsigned long long* dir_max;  // [2] bit patterns of max_error_norm, max_error_component
+  int64_t* range;               // [2] {0, w * h}: the one range of launch_report_statistics
+  double* partial;              // report_partial_size(1)
+  unsigned int* select_hist;    // [256]
+  ReportCam* stats;             // count / sum / max / median
+};
+
 // Up to four ranges [lo, hi) of global unknown indices held fixed (debug_fix_* of OptimizeJointly).
 struct FixedRanges {
   int n;

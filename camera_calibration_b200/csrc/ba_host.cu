@@ -2361,6 +2361,99 @@ int b200ba_fit_directions(int device, int32_t gw, int32_t gh, double* grid, int6
   return rc;
 }
 
+// CreateFittingErrorReport(base = A, fitted = B, Identity) (APP/fitting_report.h:55-203), numbers only. The
+// argument checks come first and touch no CUDA state: the reference compares central-generic models only
+// (compare_calibrations.cc:60-66) of one image size (fitting_report.h:65-66, a CHECK_EQ there).
+int b200ba_compare_models(int device, const b200ba_camera* cam_a, const double* intr_a, const b200ba_camera* cam_b,
+                          const double* intr_b, b200ba_fitting_report* report, double* direction_errors,
+                          double* reprojection_errors, double* device_ms) {
+  if (!cam_a || !intr_a || !cam_b || !intr_b || !report) {
+    g_create_error = "b200ba_compare_models: a required argument is NULL";
+    return 2;
+  }
+  if (cam_a->model_type != B200BA_MODEL_CENTRAL_GENERIC || cam_b->model_type != B200BA_MODEL_CENTRAL_GENERIC) {
+    g_create_error = "b200ba_compare_models: calibration comparison is only implemented for CentralGenericModel";
+    return 2;
+  }
+  if (cam_a->width != cam_b->width || cam_a->height != cam_b->height || cam_a->width < 1 || cam_a->height < 1) {
+    g_create_error = "b200ba_compare_models: the models differ in image size (" + std::to_string(cam_a->width) + " x " +
+                     std::to_string(cam_a->height) + " against " + std::to_string(cam_b->width) + " x " +
+                     std::to_string(cam_b->height) + ")";
+    return 2;
+  }
+  if (cam_a->grid_width < 4 || cam_a->grid_height < 4 || cam_b->grid_width < 4 || cam_b->grid_height < 4) {
+    g_create_error = "b200ba_compare_models: a grid is smaller than 4 x 4";
+    return 2;
+  }
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
+    g_create_error = "no CUDA device available (this library has no CPU fallback)";
+    return 3;
+  }
+  if (device >= 0) cudaSetDevice(device);
+  CamDev ca{}, cb{};
+  fill_camdev(*cam_a, &ca);
+  fill_camdev(*cam_b, &cb);
+  const int64_t n = static_cast<int64_t>(cam_a->width) * cam_a->height;
+  const int64_t na = intrinsics_size(*cam_a), nb = intrinsics_size(*cam_b);
+  const int64_t range[2] = {0, n};
+  double *dga = nullptr, *dgb = nullptr;
+  CompareDev d{};
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  int rc = 0;
+  auto ok = [&](cudaError_t e) {
+    if (e != cudaSuccess && rc == 0) {
+      g_create_error = cudaGetErrorString(e);
+      rc = 1;
+    }
+  };
+  ok(cudaMalloc(&dga, sizeof(double) * na));
+  ok(cudaMalloc(&dgb, sizeof(double) * nb));
+  ok(cudaMalloc(&d.mag, sizeof(double) * n));
+  if (direction_errors) ok(cudaMalloc(&d.dir_err, sizeof(double) * 3 * n));
+  if (reprojection_errors) ok(cudaMalloc(&d.rep_err, sizeof(double) * 2 * n));
+  ok(cudaMalloc(&d.dir_max, 2 * sizeof(unsigned long long)));
+  ok(cudaMalloc(&d.range, sizeof(range)));
+  ok(cudaMalloc(&d.partial, sizeof(double) * report_partial_size(1)));
+  ok(cudaMalloc(&d.select_hist, 256 * sizeof(unsigned int)));
+  ok(cudaMalloc(&d.stats, sizeof(ReportCam)));
+  ok(cudaEventCreate(&e0));
+  ok(cudaEventCreate(&e1));
+  ReportCam stats{};
+  unsigned long long dir_max[2] = {0, 0};
+  if (rc == 0) {
+    ok(cudaMemcpy(dga, intr_a, sizeof(double) * na, cudaMemcpyHostToDevice));
+    ok(cudaMemcpy(dgb, intr_b, sizeof(double) * nb, cudaMemcpyHostToDevice));
+    ok(cudaMemcpy(d.range, range, sizeof(range), cudaMemcpyHostToDevice));
+  }
+  if (rc == 0) {
+    cudaEventRecord(e0, 0);
+    launch_compare_models(ca, dga, cb, dgb, d, 0);
+    cudaEventRecord(e1, 0);
+    ok(cudaGetLastError());
+    ok(cudaMemcpy(&stats, d.stats, sizeof(ReportCam), cudaMemcpyDeviceToHost));
+    ok(cudaMemcpy(dir_max, d.dir_max, sizeof(dir_max), cudaMemcpyDeviceToHost));
+    if (direction_errors) ok(cudaMemcpy(direction_errors, d.dir_err, sizeof(double) * 3 * n, cudaMemcpyDeviceToHost));
+    if (reprojection_errors) ok(cudaMemcpy(reprojection_errors, d.rep_err, sizeof(double) * 2 * n, cudaMemcpyDeviceToHost));
+  }
+  if (rc == 0) {
+    float ms = 0;
+    ok(cudaEventElapsedTime(&ms, e0, e1));
+    if (device_ms) *device_ms = ms;
+    report->reprojection_error_count = stats.count;
+    report->reprojection_error_sum = stats.sum;
+    report->reprojection_error_max = stats.max;
+    report->reprojection_error_median = stats.median;
+    memcpy(&report->max_error_norm, &dir_max[0], sizeof(double));
+    memcpy(&report->max_error_component, &dir_max[1], sizeof(double));
+  }
+  cudaFree(dga); cudaFree(dgb); cudaFree(d.mag); cudaFree(d.dir_err); cudaFree(d.rep_err); cudaFree(d.dir_max);
+  cudaFree(d.range); cudaFree(d.partial); cudaFree(d.select_hist); cudaFree(d.stats);
+  if (e0) cudaEventDestroy(e0);
+  if (e1) cudaEventDestroy(e1);
+  return rc;
+}
+
 // ---- multi-GPU -------------------------------------------------------------------------------------
 int b200ba_nccl_unique_id(uint8_t id[B200BA_NCCL_UNIQUE_ID_BYTES]) {
   std::string err;

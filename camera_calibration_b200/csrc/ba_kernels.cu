@@ -2054,18 +2054,24 @@ __global__ void report_fov_kernel(ProblemDev pb, int n_cameras, StateDev st, Rep
   rc[cam].vfov = vfov;
 }
 
+// count / sum / max in the fixed two-stage order and the exact median of the non-NaN mag values of
+// every range [off[c], off[c + 1]), c < n_ranges (<= 32); results in rc[c].
+void launch_report_statistics(int n_ranges, const int64_t* off, const double* mag, double* partial,
+                              unsigned int* select_hist, ReportCam* rc, cudaStream_t s) {
+  report_reduce_stage1<<<dim3(kReportBlocks, n_ranges), kReportThreads, 0, s>>>(off, mag, partial);
+  report_reduce_stage2<<<1, 32, 0, s>>>(n_ranges, partial, rc);
+  cudaMemsetAsync(select_hist, 0, sizeof(unsigned int) * 256 * n_ranges, s);
+  for (int pass = 0; pass < 8; ++pass) {
+    report_select_hist_kernel<<<dim3(kSelectBlocks, n_ranges), kReportThreads, 0, s>>>(pass, off, mag, rc, select_hist);
+    report_select_scan_kernel<<<1, 32, 0, s>>>(pass, n_ranges, select_hist, rc);
+  }
+}
+
 void launch_calibration_report(const ProblemDev& pb, int n_cameras, const StateDev& st, const ReportDev& r,
                                cudaStream_t s) {
   const int64_t n = pb.n_obs;
   if (n > 0) report_errors_kernel<<<static_cast<unsigned>((n + 127) / 128), 128, 0, s>>>(pb, n_cameras, st, r.err, r.mag);
-  report_reduce_stage1<<<dim3(kReportBlocks, n_cameras), kReportThreads, 0, s>>>(r.cam_off, r.mag, r.partial);
-  report_reduce_stage2<<<1, 32, 0, s>>>(n_cameras, r.partial, r.cams);
-  cudaMemsetAsync(r.select_hist, 0, sizeof(unsigned int) * 256 * n_cameras, s);
-  for (int pass = 0; pass < 8; ++pass) {
-    report_select_hist_kernel<<<dim3(kSelectBlocks, n_cameras), kReportThreads, 0, s>>>(pass, r.cam_off, r.mag, r.cams,
-                                                                                        r.select_hist);
-    report_select_scan_kernel<<<1, 32, 0, s>>>(pass, n_cameras, r.select_hist, r.cams);
-  }
+  launch_report_statistics(n_cameras, r.cam_off, r.mag, r.partial, r.select_hist, r.cams, s);
   cudaMemsetAsync(r.hist, 0, sizeof(int) * n_cameras * B200BA_REPORT_HIST * B200BA_REPORT_HIST, s);
   report_hist_kernel<<<dim3(kHistBlocks, n_cameras), kReportThreads, 0, s>>>(r.cam_off, r.err, r.hist);
   const int n_cells = n_cameras * kReportBiasCells * kReportBiasCells;
@@ -2074,6 +2080,106 @@ void launch_calibration_report(const ProblemDev& pb, int n_cameras, const StateD
   report_fov_kernel<<<1, 32, 0, s>>>(pb, n_cameras, st, r.cams);
 }
 int report_partial_size(int n_cameras) { return n_cameras * kReportBlocks * 3; }
+
+// ------------------------------------------------------------------------------------------
+// comparison of two central-generic models (CreateFittingErrorReport, APP/fitting_report.h:83-125,
+// with parametric_r_dense = Identity and no border; called by tools/compare_calibrations.cc:68-72)
+// ------------------------------------------------------------------------------------------
+// One thread per pixel (x, y) of the image, in 2-D tiles so that a warp works on neighbouring pixels
+// and therefore on the same control points:
+//   A un-projects (x + 0.5f, y + 0.5f): outside A's calibrated area the pixel is skipped (NaN outputs);
+//   B un-projects the same pixel: error = dir_B - dir_A, or +inf where B fails;
+//   the two direction maxima over the pixels where both succeed;
+//   B.Project(dir_A) from the centre of B's calibrated area (no warm start): e = pixel - projection.
+// mag = |e| (NaN where A or Project fails) feeds launch_report_statistics.
+constexpr int kCompareTileX = 16, kCompareTileY = 8;
+__device__ __forceinline__ bool compare_unproject(const CamDev& c, const double* __restrict__ grid, double x, double y,
+                                                  d3& d) {
+  if (!in_area(c, x, y)) return false;  // CentralGenericModel::Unproject (central_generic.h:97-105)
+  CentralEval e;
+  central_eval(c, grid, x, y, e);
+  d = e.u;
+  return true;
+}
+__global__ void __launch_bounds__(kCompareTileX * kCompareTileY)
+    compare_models_kernel(CamDev ca, const double* __restrict__ ga, CamDev cb, const double* __restrict__ gb,
+                          double* __restrict__ mag, double* __restrict__ dir_err, double* __restrict__ rep_err,
+                          unsigned long long* __restrict__ dir_max) {
+  const int x = blockIdx.x * kCompareTileX + threadIdx.x;
+  const int y = blockIdx.y * kCompareTileY + threadIdx.y;
+  const bool inside = x < ca.width && y < ca.height;
+  double max_norm = 0, max_comp = 0;
+  if (inside) {
+    const int64_t p = static_cast<int64_t>(y) * ca.width + x;
+    // the reference passes x + 0.5f (a float) where Unproject takes a double
+    const double px = static_cast<double>(x + 0.5f), py = static_cast<double>(y + 0.5f);
+    const double nan_v = nan("");
+    double m = nan_v, ex = nan_v, ey = nan_v;
+    d3 da;
+    if (compare_unproject(ca, ga, px, py, da)) {
+      d3 db, err;
+      if (compare_unproject(cb, gb, px, py, db)) {
+        // __dsub_rn: the normalisation's product inside db must not be fused into this subtraction, so that
+        // dir_B - dir_A is the difference of the two rounded directions (exactly 0 when A and B agree)
+        err = mk3(__dsub_rn(db.x, da.x), __dsub_rn(db.y, da.y), __dsub_rn(db.z, da.z));
+        max_comp = fmax(fabs(err.x), fmax(fabs(err.y), fabs(err.z)));
+        // Vector3d::norm() in Eigen's order, no fused multiply-add
+        max_norm = sqrt(__dadd_rn(__dadd_rn(__dmul_rn(err.x, err.x), __dmul_rn(err.y, err.y)), __dmul_rn(err.z, err.z)));
+      } else {
+        err = mk3(INFINITY, INFINITY, INFINITY);
+      }
+      if (dir_err) {
+        dir_err[3 * p] = err.x;
+        dir_err[3 * p + 1] = err.y;
+        dir_err[3 * p + 2] = err.z;
+      }
+      // CentralGridModel::Project (central_grid.h:79-97): normalise, start at CenterOfCalibratedArea()
+      double qx = cb.center_x, qy = cb.center_y;
+      CentralEval e;
+      int ne = 0;
+      if (central_project(cb, gb, rsqrt(dot3(da, da)) * da, qx, qy, e, ne, kUnlimitedEvals) == kProjOk) {
+        ex = px - qx;
+        ey = py - qy;
+        m = report_norm(ex, ey);
+      }
+    } else if (dir_err) {
+      dir_err[3 * p] = dir_err[3 * p + 1] = dir_err[3 * p + 2] = nan_v;
+    }
+    mag[p] = m;
+    if (rep_err) {
+      rep_err[2 * p] = ex;
+      rep_err[2 * p + 1] = ey;
+    }
+  }
+  // first stage of the maxima: the block's maximum, then one atomicMax per block on the bit patterns
+  // (non-negative doubles order like their uint64 patterns; max is order-independent, so this is exact)
+  for (int o = 16; o > 0; o >>= 1) {
+    max_norm = fmax(max_norm, __shfl_xor_sync(0xffffffffu, max_norm, o));
+    max_comp = fmax(max_comp, __shfl_xor_sync(0xffffffffu, max_comp, o));
+  }
+  constexpr int kWarps = kCompareTileX * kCompareTileY / 32;
+  __shared__ double sh[2][kWarps];
+  const int t = threadIdx.y * kCompareTileX + threadIdx.x;
+  if ((t & 31) == 0) {
+    sh[0][t >> 5] = max_norm;
+    sh[1][t >> 5] = max_comp;
+  }
+  __syncthreads();
+  if (t < 2) {
+    double v = 0;
+    for (int w = 0; w < kWarps; ++w) v = fmax(v, sh[t][w]);
+    if (v > 0) atomicMax(dir_max + t, static_cast<unsigned long long>(__double_as_longlong(v)));
+  }
+}
+
+void launch_compare_models(const CamDev& a, const double* ga, const CamDev& b, const double* gb, const CompareDev& d,
+                           cudaStream_t s) {
+  cudaMemsetAsync(d.dir_max, 0, 2 * sizeof(unsigned long long), s);  // the bits of +0.0
+  const dim3 grid((a.width + kCompareTileX - 1) / kCompareTileX, (a.height + kCompareTileY - 1) / kCompareTileY);
+  compare_models_kernel<<<grid, dim3(kCompareTileX, kCompareTileY), 0, s>>>(a, ga, b, gb, d.mag, d.dir_err, d.rep_err,
+                                                                           d.dir_max);
+  launch_report_statistics(1, d.range, d.mag, d.partial, d.select_hist, d.stats, s);
+}
 
 // Generic small-block Schur preparation for b200ba_schur_solve (block size <= 6, arbitrary
 // symmetric blocks like the reference's known-answer test): D^-1 by Gauss-Jordan with partial

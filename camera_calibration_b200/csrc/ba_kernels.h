@@ -55,6 +55,10 @@ void launch_unproject_pixels(const CamDev& c, const double* intr, int64_t n, con
 void launch_calibration_report(const ProblemDev& pb, int n_cameras, const StateDev& st, const ReportDev& r,
                                cudaStream_t s);
 int report_partial_size(int n_cameras);
+// comparison of two central-generic models of the same image size (b200ba_compare_models); the grids a and b are
+// on the device
+void launch_compare_models(const CamDev& a, const double* ga, const CamDev& b, const double* gb, const CompareDev& d,
+                           cudaStream_t s);
 void launch_generic_block_inverse(int bs, int nb, int nd, const double* D, const double* B, const double* b1,
                                   double* DinvB, double* Dinvb, cudaStream_t s);
 void launch_symmetrize(int n, double* M, cudaStream_t s);

@@ -478,3 +478,29 @@ def WriteReportInfoFile(path: str, cam: CameraModel, horizontal_fov: float, vert
     except OSError:
         return False
     return True
+
+
+# ---------------------------------------------------------------------------------------
+# model comparison
+# ---------------------------------------------------------------------------------------
+def WriteFittingInfoFile(path: str, report) -> bool:
+    """``<base>_fitting_info.txt`` (APP/fitting_report.h:186-200) from a ``cabi.FittingReport``. The
+    reference sorts its error vector for the median; here the median comes in (it is computed on the
+    device) and its line is written when there is at least one error. The average is sum / count (NaN
+    for no errors). NaN is written as ``nan`` whatever its sign bit, so that the C++ writer
+    (b200ba_pipeline.hpp) produces the same bytes."""
+    count = int(report.reprojection_error_count)
+    lines = []
+    if count > 0:
+        lines.append(f"median_reprojection_error : {_g(report.reprojection_error_median)}")
+    average = float(report.reprojection_error_sum) / count if count > 0 else float("nan")
+    lines += [f"average_reprojection_error : {_g(average)}",
+              f"maximum_reprojection_error : {_g(report.reprojection_error_max)}",
+              f"error_magnitude_visualization_max_error_norm : {_g(report.max_error_norm)}",
+              f"error_direction_visualization_max_error_component : {_g(report.max_error_component)}"]
+    try:
+        with open(path, "w") as f:
+            f.write("\n".join(lines) + "\n")
+    except OSError:
+        return False
+    return True

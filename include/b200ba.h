@@ -310,6 +310,26 @@ B200BA_API int b200ba_fit_directions(int device, int32_t grid_width, int32_t gri
                           const double* grid_points, const double* directions, int32_t max_iteration_count,
                           b200ba_fit_report* report);
 
+/* ---- model comparison: CreateFittingErrorReport (APP/fitting_report.h:55-203) as the
+ * --compare_calibrations tool runs it (APP/tools/compare_calibrations.cc:39-74: base = A, fitted = B,
+ * rotation Identity, no border), numbers only. For every pixel (x, y) of the image: A un-projects
+ * (x + 0.5f, y + 0.5f); where that succeeds, B un-projects the same pixel (direction error
+ * dir_B - dir_A, +inf where B fails) and B projects A's direction (Project: start at the centre of B's
+ * calibrated area, no warm start), the re-projection error being (x + 0.5f, y + 0.5f) - projection.
+ * Both models must be central-generic, with the same width / height and grids of at least 4 x 4. */
+typedef struct b200ba_fitting_report {
+  int64_t reprojection_error_count;      /* pixels where A un-projects and B projects A's direction */
+  double reprojection_error_sum, reprojection_error_max, reprojection_error_median; /* median NaN if count == 0 */
+  double max_error_norm, max_error_component; /* over pixels where both un-projections succeed; 0 if none */
+} b200ba_fitting_report;
+/* Stand-alone (allocates, computes, frees). intr_a / intr_b: the grids [3 * grid_width * grid_height]; not
+ * modified. direction_errors (nullable): [3*w*h] row-major (y, x), NaN where A fails, +inf where B fails.
+ * reprojection_errors (nullable): [2*w*h], NaN where A or Project fails (the reference's image holds 0 there).
+ * device_ms (nullable): device time of the comparison. Returns 2 for a bad argument, 3 without a device. */
+B200BA_API int b200ba_compare_models(int device, const b200ba_camera* cam_a, const double* intr_a,
+                                     const b200ba_camera* cam_b, const double* intr_b, b200ba_fitting_report* report,
+                                     double* direction_errors, double* reprojection_errors, double* device_ms);
+
 /* ---- multi-GPU: imagesets sharded over ranks, one NCCL all-reduce per H/b build --- */
 #define B200BA_NCCL_UNIQUE_ID_BYTES 128
 B200BA_API int b200ba_nccl_unique_id(uint8_t id[B200BA_NCCL_UNIQUE_ID_BYTES]);

@@ -1,6 +1,6 @@
 // b200ba_pipeline.hpp -- C++ host logic of the callers either side of the hot path (SURVEY.md 8f-3 / 8f-4):
 // the outlier deletion between bundle-adjustment rounds, the metric rescaling, the pyramid resampling of the generic
-// models and the calibration report's info files, over the containers of
+// models, the calibration report's info files and the comparison of two calibrations, over the containers of
 // b200ba_shim.hpp. (RunBundleAdjustment itself -- 8f-2 -- is in b200ba_shim.hpp and runs device-resident in the
 // library.) The Python mirror is camera_calibration_b200/pipeline.py.
 //
@@ -10,13 +10,16 @@
 
 #include <algorithm>
 #include <cmath>
+#include <cstdlib>
 #include <filesystem>
 #include <fstream>
 #include <functional>
 #include <iomanip>
+#include <iostream>
 #include <map>
 #include <sstream>
 
+#include "b200ba_io.hpp"
 #include "b200ba_shim.hpp"
 
 namespace b200ba_shim {
@@ -476,6 +479,84 @@ inline std::vector<b200ba_camera_report> CreateCalibrationReport(const Dataset& 
       throw std::runtime_error("CreateCalibrationReport: cannot write " + path);
   }
   return reports;
+}
+
+// ---- comparison of two calibrations ----------------------------------------------------------------------------
+// fitting_report.h:186-200 -- <base>_fitting_info.txt. The reference sorts its error vector for the median; here the
+// median comes in (b200ba_compare_models computes it) and its line is written when there is at least one error. The
+// average is sum / count (NaN without errors). Returns false if the file cannot be opened.
+inline bool WriteFittingInfoFile(const std::string& path, const b200ba_fitting_report& report) {
+  std::ofstream stream(path, std::ios::out);
+  if (!stream) return false;
+  using detail::report_number;
+  const int64_t count = report.reprojection_error_count;
+  if (count > 0) stream << "median_reprojection_error : " << report_number(report.reprojection_error_median) << "\n";
+  const double average = count > 0 ? report.reprojection_error_sum / static_cast<double>(count) : std::nan("");
+  stream << "average_reprojection_error : " << report_number(average) << "\n";
+  stream << "maximum_reprojection_error : " << report_number(report.reprojection_error_max) << "\n";
+  stream << "error_magnitude_visualization_max_error_norm : " << report_number(report.max_error_norm) << "\n";
+  stream << "error_direction_visualization_max_error_component : " << report_number(report.max_error_component) << "\n";
+  return static_cast<bool>(stream);
+}
+
+// tools/compare_calibrations.cc:39-74 without the visualisations: load both models, compare them in the library
+// (b200ba_compare_models: CreateFittingErrorReport with base = A, fitted = B, rotation Identity) and write
+// <report_base_path>_fitting_info.txt. Returns EXIT_SUCCESS / EXIT_FAILURE with the reference's messages on stderr.
+// Where the reference aborts on models of different image sizes (fitting_report.h:65-66), and where the info file
+// cannot be written, this returns EXIT_FAILURE. Throws on a library error.
+inline int CompareCalibrations(const std::string& calibration_a, const std::string& calibration_b,
+                               const std::string& report_base_path) {
+  if (calibration_a.empty() || calibration_b.empty() || report_base_path.empty()) {
+    std::cerr << "For calibration comparison (--compare_calibrations), the input calibrations must be given with "
+                 "--calibration_a and --calibration_b, and the output base path with --report_base_path.\n";
+    return EXIT_FAILURE;
+  }
+  std::shared_ptr<CameraModel> model_a = LoadCameraModel(calibration_a.c_str());
+  if (!model_a) {
+    std::cerr << "Cannot load file: " << calibration_a << "\n";
+    return EXIT_FAILURE;
+  }
+  std::shared_ptr<CameraModel> model_b = LoadCameraModel(calibration_b.c_str());
+  if (!model_b) {
+    std::cerr << "Cannot load file: " << calibration_b << "\n";
+    return EXIT_FAILURE;
+  }
+  auto* a = dynamic_cast<CentralGenericModel*>(model_a.get());
+  auto* b = dynamic_cast<CentralGenericModel*>(model_b.get());
+  if (!a || !b) {
+    std::cerr << "Calibration comparison is only implemented for CentralGenericModel at the moment.\n";
+    return EXIT_FAILURE;
+  }
+  if (a->width() != b->width() || a->height() != b->height()) {
+    std::cerr << "The calibrations differ in image size (" << a->width() << " x " << a->height() << " against "
+              << b->width() << " x " << b->height() << ").\n";
+    return EXIT_FAILURE;
+  }
+  const std::filesystem::path parent = std::filesystem::path(report_base_path).parent_path();
+  if (!parent.empty()) std::filesystem::create_directories(parent);  // QFileInfo(base_path).dir().mkpath(".")
+  auto camera = [](const CentralGenericModel& m) {
+    b200ba_camera c{};
+    c.model_type = B200BA_MODEL_CENTRAL_GENERIC;
+    c.width = m.width();
+    c.height = m.height();
+    c.calibration_min_x = m.calibration_min_x();
+    c.calibration_min_y = m.calibration_min_y();
+    c.calibration_max_x = m.calibration_max_x();
+    c.calibration_max_y = m.calibration_max_y();
+    c.grid_width = m.gw;
+    c.grid_height = m.gh;
+    return c;
+  };
+  const b200ba_camera cam_a = camera(*a), cam_b = camera(*b);
+  b200ba_fitting_report report{};
+  if (b200ba_compare_models(-1, &cam_a, a->grid.data(), &cam_b, b->grid.data(), &report, nullptr, nullptr, nullptr) != 0)
+    throw std::runtime_error(std::string("b200ba_compare_models: ") + b200ba_last_error(nullptr));
+  const std::string path = report_base_path + "_fitting_info.txt";
+  if (!WriteFittingInfoFile(path, report)) {
+    std::cerr << "Cannot write file: " << path << "\n";
+    return EXIT_FAILURE;
+  }
+  return EXIT_SUCCESS;
 }
 
 }  // namespace b200ba_shim

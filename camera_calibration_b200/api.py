@@ -173,6 +173,25 @@ class BundleAdjuster:
                self._h)
         return list(reports), errors, ms.value
 
+    def report_images(self, camera: int, observation_directions: bool = True, error_maps: bool = True):
+        """The images of CreateCalibrationReportForCamera (calibration_report.cc:713-838) for one camera on the
+        device-resident state (``b200ba_report_images``). Returns a dict with the [h, w, 3] uint8 images
+        ``observation_directions`` (None if not requested; central- and non-central-generic cameras only),
+        ``error_directions`` and ``error_magnitudes`` (None if ``error_maps`` is False), the number of Voronoi
+        sites ``n_sites`` and the device time ``device_ms``. The state, last_projection and the Jacobians of the
+        last evaluation are left as they were."""
+        cam = self.problem.cameras[camera] if 0 <= camera < self.problem.n_cameras else None
+        shape = (cam.height, cam.width, 3) if cam is not None else (1, 1, 3)
+        od = np.zeros(shape, np.uint8) if observation_directions else None
+        ed = np.zeros(shape, np.uint8) if error_maps else None
+        em = np.zeros(shape, np.uint8) if error_maps else None
+        n_sites = C.c_int64(0)
+        ms = C.c_double(0)
+        _check(self.lib.b200ba_report_images(self._h, int(camera), _u8p(od), _u8p(ed), _u8p(em), C.byref(n_sites),
+                                             C.byref(ms)), self._h)
+        return {"observation_directions": od, "error_directions": ed, "error_magnitudes": em,
+                "n_sites": int(n_sites.value), "device_ms": ms.value}
+
     def timings(self) -> cabi.Timings:
         t = cabi.Timings()
         _check(self.lib.b200ba_get_timings(self._h, C.byref(t)), self._h)
@@ -185,6 +204,25 @@ class BundleAdjuster:
 
 def _dp(a):
     return a.ctypes.data_as(C.POINTER(C.c_double))
+
+
+def _u8p(a):
+    return None if a is None else a.ctypes.data_as(C.POINTER(C.c_uint8))
+
+
+def RenderVoronoi(width: int, height: int, sites_q, colors, device: int = -1):
+    """Voronoi coverage rendering on the device (``b200ba_render_voronoi``): sites_q [n, 2] integer sites in
+    quarter pixels, colors [n, 3]. Returns (image [height, width, 3] uint8, device_ms)."""
+    lib = cabi.load_library()
+    s = np.ascontiguousarray(np.asarray(sites_q, dtype=np.int32).reshape(-1, 2))
+    c = np.ascontiguousarray(np.asarray(colors, dtype=np.float32).reshape(-1, 3))
+    if len(s) != len(c):
+        raise ValueError("sites_q and colors differ in length")
+    img = np.zeros((height, width, 3), np.uint8)
+    ms = C.c_double(0)
+    _check(lib.b200ba_render_voronoi(device, int(width), int(height), len(s), s.ctypes.data_as(C.POINTER(C.c_int32)),
+                                     c.ctypes.data_as(C.POINTER(C.c_float)), _u8p(img), C.byref(ms)))
+    return img, ms.value
 
 
 def nccl_unique_id() -> bytes:
@@ -925,6 +963,15 @@ def CalibrationReports(dataset: Dataset, state: BAState, with_errors: bool = Fal
     ctx = _report_context(dataset, state)
     reports, errors, _ = ctx.adjuster.calibration_report(with_errors)
     return reports, errors, ctx
+
+
+def ReportImages(dataset: Dataset, state: BAState, camera: int):
+    """The images of CreateCalibrationReportForCamera for one camera of (dataset, state) on the device:
+    ``BundleAdjuster.report_images`` through the cached ``_Context``. The observation-direction image is None for
+    OpenCV cameras, which have no device un-projection."""
+    ctx = _report_context(dataset, state)
+    generic = ctx.problem.cameras[camera].model_type in (cabi.MODEL_CENTRAL_GENERIC, cabi.MODEL_NONCENTRAL_GENERIC)
+    return ctx.adjuster.report_images(camera, observation_directions=generic)
 
 
 def ComputeAllReprojectionErrors(camera_index: int, dataset: Dataset, state: BAState):

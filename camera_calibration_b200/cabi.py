@@ -403,6 +403,10 @@ SYMBOLS = {
     "b200ba_run_bundle_adjustment": (C.c_int, [C.c_void_p, C.POINTER(Options), C.c_int32, C.c_double, C.POINTER(BAReport),
                                               ON_ITERATION, C.c_void_p]),
     "b200ba_calibration_report": (C.c_int, [C.c_void_p, C.POINTER(CameraReport), _D, _D]),
+    "b200ba_report_images": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_uint8), C.POINTER(C.c_uint8),
+                                       C.POINTER(C.c_uint8), C.POINTER(C.c_int64), _D]),
+    "b200ba_render_voronoi": (C.c_int, [C.c_int, C.c_int32, C.c_int32, C.c_int64, _I32, C.POINTER(C.c_float),
+                                        C.POINTER(C.c_uint8), _D]),
     "b200ba_snapshot_state": (C.c_int, [C.c_void_p]),
     "b200ba_restore_state": (C.c_int, [C.c_void_p]),
     "b200ba_version": (C.c_char_p, []),

@@ -145,6 +145,24 @@ struct CompareDev {
   ReportCam* stats;             // count / sum / max / median
 };
 
+// Voronoi coverage renderer (b200ba_render_voronoi, b200ba_report_images). Sites are integer points in
+// quarter-pixel units; a site whose x is kVoronoiNoSite is ignored. The sites are binned into a uniform
+// grid of square buckets that covers the image and every site: bucket (bx, by) holds the sites with
+// x0 + bx * bs <= x < x0 + (bx + 1) * bs (alike in y), listed in index order in idx[off[b], off[b + 1]).
+constexpr int kVoronoiNoSite = INT32_MIN;
+struct VoronoiGrid {
+  int x0, y0;       // quarter-pixel origin
+  int bs;           // bucket size in quarter pixels
+  int nx, ny;       // buckets
+  int* off;         // [nx * ny + 1]
+  int* count;       // [nx * ny] scratch of the counting sort
+  int* idx;         // [n_sites]
+  int* scan_sums;   // [kVoronoiScanMax] scratch of the scan
+};
+constexpr int kVoronoiScanChunk = 4096;                                  // elements per block of the scan
+constexpr int kVoronoiScanMax = 4096;                                    // blocks of the scan
+constexpr int64_t kVoronoiMaxBuckets = int64_t(kVoronoiScanChunk) * kVoronoiScanMax - 1;
+
 // Up to four ranges [lo, hi) of global unknown indices held fixed (debug_fix_* of OptimizeJointly).
 struct FixedRanges {
   int n;

@@ -170,6 +170,12 @@ struct b200ba_handle {
   ReportDev rep{};
   double2* d_rep_stage = nullptr;  // errors in the caller's order (D2H staging)
   bool have_report = false;
+  // report images: observations grouped by (camera, integer feature pixel), allocated by the first
+  // b200ba_report_images
+  std::vector<int64_t> img_cam_groups;  // [n_cameras + 1] range of each camera's groups
+  int* d_img_group_off = nullptr;       // [n_groups + 1] into d_img_group_obs
+  uint32_t* d_img_group_obs = nullptr;  // device positions, the caller's order inside a group
+  bool have_images = false;
 
   // multi-GPU
   void* comm = nullptr;
@@ -1146,6 +1152,8 @@ void free_handle_buffers(b200ba_handle* h) {
   F(h->rep.err); F(h->rep.mag); F(h->rep.cam_off); F(h->rep.cell_off); F(h->rep.cell_order); F(h->rep.Q);
   F(h->rep.partial); F(h->rep.select_hist); F(h->rep.hist); F(h->rep.kl); F(h->rep.cams); F(h->d_rep_stage);
   h->have_report = false;
+  F(h->d_img_group_off); F(h->d_img_group_obs);
+  h->have_images = false;
   F(h->dn.Lpack); F(h->dn.tmp); F(h->dn.d_panel_off); F(h->dn.d_panel_h); F(h->d_ident_cols); F(h->d_gemv_partial);
   h->dn.S = nullptr;
   h->dense_planned_n = -1;
@@ -1216,6 +1224,76 @@ int setup_report(b200ba_handle* h) {
   h->have_report = true;
   return 0;
 }
+
+// First b200ba_report_images: groups every camera's observations by their integer feature pixel
+// ((int)x, (int)y) as CreateVoronoiDiagram de-duplicates them (calibration_report.cc:366-383), the caller's order
+// inside a group. Its de-duplication image is 4W x 4H and indexed at (ix, iy), so observations outside
+// 0 <= ix < 4W, 0 <= iy < 4H (undefined there) are left out.
+int setup_images(b200ba_handle* h) {
+  if (h->have_images) return 0;
+  const int64_t n = h->n_obs;
+  const int nc = h->n_cameras;
+  std::vector<uint32_t> pos(n);
+  for (int64_t i = 0; i < n; ++i) pos[h->perm[i]] = static_cast<uint32_t>(i);
+  std::vector<std::pair<int64_t, uint32_t>> keyed;  // (camera-major key, caller index)
+  keyed.reserve(n);
+  for (int64_t o = 0; o < n; ++o) {
+    const b200ba_camera& c = h->cams_host[h->h_obs_camera[o]];
+    const float x = h->h_obs_xy[2 * o], y = h->h_obs_xy[2 * o + 1];
+    if (!(x > -1.f && y > -1.f && x < 4.f * c.width && y < 4.f * c.height)) continue;
+    const int64_t ix = static_cast<int>(x), iy = static_cast<int>(y);
+    if (ix >= 4 * static_cast<int64_t>(c.width) || iy >= 4 * static_cast<int64_t>(c.height)) continue;
+    const int64_t key = (static_cast<int64_t>(h->h_obs_camera[o]) << 40) | (iy * 4 * c.width + ix);
+    keyed.emplace_back(key, static_cast<uint32_t>(o));
+  }
+  std::stable_sort(keyed.begin(), keyed.end(),
+                   [](const std::pair<int64_t, uint32_t>& a, const std::pair<int64_t, uint32_t>& b) { return a.first < b.first; });
+  std::vector<int> group_off;
+  std::vector<uint32_t> group_obs(keyed.size());
+  h->img_cam_groups.assign(nc + 1, 0);
+  for (size_t k = 0; k < keyed.size(); ++k) {
+    if (k == 0 || keyed[k].first != keyed[k - 1].first) {
+      group_off.push_back(static_cast<int>(k));
+      ++h->img_cam_groups[(keyed[k].first >> 40) + 1];
+    }
+    group_obs[k] = pos[keyed[k].second];
+  }
+  group_off.push_back(static_cast<int>(keyed.size()));
+  for (int c = 0; c < nc; ++c) h->img_cam_groups[c + 1] += h->img_cam_groups[c];
+  if (dev_alloc(h, &h->d_img_group_off, group_off.size()) || dev_alloc(h, &h->d_img_group_obs, group_obs.size())) return 1;
+  CUDA_TRY(h, cudaMemcpy(h->d_img_group_off, group_off.data(), group_off.size() * sizeof(int), cudaMemcpyHostToDevice));
+  if (!group_obs.empty())
+    CUDA_TRY(h, cudaMemcpy(h->d_img_group_obs, group_obs.data(), group_obs.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+  h->have_images = true;
+  return 0;
+}
+
+// Device buffers of one Voronoi rendering: the bucket grid over a quarter-pixel box that contains the image
+// and every site.
+struct VoronoiRun {
+  VoronoiGrid g{};
+  int64_t nb = 0;
+  cudaError_t alloc(int64_t n, int64_t lo_x, int64_t lo_y, int64_t hi_x, int64_t hi_y) {
+    g = voronoi_grid_geometry(lo_x, lo_y, hi_x, hi_y);
+    nb = static_cast<int64_t>(g.nx) * g.ny;
+    cudaError_t e = cudaMalloc(&g.off, sizeof(int) * (nb + 1));
+    if (e == cudaSuccess) e = cudaMalloc(&g.count, sizeof(int) * nb);
+    if (e == cudaSuccess) e = cudaMalloc(&g.idx, sizeof(int) * std::max<int64_t>(1, n));
+    if (e == cudaSuccess) e = cudaMalloc(&g.scan_sums, sizeof(int) * kVoronoiScanMax);
+    return e;
+  }
+  // sites that took part (those not marked kVoronoiNoSite); after the stream has finished
+  cudaError_t n_valid(int64_t* out) {
+    int v = 0;
+    const cudaError_t e = cudaMemcpy(&v, g.off + nb, sizeof(int), cudaMemcpyDeviceToHost);
+    *out = v;
+    return e;
+  }
+  void release() {
+    cudaFree(g.off); cudaFree(g.count); cudaFree(g.idx); cudaFree(g.scan_sums);
+    g = VoronoiGrid{};
+  }
+};
 
 }  // namespace
 
@@ -1611,6 +1689,89 @@ int b200ba_calibration_report(b200ba_handle* h, b200ba_camera_report* reports, d
     memcpy(r.histogram, hist.data() + static_cast<size_t>(c) * kBins, kBins * sizeof(int32_t));
   }
   return 0;
+}
+
+// The images of CreateCalibrationReportForCamera (calibration_report.cc:713-838) for one camera, from the report's
+// error pass: the observation directions (:723-726) and the two Voronoi error maps (:758-787).
+int b200ba_report_images(b200ba_handle* h, int32_t camera, uint8_t* observation_directions, uint8_t* error_directions,
+                         uint8_t* error_magnitudes, int64_t* n_sites, double* device_ms) {
+  if (!h) return 1;
+  if (h->comm || h->n_ranks > 1) {
+    h->error = "b200ba_report_images: the handle is joined to a communicator and holds one shard of the "
+               "observations; the report needs all of them (use a single-rank handle)";
+    return 2;
+  }
+  if (camera < 0 || camera >= h->n_cameras) {
+    h->error = "b200ba_report_images: camera index out of range";
+    return 2;
+  }
+  if (!h->have_state) {
+    h->error = "no state: call b200ba_set_state first";
+    return 2;
+  }
+  const b200ba_camera& cam = h->cams_host[camera];
+  if (observation_directions && cam.model_type != B200BA_MODEL_CENTRAL_GENERIC &&
+      cam.model_type != B200BA_MODEL_NONCENTRAL_GENERIC) {
+    h->error = "b200ba_report_images: observation directions need a device un-projection, which exists for the "
+               "central- and non-central-generic models only (pass NULL for this camera)";
+    return 2;
+  }
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  if (setup_report(h) || setup_images(h)) return 1;
+  const int nc = h->n_cameras;
+  const int64_t g0 = h->img_cam_groups[camera], n_groups = h->img_cam_groups[camera + 1] - g0;
+  const int64_t pixels = static_cast<int64_t>(cam.width) * cam.height;
+  int2* d_sites = nullptr;
+  float* d_colors = nullptr;
+  uint8_t* d_img[3] = {nullptr, nullptr, nullptr};
+  uint8_t* const out[3] = {observation_directions, error_directions, error_magnitudes};
+  VoronoiRun vr;
+  int rc = 0;
+  auto ok = [&](cudaError_t e) {
+    if (e != cudaSuccess && rc == 0) {
+      h->error = cudaGetErrorString(e);
+      rc = 1;
+    }
+  };
+  ok(cudaMalloc(&d_sites, sizeof(int2) * std::max<int64_t>(1, n_groups)));
+  ok(cudaMalloc(&d_colors, sizeof(float) * 6 * std::max<int64_t>(1, n_groups)));
+  for (int k = 0; k < 3; ++k)
+    if (out[k]) ok(cudaMalloc(&d_img[k], 3 * pixels));
+  // the sites are ((int)(4 x), (int)(4 y)) with -1 < x < 4 W, -1 < y < 4 H
+  if (rc == 0) ok(vr.alloc(n_groups, -4, -4, 16 * static_cast<int64_t>(cam.width), 16 * static_cast<int64_t>(cam.height)));
+  cudaEvent_t a = get_event(h), b = get_event(h);
+  if (rc == 0) {
+    Layout L{};
+    L.n_points = h->n_points;
+    L.n_imagesets = h->n_imagesets;
+    L.n_cameras = nc;
+    const CamDev& cd = h->pb.cams[camera];
+    cudaEventRecord(a, h->stream);
+    launch_prepare_state(h->pb, L, h->st[h->cur], h->n_control_total, h->stream);
+    launch_report_errors(h->pb, nc, h->st[h->cur], h->rep, h->stream);
+    launch_report_sites(h->pb, h->rep, n_groups, h->d_img_group_off + g0, h->d_img_group_obs, d_sites, d_colors, h->stream);
+    launch_render_voronoi(cam.width, cam.height, n_groups, d_sites, d_colors, 6, vr.g, d_img[1], d_img[2], h->stream);
+    if (d_img[0]) launch_observation_directions(cd, h->st[h->cur].intrinsics + cd.intr_off, d_img[0], h->stream);
+    cudaEventRecord(b, h->stream);
+    ok(cudaGetLastError());
+    ok(cudaStreamSynchronize(h->stream));
+  }
+  if (rc == 0) {
+    for (int k = 0; k < 3; ++k)
+      if (out[k]) ok(cudaMemcpy(out[k], d_img[k], 3 * pixels, cudaMemcpyDeviceToHost));
+    int64_t nv = 0;
+    ok(vr.n_valid(&nv));
+    if (n_sites) *n_sites = nv;
+    float ms = 0;
+    ok(cudaEventElapsedTime(&ms, a, b));
+    if (device_ms) *device_ms = ms;
+  }
+  h->event_pool.push_back(a);
+  h->event_pool.push_back(b);
+  vr.release();
+  cudaFree(d_sites); cudaFree(d_colors);
+  for (uint8_t* p : d_img) cudaFree(p);
+  return rc;
 }
 
 int32_t b200ba_degrees_of_freedom(const b200ba_handle* h, const b200ba_options* opt) {
@@ -2449,6 +2610,77 @@ int b200ba_compare_models(int device, const b200ba_camera* cam_a, const double* 
   }
   cudaFree(dga); cudaFree(dgb); cudaFree(d.mag); cudaFree(d.dir_err); cudaFree(d.rep_err); cudaFree(d.dir_max);
   cudaFree(d.range); cudaFree(d.partial); cudaFree(d.select_hist); cudaFree(d.stats);
+  if (e0) cudaEventDestroy(e0);
+  if (e1) cudaEventDestroy(e1);
+  return rc;
+}
+
+// Stand-alone Voronoi coverage rendering (allocates, computes, frees): what b200ba_report_images renders its
+// error maps with.
+int b200ba_render_voronoi(int device, int32_t width, int32_t height, int64_t n_sites, const int32_t* sites_q,
+                          const float* colors, uint8_t* image, double* device_ms) {
+  constexpr int64_t kMaxCoord = int64_t(1) << 28;
+  if (width < 1 || height < 1 || width > (1 << 24) || height > (1 << 24) || n_sites < 0 || n_sites > (int64_t(1) << 30) ||
+      !image || (n_sites > 0 && (!sites_q || !colors))) {
+    g_create_error = "b200ba_render_voronoi: bad argument";
+    return 2;
+  }
+  int64_t lo_x = 0, lo_y = 0, hi_x = 4 * static_cast<int64_t>(width), hi_y = 4 * static_cast<int64_t>(height);
+  for (int64_t i = 0; i < n_sites; ++i) {
+    const int64_t x = sites_q[2 * i], y = sites_q[2 * i + 1];
+    if (x < -kMaxCoord || x > kMaxCoord || y < -kMaxCoord || y > kMaxCoord) {
+      g_create_error = "b200ba_render_voronoi: a site lies outside [-2^28, 2^28] quarter pixels";
+      return 2;
+    }
+    lo_x = std::min(lo_x, x);
+    lo_y = std::min(lo_y, y);
+    hi_x = std::max(hi_x, x);
+    hi_y = std::max(hi_y, y);
+  }
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
+    g_create_error = "no CUDA device available (this library has no CPU fallback)";
+    return 3;
+  }
+  if (device >= 0) cudaSetDevice(device);
+  const int64_t pixels = static_cast<int64_t>(width) * height;
+  const size_t nn = static_cast<size_t>(std::max<int64_t>(1, n_sites));
+  int2* d_sites = nullptr;
+  float* d_colors = nullptr;
+  uint8_t* d_img = nullptr;
+  VoronoiRun vr;
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  int rc = 0;
+  auto ok = [&](cudaError_t e) {
+    if (e != cudaSuccess && rc == 0) {
+      g_create_error = cudaGetErrorString(e);
+      rc = 1;
+    }
+  };
+  ok(cudaMalloc(&d_sites, sizeof(int2) * nn));
+  ok(cudaMalloc(&d_colors, sizeof(float) * 3 * nn));
+  ok(cudaMalloc(&d_img, 3 * pixels));
+  if (rc == 0) ok(vr.alloc(n_sites, lo_x, lo_y, hi_x, hi_y));
+  ok(cudaEventCreate(&e0));
+  ok(cudaEventCreate(&e1));
+  if (rc == 0 && n_sites > 0) {
+    ok(cudaMemcpy(d_sites, sites_q, sizeof(int2) * n_sites, cudaMemcpyHostToDevice));
+    ok(cudaMemcpy(d_colors, colors, sizeof(float) * 3 * n_sites, cudaMemcpyHostToDevice));
+  }
+  if (rc == 0) {
+    cudaEventRecord(e0, 0);
+    launch_render_voronoi(width, height, n_sites, d_sites, d_colors, 3, vr.g, d_img, nullptr, 0);
+    cudaEventRecord(e1, 0);
+    ok(cudaGetLastError());
+    ok(cudaMemcpy(image, d_img, 3 * pixels, cudaMemcpyDeviceToHost));
+  }
+  if (rc == 0) {
+    float ms = 0;
+    ok(cudaEventElapsedTime(&ms, e0, e1));
+    if (device_ms) *device_ms = ms;
+  }
+  vr.release();
+  cudaFree(d_sites); cudaFree(d_colors); cudaFree(d_img);
   if (e0) cudaEventDestroy(e0);
   if (e1) cudaEventDestroy(e1);
   return rc;

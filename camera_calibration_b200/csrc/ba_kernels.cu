@@ -2069,8 +2069,7 @@ void launch_report_statistics(int n_ranges, const int64_t* off, const double* ma
 
 void launch_calibration_report(const ProblemDev& pb, int n_cameras, const StateDev& st, const ReportDev& r,
                                cudaStream_t s) {
-  const int64_t n = pb.n_obs;
-  if (n > 0) report_errors_kernel<<<static_cast<unsigned>((n + 127) / 128), 128, 0, s>>>(pb, n_cameras, st, r.err, r.mag);
+  launch_report_errors(pb, n_cameras, st, r, s);
   launch_report_statistics(n_cameras, r.cam_off, r.mag, r.partial, r.select_hist, r.cams, s);
   cudaMemsetAsync(r.hist, 0, sizeof(int) * n_cameras * B200BA_REPORT_HIST * B200BA_REPORT_HIST, s);
   report_hist_kernel<<<dim3(kHistBlocks, n_cameras), kReportThreads, 0, s>>>(r.cam_off, r.err, r.hist);
@@ -2080,6 +2079,10 @@ void launch_calibration_report(const ProblemDev& pb, int n_cameras, const StateD
   report_fov_kernel<<<1, 32, 0, s>>>(pb, n_cameras, st, r.cams);
 }
 int report_partial_size(int n_cameras) { return n_cameras * kReportBlocks * 3; }
+void launch_report_errors(const ProblemDev& pb, int n_cameras, const StateDev& st, const ReportDev& r, cudaStream_t s) {
+  const int64_t n = pb.n_obs;
+  if (n > 0) report_errors_kernel<<<static_cast<unsigned>((n + 127) / 128), 128, 0, s>>>(pb, n_cameras, st, r.err, r.mag);
+}
 
 // ------------------------------------------------------------------------------------------
 // comparison of two central-generic models (CreateFittingErrorReport, APP/fitting_report.h:83-125,
@@ -2179,6 +2182,463 @@ void launch_compare_models(const CamDev& a, const double* ga, const CamDev& b, c
   compare_models_kernel<<<grid, dim3(kCompareTileX, kCompareTileY), 0, s>>>(a, ga, b, gb, d.mag, d.dir_err, d.rep_err,
                                                                            d.dir_max);
   launch_report_statistics(1, d.range, d.mag, d.partial, d.select_hist, d.stats, s);
+}
+
+// ------------------------------------------------------------------------------------------
+// report images (CreateCalibrationReportForCamera, APP/calibration_report.cc:713-838)
+// ------------------------------------------------------------------------------------------
+// Error maps (:354-603): every feature site owns its Voronoi cell; a pixel's colour is the sum over the
+// cells of area(pixel n cell) * colour(cell), + 0.5, clamped to [0, 255.99] and truncated. The reference
+// triangulates each cell with Boost.Polygon and rasterises the triangle fan on the CPU; here every pixel
+// gathers the cells that can reach it and computes the exact partition:
+//   1. counting sort of the sites into a uniform bucket grid (buckets listed in index order);
+//   2. per 8 x 8 tile: the exact nearest site s0 of the tile centre (block-wide ring search), so that every
+//      point of the tile is within U = |c - s0| + half diagonal of some site: only the sites within U of
+//      the tile rectangle can own part of it, and they are read row of buckets by row of buckets (one
+//      contiguous range of idx per row), the same sequence for every thread of the block (broadcast loads);
+//   3. per pixel: the nearest site of its centre and of its four corners (integer squared distances in
+//      quarter pixels, first site wins a tie). Cells are convex, so if the four corners share their nearest
+//      site the pixel lies in that cell (the fast path). Otherwise the pixel's candidates are the sites whose
+//      distance to the pixel square is at most the centre's nearest distance + sqrt(2)/2 px, and the square
+//      is clipped, in double, by the bisector half-planes of every candidate pair; area * colour is summed
+//      in the fixed candidate order.
+// No atomics touch the images, so two calls give identical bytes.
+constexpr int kVorTile = 8;
+constexpr int kVorThreads = kVorTile * kVorTile;
+constexpr int kVorMaxCand = 24;  // candidates held per slow pixel; beyond that the pixel re-reads the buckets
+constexpr int kVorMaxPoly = 32;  // vertices of a clipped square (4 + one per cutting half-plane)
+
+VoronoiGrid voronoi_grid_geometry(int64_t lo_x, int64_t lo_y, int64_t hi_x, int64_t hi_y) {
+  VoronoiGrid g{};
+  int64_t bs = 32;  // 8 pixels
+  while (((hi_x - lo_x) / bs + 1) * ((hi_y - lo_y) / bs + 1) > kVoronoiMaxBuckets) bs *= 2;
+  g.x0 = static_cast<int>(lo_x);
+  g.y0 = static_cast<int>(lo_y);
+  g.bs = static_cast<int>(bs);
+  g.nx = static_cast<int>((hi_x - lo_x) / bs + 1);
+  g.ny = static_cast<int>((hi_y - lo_y) / bs + 1);
+  return g;
+}
+
+__device__ __forceinline__ int vor_bucket(const VoronoiGrid& g, int2 p) {
+  return ((p.y - g.y0) / g.bs) * g.nx + (p.x - g.x0) / g.bs;
+}
+__global__ void vor_count_kernel(int64_t n, const int2* __restrict__ sites, VoronoiGrid g) {
+  const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (i >= n || sites[i].x == kVoronoiNoSite) return;
+  atomicAdd(&g.count[vor_bucket(g, sites[i])], 1);
+}
+__global__ void vor_scatter_kernel(int64_t n, const int2* __restrict__ sites, VoronoiGrid g) {
+  const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (i >= n || sites[i].x == kVoronoiNoSite) return;
+  const int b = vor_bucket(g, sites[i]);
+  g.idx[g.off[b] + atomicAdd(&g.count[b], 1)] = static_cast<int>(i);
+}
+// the scatter's order inside a bucket depends on the atomics: sort every bucket by site index
+__global__ void vor_sort_buckets_kernel(VoronoiGrid g) {
+  const int64_t b = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (b >= static_cast<int64_t>(g.nx) * g.ny) return;
+  int* v = g.idx + g.off[b];
+  const int m = g.off[b + 1] - g.off[b];
+  for (int i = 1; i < m; ++i) {
+    const int x = v[i];
+    int j = i - 1;
+    while (j >= 0 && v[j] > x) {
+      v[j + 1] = v[j];
+      --j;
+    }
+    v[j + 1] = x;
+  }
+}
+
+// exclusive scan of the bucket counts (1024 threads, 4 consecutive elements each per block)
+constexpr int kScanThreads = kVoronoiScanChunk / 4;
+__device__ __forceinline__ int vor_block_scan(int v, int& total) {
+  __shared__ int warp_sum[32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int x = v;
+  for (int o = 1; o < 32; o <<= 1) {
+    const int y = __shfl_up_sync(0xffffffffu, x, o);
+    if (lane >= o) x += y;
+  }
+  if (lane == 31) warp_sum[warp] = x;
+  __syncthreads();
+  if (warp == 0) {
+    int s = warp_sum[lane];
+    for (int o = 1; o < 32; o <<= 1) {
+      const int y = __shfl_up_sync(0xffffffffu, s, o);
+      if (lane >= o) s += y;
+    }
+    warp_sum[lane] = s;
+  }
+  __syncthreads();
+  const int excl = x - v + (warp > 0 ? warp_sum[warp - 1] : 0);
+  total = warp_sum[31];
+  __syncthreads();
+  return excl;
+}
+__device__ __forceinline__ void vor_scan_chunk(int64_t n, const int* in, int* out, int base_add, int& total) {
+  int v[4], s = 0;
+  const int64_t base = static_cast<int64_t>(threadIdx.x) * 4;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    v[k] = base + k < n ? in[base + k] : 0;
+    s += v[k];
+  }
+  int run = vor_block_scan(s, total) + base_add;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    if (base + k < n) out[base + k] = run;
+    run += v[k];
+  }
+}
+__global__ void __launch_bounds__(kScanThreads) vor_scan_blocks_kernel(int64_t n, const int* __restrict__ in, int* out,
+                                                                       int* __restrict__ sums) {
+  const int64_t b0 = static_cast<int64_t>(blockIdx.x) * kVoronoiScanChunk;
+  int total;
+  const int64_t m = n - b0 < kVoronoiScanChunk ? n - b0 : kVoronoiScanChunk;
+  vor_scan_chunk(m, in + b0, out + b0, 0, total);
+  if (threadIdx.x == 0) sums[blockIdx.x] = total;
+}
+__global__ void __launch_bounds__(kScanThreads) vor_scan_sums_kernel(int n_blocks, int* sums, int* total_out) {
+  int total;
+  vor_scan_chunk(n_blocks, sums, sums, 0, total);
+  if (threadIdx.x == 0) *total_out = total;
+}
+__global__ void vor_scan_add_kernel(int64_t n, int* out, const int* __restrict__ sums) {
+  const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (i < n) out[i] += sums[i / kVoronoiScanChunk];
+}
+
+__device__ __forceinline__ long long vor_d2(int ax, int ay, int bx, int by) {
+  const long long dx = ax - bx, dy = ay - by;
+  return dx * dx + dy * dy;
+}
+// squared distance from (x, y) to the box [x0, x1] x [y0, y1]
+__device__ __forceinline__ long long vor_box_d2(int x, int y, int x0, int y0, int x1, int y1) {
+  const long long dx = max(max(x0 - x, x - x1), 0), dy = max(max(y0 - y, y - y1), 0);
+  return dx * dx + dy * dy;
+}
+__device__ __forceinline__ long long vor_block_min(long long v) {
+  __shared__ long long sh[kVorThreads / 32];
+  for (int o = 16; o > 0; o >>= 1) v = min(v, __shfl_xor_sync(0xffffffffu, v, o));
+  const int t = threadIdx.y * kVorTile + threadIdx.x;
+  if ((t & 31) == 0) sh[t >> 5] = v;
+  __syncthreads();
+  long long r = sh[0];
+  for (int k = 1; k < kVorThreads / 32; ++k) r = min(r, sh[k]);
+  __syncthreads();
+  return r;
+}
+// cell k of the Chebyshev ring r around a bucket: top row, bottom row, left and right columns
+__device__ __forceinline__ void vor_ring_cell(int r, int k, int& dx, int& dy) {
+  if (k < 2 * r + 1) {
+    dx = -r + k;
+    dy = -r;
+  } else if (k < 4 * r + 2) {
+    dx = -r + (k - (2 * r + 1));
+    dy = r;
+  } else if (k < 6 * r + 1) {
+    dx = -r;
+    dy = -r + 1 + (k - (4 * r + 2));
+  } else {
+    dx = r;
+    dy = -r + 1 + (k - (6 * r + 1));
+  }
+}
+// keep the part of the convex polygon (x, y)[n] where a X + b Y <= c (Sutherland-Hodgman); writes (ox, oy)
+__device__ __forceinline__ int vor_clip(const double* x, const double* y, int n, double a, double b, double c, double* ox,
+                                        double* oy) {
+  int m = 0;
+  for (int k = 0; k < n; ++k) {
+    const int k1 = k + 1 == n ? 0 : k + 1;
+    const double f0 = a * x[k] + b * y[k] - c, f1 = a * x[k1] + b * y[k1] - c;
+    if (f0 <= 0 && m < kVorMaxPoly) {
+      ox[m] = x[k];
+      oy[m] = y[k];
+      ++m;
+    }
+    if (((f0 < 0 && f1 > 0) || (f0 > 0 && f1 < 0)) && m < kVorMaxPoly) {
+      const double t = f0 / (f0 - f1);
+      ox[m] = x[k] + t * (x[k1] - x[k]);
+      oy[m] = y[k] + t * (y[k1] - y[k]);
+      ++m;
+    }
+  }
+  return m;
+}
+
+// The tile's candidate sites in the fixed order (rows of buckets, index order inside a row): f(site index, site)
+// for every site whose squared distance to the tile rectangle is <= U2.
+struct VorTile {
+  int X0, Y0, X1, Y1;  // quarter-pixel rectangle of the tile (clipped to the image)
+  double U2;
+  int bx0, bx1, by0, by1;
+};
+template <class F>
+__device__ __forceinline__ void vor_for_tile_sites(const VoronoiGrid& g, const VorTile& T, const int2* __restrict__ sites,
+                                                   F f) {
+  for (int by = T.by0; by <= T.by1; ++by) {
+    const int row = by * g.nx;
+    const int a = __ldg(g.off + row + T.bx0), b = __ldg(g.off + row + T.bx1 + 1);
+    for (int j = a; j < b; ++j) {
+      const int i = __ldg(g.idx + j);
+      const int2 s = __ldg(sites + i);
+      if (static_cast<double>(vor_box_d2(s.x, s.y, T.X0, T.Y0, T.X1, T.Y1)) > T.U2) continue;
+      f(i, s);
+    }
+  }
+}
+
+// area of (cell of site i) n (pixel square), in pixels: the square [0, 4]^2 in quarter pixels relative to the
+// pixel corner (qx, qy), clipped by the bisector of i and every other candidate j (enumerated by for_each_j)
+template <class ForEachJ>
+__device__ __forceinline__ double vor_cell_area(int i, int2 si, int qx, int qy, ForEachJ for_each_j) {
+  double px[kVorMaxPoly], py[kVorMaxPoly], tx[kVorMaxPoly], ty[kVorMaxPoly];
+  px[0] = 0; py[0] = 0; px[1] = 4; py[1] = 0; px[2] = 4; py[2] = 4; px[3] = 0; py[3] = 4;
+  int n = 4;
+  const long long rix = si.x - qx, riy = si.y - qy;
+  for_each_j([&](int j, int2 sj) {
+    if (j == i || n == 0) return;
+    const long long rjx = sj.x - qx, rjy = sj.y - qy;
+    if (rjx == rix && rjy == riy) {  // a repeated position: the lower index owns it
+      if (j < i) n = 0;
+      return;
+    }
+    // |q - r_i|^2 <= |q - r_j|^2  <=>  2 (r_j - r_i) . q <= |r_j|^2 - |r_i|^2
+    const double c = static_cast<double>((rjx * rjx + rjy * rjy) - (rix * rix + riy * riy));
+    n = vor_clip(px, py, n, 2.0 * static_cast<double>(rjx - rix), 2.0 * static_cast<double>(rjy - riy), c, tx, ty);
+    for (int k = 0; k < n; ++k) {
+      px[k] = tx[k];
+      py[k] = ty[k];
+    }
+  });
+  double area2 = 0;
+  for (int k = 0; k < n; ++k) {
+    const int k1 = k + 1 == n ? 0 : k + 1;
+    area2 += px[k] * py[k1] - px[k1] * py[k];
+  }
+  return fabs(area2) * (0.5 / 16.0);
+}
+
+template <int NCH>
+__global__ void __launch_bounds__(kVorThreads)
+    voronoi_render_kernel(int w, int h, const int2* __restrict__ sites, const float* __restrict__ colors, VoronoiGrid g,
+                          uint8_t* __restrict__ img0, uint8_t* __restrict__ img1) {
+  const int tid = threadIdx.y * kVorTile + threadIdx.x;
+  const int x = blockIdx.x * kVorTile + threadIdx.x, y = blockIdx.y * kVorTile + threadIdx.y;
+  const bool inside = x < w && y < h;
+  double acc[NCH];
+#pragma unroll
+  for (int k = 0; k < NCH; ++k) acc[k] = 0;
+  const int n_sites = __ldg(g.off + static_cast<int64_t>(g.nx) * g.ny);
+  if (n_sites > 0) {
+    VorTile T;
+    T.X0 = 4 * blockIdx.x * kVorTile;
+    T.Y0 = 4 * blockIdx.y * kVorTile;
+    T.X1 = 4 * min(static_cast<int>(blockIdx.x + 1) * kVorTile, w);
+    T.Y1 = 4 * min(static_cast<int>(blockIdx.y + 1) * kVorTile, h);
+    // 1. exact nearest site of the tile centre: rings of buckets until the ring is farther than the best
+    const int cx = (T.X0 + T.X1) / 2, cy = (T.Y0 + T.Y1) / 2;
+    const int cbx = min(g.nx - 1, (cx - g.x0) / g.bs), cby = min(g.ny - 1, (cy - g.y0) / g.bs);
+    long long best = LLONG_MAX;
+    for (int r = 0; r <= max(g.nx, g.ny); ++r) {
+      if (r > 1 && best != LLONG_MAX) {
+        const long long lb = static_cast<long long>(r - 1) * g.bs;
+        if (lb * lb > best) break;
+      }
+      long long local = LLONG_MAX;
+      const int cells = r == 0 ? 1 : 8 * r;
+      for (int k = tid; k < cells; k += kVorThreads) {
+        int dx = 0, dy = 0;
+        if (r > 0) vor_ring_cell(r, k, dx, dy);
+        const int bx = cbx + dx, by = cby + dy;
+        if (bx < 0 || by < 0 || bx >= g.nx || by >= g.ny) continue;
+        const int b = by * g.nx + bx;
+        for (int j = __ldg(g.off + b); j < __ldg(g.off + b + 1); ++j) {
+          const int2 s = __ldg(sites + __ldg(g.idx + j));
+          local = min(local, vor_d2(s.x, s.y, cx, cy));
+        }
+      }
+      best = min(best, vor_block_min(local));
+    }
+    // 2. every point of the tile is within U of s0
+    const double U = sqrt(static_cast<double>(best)) +
+                     0.5 * sqrt(static_cast<double>(T.X1 - T.X0) * (T.X1 - T.X0) + static_cast<double>(T.Y1 - T.Y0) * (T.Y1 - T.Y0));
+    T.U2 = U * U * (1 + 1e-12) + 1e-6;
+    T.bx0 = max(0, static_cast<int>(floor((T.X0 - U - g.x0) / g.bs)));
+    T.bx1 = min(g.nx - 1, static_cast<int>(floor((T.X1 + U - g.x0) / g.bs)));
+    T.by0 = max(0, static_cast<int>(floor((T.Y0 - U - g.y0) / g.bs)));
+    T.by1 = min(g.ny - 1, static_cast<int>(floor((T.Y1 + U - g.y0) / g.bs)));
+    // 3. nearest site of the pixel centre and of its four corners
+    const int qx = 4 * x, qy = 4 * y;
+    long long dc = LLONG_MAX, dk[4] = {LLONG_MAX, LLONG_MAX, LLONG_MAX, LLONG_MAX};
+    int ik[4] = {-1, -1, -1, -1};
+    vor_for_tile_sites(g, T, sites, [&](int i, int2 s) {
+      dc = min(dc, vor_d2(s.x, s.y, qx + 2, qy + 2));
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const long long d = vor_d2(s.x, s.y, qx + 4 * (k & 1), qy + 4 * (k >> 1));
+        if (d < dk[k]) {
+          dk[k] = d;
+          ik[k] = i;
+        }
+      }
+    });
+    const bool slow = inside && !(ik[0] == ik[1] && ik[0] == ik[2] && ik[0] == ik[3]);
+    if (inside && !slow) {
+#pragma unroll
+      for (int k = 0; k < NCH; ++k) acc[k] = __ldg(colors + static_cast<int64_t>(ik[0]) * NCH + k);
+    }
+    if (__syncthreads_or(slow)) {
+      // 4. the pixel's candidates: distance to the square <= centre's nearest distance + sqrt(2)/2 px
+      const double bound = sqrt(static_cast<double>(dc)) + 2.0 * sqrt(2.0);
+      const double bound2 = bound * bound * (1 + 1e-12) + 1e-6;
+      int cand[kVorMaxCand];
+      int nc = 0;
+      bool overflow = false;
+      vor_for_tile_sites(g, T, sites, [&](int i, int2 s) {
+        if (!slow || static_cast<double>(vor_box_d2(s.x, s.y, qx, qy, qx + 4, qy + 4)) > bound2) return;
+        if (nc < kVorMaxCand)
+          cand[nc++] = i;
+        else
+          overflow = true;
+      });
+      if (slow) {
+        auto add = [&](int i, double area) {
+          if (area <= 0) return;
+#pragma unroll
+          for (int k = 0; k < NCH; ++k) acc[k] += area * static_cast<double>(__ldg(colors + static_cast<int64_t>(i) * NCH + k));
+        };
+        if (!overflow) {
+          for (int a = 0; a < nc; ++a) {
+            const int i = cand[a];
+            add(i, vor_cell_area(i, __ldg(sites + i), qx, qy, [&](auto f) {
+                  for (int b = 0; b < nc; ++b) f(cand[b], __ldg(sites + cand[b]));
+                }));
+          }
+        } else {
+          auto each = [&](auto f) {
+            vor_for_tile_sites(g, T, sites, [&](int j, int2 s) {
+              if (static_cast<double>(vor_box_d2(s.x, s.y, qx, qy, qx + 4, qy + 4)) <= bound2) f(j, s);
+            });
+          };
+          each([&](int i, int2 s) { add(i, vor_cell_area(i, s, qx, qy, each)); });
+        }
+      }
+    }
+  }
+  if (!inside) return;
+  const int64_t p = 3 * (static_cast<int64_t>(y) * w + x);
+  uint8_t* imgs[2] = {img0, img1};
+#pragma unroll
+  for (int m = 0; m < NCH / 3; ++m) {
+    if (!imgs[m]) continue;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      const double v = fmin(fmax(acc[3 * m + k] + 0.5, 0.0), static_cast<double>(255.99f));
+      imgs[m][p + k] = static_cast<uint8_t>(static_cast<int>(v));
+    }
+  }
+}
+
+void launch_render_voronoi(int w, int h, int64_t n, const int2* sites, const float* colors, int nch, const VoronoiGrid& g,
+                           uint8_t* img0, uint8_t* img1, cudaStream_t s) {
+  const int64_t nb = static_cast<int64_t>(g.nx) * g.ny;
+  cudaMemsetAsync(g.count, 0, sizeof(int) * nb, s);
+  if (n > 0) vor_count_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(n, sites, g);
+  const int n_blocks = static_cast<int>((nb + kVoronoiScanChunk - 1) / kVoronoiScanChunk);
+  vor_scan_blocks_kernel<<<n_blocks, kScanThreads, 0, s>>>(nb, g.count, g.off, g.scan_sums);
+  vor_scan_sums_kernel<<<1, kScanThreads, 0, s>>>(n_blocks, g.scan_sums, g.off + nb);
+  vor_scan_add_kernel<<<static_cast<unsigned>((nb + 255) / 256), 256, 0, s>>>(nb, g.off, g.scan_sums);
+  cudaMemsetAsync(g.count, 0, sizeof(int) * nb, s);
+  if (n > 0) vor_scatter_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(n, sites, g);
+  vor_sort_buckets_kernel<<<static_cast<unsigned>((nb + 255) / 256), 256, 0, s>>>(g);
+  const dim3 grid((w + kVorTile - 1) / kVorTile, (h + kVorTile - 1) / kVorTile);
+  if (nch == 6)
+    voronoi_render_kernel<6><<<grid, dim3(kVorTile, kVorTile), 0, s>>>(w, h, sites, colors, g, img0, img1);
+  else
+    voronoi_render_kernel<3><<<grid, dim3(kVorTile, kVorTile), 0, s>>>(w, h, sites, colors, g, img0, nullptr);
+}
+
+// CreateVoronoiDiagram (:362-384) and the colour computers (:547-558, :576-586) for one group of observations
+// sharing the integer feature pixel ((int)x, (int)y): the first observation (caller's order) whose projection
+// succeeded gives the site ((int)(4 x), (int)(4 y)) and, from its error e cast to float,
+//   direction: theta = (double)atan2f(e.y, e.x); (127 + 127 sin theta, 127 + 127 cos theta, 127), in double
+//   magnitude: f = min(1, (double)|e|_float / 0.5); (255.99f * f, 255.99f * (1 - f), 0), in double
+// each rounded to float; no fused multiply-add anywhere.
+__global__ void report_sites_kernel(ProblemDev pb, const double2* __restrict__ err, const double* __restrict__ mag,
+                                    int64_t n_groups, const int* __restrict__ group_off,
+                                    const uint32_t* __restrict__ group_obs, int2* __restrict__ sites,
+                                    float* __restrict__ colors) {
+  const int64_t g = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (g >= n_groups) return;
+  int2 site = make_int2(kVoronoiNoSite, 0);
+  float c[6] = {0, 0, 0, 0, 0, 0};
+  for (int m = group_off[g]; m < group_off[g + 1]; ++m) {
+    const uint32_t o = group_obs[m];
+    if (isnan(mag[o])) continue;
+    const float2 xy = pb.obs_xy[o];
+    site = make_int2(__float2int_rz(4.f * xy.x), __float2int_rz(4.f * xy.y));
+    const double2 e = err[o];
+    const float ex = static_cast<float>(e.x), ey = static_cast<float>(e.y);
+    const double theta = static_cast<double>(atan2f(ey, ex));
+    c[0] = static_cast<float>(__dadd_rn(127.0, __dmul_rn(127.0, sin(theta))));
+    c[1] = static_cast<float>(__dadd_rn(127.0, __dmul_rn(127.0, cos(theta))));
+    c[2] = 127.f;
+    const float norm = sqrtf(__fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey)));
+    const double f = fmin(1.0, static_cast<double>(norm) / 0.5);
+    c[3] = static_cast<float>(__dmul_rn(static_cast<double>(255.99f), f));
+    c[4] = static_cast<float>(__dmul_rn(static_cast<double>(255.99f), __dsub_rn(1.0, f)));
+    c[5] = 0.f;
+    break;
+  }
+  sites[g] = site;
+#pragma unroll
+  for (int k = 0; k < 6; ++k) colors[6 * g + k] = c[k];
+}
+void launch_report_sites(const ProblemDev& pb, const ReportDev& r, int64_t n_groups, const int* group_off,
+                         const uint32_t* group_obs, int2* sites, float* colors, cudaStream_t s) {
+  if (n_groups == 0) return;
+  report_sites_kernel<<<static_cast<unsigned>((n_groups + 127) / 128), 128, 0, s>>>(pb, r.err, r.mag, n_groups, group_off,
+                                                                                     group_obs, sites, colors);
+}
+
+// VisualizeModelDirections (:1165-1190) with CreateObservationDirectionsImage (util.cc:190-229): the direction of
+// (x + 0.5f, y + 0.5f) (the line direction for non-central models), black where the un-projection fails; the colour
+// ((70 * 255.99f) / 2.f) * (d + 1) (x, y) and ((270 * 255.99f) / 2.f) * (d + 1) (z) is a double that the reference
+// converts to u8 as x86-64 does: truncation to int32, then the low byte (hence the stripes).
+constexpr int kDirTileX = 16, kDirTileY = 8;
+__global__ void __launch_bounds__(kDirTileX * kDirTileY)
+    observation_directions_kernel(CamDev c, const double* __restrict__ intr, uint8_t* __restrict__ img) {
+  const int x = blockIdx.x * kDirTileX + threadIdx.x, y = blockIdx.y * kDirTileY + threadIdx.y;
+  if (x >= c.width || y >= c.height) return;
+  const double px = static_cast<double>(x + 0.5f), py = static_cast<double>(y + 0.5f);
+  uint8_t out[3] = {0, 0, 0};
+  if (in_area(c, px, py)) {
+    d3 d;
+    if (c.model_type == B200BA_MODEL_CENTRAL_GENERIC) {
+      CentralEval e;
+      central_eval(c, intr, px, py, e);
+      d = e.u;
+    } else {
+      NoncentralEval e;
+      noncentral_eval(c, intr, intr + 3 * static_cast<int64_t>(c.gw) * c.gh, px, py, e);
+      d = e.u;
+    }
+    const double kxy = static_cast<double>((70 * 255.99f) / 2.f), kz = static_cast<double>((270 * 255.99f) / 2.f);
+    out[0] = static_cast<uint8_t>(report_trunc(__dmul_rn(kxy, __dadd_rn(d.x, 1.0))));
+    out[1] = static_cast<uint8_t>(report_trunc(__dmul_rn(kxy, __dadd_rn(d.y, 1.0))));
+    out[2] = static_cast<uint8_t>(report_trunc(__dmul_rn(kz, __dadd_rn(d.z, 1.0))));
+  }
+  const int64_t p = 3 * (static_cast<int64_t>(y) * c.width + x);
+  img[p] = out[0];
+  img[p + 1] = out[1];
+  img[p + 2] = out[2];
+}
+void launch_observation_directions(const CamDev& c, const double* intr, uint8_t* img, cudaStream_t s) {
+  const dim3 grid((c.width + kDirTileX - 1) / kDirTileX, (c.height + kDirTileY - 1) / kDirTileY);
+  observation_directions_kernel<<<grid, dim3(kDirTileX, kDirTileY), 0, s>>>(c, intr, img);
 }
 
 // Generic small-block Schur preparation for b200ba_schur_solve (block size <= 6, arbitrary

@@ -59,6 +59,22 @@ int report_partial_size(int n_cameras);
 // on the device
 void launch_compare_models(const CamDev& a, const double* ga, const CamDev& b, const double* gb, const CompareDev& d,
                            cudaStream_t s);
+// re-projection errors of every observation into r.err / r.mag (the first kernel of launch_calibration_report)
+void launch_report_errors(const ProblemDev& pb, int n_cameras, const StateDev& st, const ReportDev& r, cudaStream_t s);
+// Voronoi coverage rendering of n sites (quarter-pixel int2, kVoronoiNoSite.x = skipped) with nch = 3 or 6 float
+// colours per site into the RGB images img0 (channels 0-2) and img1 (channels 3-5, nch == 6), both [h * w * 3],
+// nullable. g's geometry must be set (voronoi_grid_geometry) and its buffers allocated.
+void launch_render_voronoi(int w, int h, int64_t n, const int2* sites, const float* colors, int nch, const VoronoiGrid& g,
+                           uint8_t* img0, uint8_t* img1, cudaStream_t s);
+// bucket grid over the quarter-pixel box [lo_x, hi_x] x [lo_y, hi_y] (which must contain the image)
+VoronoiGrid voronoi_grid_geometry(int64_t lo_x, int64_t lo_y, int64_t hi_x, int64_t hi_y);
+// sites and colours of the error maps of one camera: group_off [n_groups + 1] lists, per integer feature pixel, the
+// device positions group_obs of its observations in the caller's order; the first one whose projection succeeded
+// gives the group's site and its direction (colors[6g..6g+2]) and magnitude (colors[6g+3..6g+5]) colours
+void launch_report_sites(const ProblemDev& pb, const ReportDev& r, int64_t n_groups, const int* group_off,
+                         const uint32_t* group_obs, int2* sites, float* colors, cudaStream_t s);
+// observation-direction image of one camera (VisualizeModelDirections): central- or non-central-generic
+void launch_observation_directions(const CamDev& c, const double* intr, uint8_t* img, cudaStream_t s);
 void launch_generic_block_inverse(int bs, int nb, int nd, const double* D, const double* B, const double* b1,
                                   double* DinvB, double* Dinvb, cudaStream_t s);
 void launch_symmetrize(int n, double* M, cudaStream_t s);

@@ -483,6 +483,82 @@ def WriteReportInfoFile(path: str, cam: CameraModel, horizontal_fov: float, vert
 # ---------------------------------------------------------------------------------------
 # model comparison
 # ---------------------------------------------------------------------------------------
+def _png_chunk(kind: bytes, data: bytes) -> bytes:
+    import zlib
+    return struct.pack(">I", len(data)) + kind + data + struct.pack(">I", zlib.crc32(kind + data) & 0xFFFFFFFF)
+
+
+def EncodePNG(image: np.ndarray) -> bytes:
+    """An 8-bit grey ([h, w] or [h, w, 1]) or RGB ([h, w, 3]) image as a PNG file: one IDAT chunk holding a zlib
+    stream of stored (uncompressed) deflate blocks of at most 65535 bytes, filter type 0 on every row. The C++
+    writer (b200ba_io.hpp, WritePNG) produces the same bytes."""
+    import zlib
+    a = np.ascontiguousarray(image, dtype=np.uint8)
+    if a.ndim == 3 and a.shape[2] == 1:
+        a = a[:, :, 0]
+    if a.ndim == 2:
+        color_type = 0
+    elif a.ndim == 3 and a.shape[2] == 3:
+        color_type = 2
+    else:
+        raise ValueError("EncodePNG: expected an [h, w] or [h, w, 3] uint8 image")
+    h, w = a.shape[0], a.shape[1]
+    rows = a.reshape(h, -1)
+    raw = np.zeros((h, rows.shape[1] + 1), np.uint8)
+    raw[:, 1:] = rows
+    raw = raw.tobytes()
+    z = bytearray(b"\x78\x01")
+    pos = 0
+    while True:
+        block = raw[pos:pos + 65535]
+        pos += len(block)
+        final = pos >= len(raw)
+        z += bytes([1 if final else 0]) + struct.pack("<HH", len(block), len(block) ^ 0xFFFF) + block
+        if final:
+            break
+    z += struct.pack(">I", zlib.adler32(raw) & 0xFFFFFFFF)
+    ihdr = struct.pack(">IIBBBBB", w, h, 8, color_type, 0, 0, 0)
+    return (b"\x89PNG\r\n\x1a\n" + _png_chunk(b"IHDR", ihdr) + _png_chunk(b"IDAT", bytes(z)) +
+            _png_chunk(b"IEND", b""))
+
+
+def WritePNG(path: str, image: np.ndarray) -> bool:
+    """Writes EncodePNG(image) to path. Returns False if the file cannot be written."""
+    try:
+        data = EncodePNG(image)
+        with open(path, "wb") as f:
+            f.write(data)
+        return True
+    except OSError:
+        return False
+
+
+def HistogramImage(histogram) -> np.ndarray:
+    """The _errors_histogram.png image (calibration_report.cc:744-755): every bin scaled as count * 255.99f / max
+    (float times double, then divided), truncated to u8, [50, 50] y-major. An all-zero histogram gives an all-zero
+    image (the reference divides 0 by 0 there)."""
+    hist = np.asarray(histogram, dtype=np.float64).reshape(50, 50)
+    m = hist.max()
+    if m <= 0:
+        return np.zeros((50, 50), np.uint8)
+    return (hist * float(np.float32(255.99)) / m).astype(np.int64).astype(np.uint8)
+
+
+def GridPointLocationsImage(model: CentralGenericModel) -> np.ndarray:
+    """The _grid_point_locations.png image (calibration_report.cc:820-838): white where a B-spline control point
+    falls, GridPointToPixelCornerConv truncated with static_cast<int> (so (-1, 0) counts as 0), black elsewhere."""
+    w, h = model.width(), model.height()
+    img = np.zeros((h, w, 3), np.uint8)
+    gw, gh = model.GetGridResolution()
+    for y in range(gh):
+        for x in range(gw):
+            px, py = model.GridPointToPixelCornerConv(x, y)
+            ix, iy = int(px), int(py)  # truncation toward zero, as static_cast<int>
+            if 0 <= ix < w and 0 <= iy < h:
+                img[iy, ix] = 255
+    return img
+
+
 def WriteFittingInfoFile(path: str, report) -> bool:
     """``<base>_fitting_info.txt`` (APP/fitting_report.h:186-200) from a ``cabi.FittingReport``. The
     reference sorts its error vector for the median; here the median comes in (it is computed on the

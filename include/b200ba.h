@@ -239,6 +239,23 @@ typedef struct b200ba_camera_report {
  * report's buffers are allocated on the first call. Single-rank handles only. */
 B200BA_API int b200ba_calibration_report(b200ba_handle* h, b200ba_camera_report* reports /* [n_cameras] */,
                                          double* errors, double* report_ms);
+/* The images of CreateCalibrationReportForCamera (calibration_report.cc:713-838) for one camera, each [h*w*3]
+ * RGB row-major and nullable:
+ *   observation_directions  the un-projected direction of every pixel (x + 0.5f, y + 0.5f), coloured
+ *                           ((70*255.99f)/2.f)*(d+1) for x, y and ((270*255.99f)/2.f)*(d+1) for z, converted to u8
+ *                           as x86-64 does (truncation to int32, low byte); black where the un-projection fails.
+ *                           Central- and non-central-generic cameras only (returns 2 for others).
+ *   error_directions,       Voronoi maps of the feature sites: the first successful projection (caller's order) per
+ *   error_magnitudes        integer feature pixel ((int)x, (int)y) with 0 <= (int)x < 4w, 0 <= (int)y < 4h is a site
+ *                           at the quarter pixel ((int)(4x), (int)(4y)), coloured by its error's direction or by its
+ *                           magnitude (saturating at 0.5 px); a pixel is the sum of area(pixel n cell) * colour
+ *                           over the cells, + 0.5, clamped to [0, 255.99] and truncated (exact partition).
+ * n_sites (nullable): the number of sites; device_ms (nullable): device time. Uses the report's error pass and
+ * buffers; reads the state and writes none of it (nor last_projection, nor what b200ba_get_jacobians reads).
+ * Single-rank handles only; returns 2 for a bad camera index. */
+B200BA_API int b200ba_report_images(b200ba_handle* h, int32_t camera, uint8_t* observation_directions,
+                                    uint8_t* error_directions, uint8_t* error_magnitudes, int64_t* n_sites,
+                                    double* device_ms);
 
 /* ---- building blocks, exposed for parity tests and profiling -------------- */
 /* One pass of JointOptimizationCostFunction::Compute<compute_jacobians>
@@ -286,6 +303,14 @@ B200BA_API int b200ba_project(int device, const b200ba_camera* cam, const double
                    const double* local_points, double* pixels, int32_t* ok);
 B200BA_API int b200ba_unproject(int device, const b200ba_camera* cam, const double* intrinsics, int64_t n,
                      const double* pixels, double* directions, double* origins, int32_t* ok);
+
+/* Voronoi coverage rendering, the renderer of b200ba_report_images' error maps. sites_q [2n]: integer sites in
+ * quarter pixels, |x|, |y| <= 2^28 (a repeated position belongs to its lowest index); colors [3n]. image [h*w*3]
+ * RGB row-major: per pixel the sum over the Voronoi cells of area(pixel n cell) * colour, + 0.5, clamped to
+ * [0, 255.99] and truncated; no site gives black. device_ms (nullable): device time. Stand-alone (allocates,
+ * computes, frees); returns 2 for a bad argument, 3 without a device. */
+B200BA_API int b200ba_render_voronoi(int device, int32_t width, int32_t height, int64_t n_sites, const int32_t* sites_q,
+                                     const float* colors, uint8_t* image, double* device_ms);
 
 /* ---- model resampling (row f-4): CentralGenericModel::FitToPixelDirectionsImpl --------
  * (APP/models/central_generic.cc:551-568 with the cost function of :152-228 and the state of

@@ -22,6 +22,7 @@
 // file, like the reference's.
 #pragma once
 
+#include <algorithm>
 #include <cerrno>
 #include <cstdio>
 #include <cstdlib>
@@ -561,6 +562,79 @@ inline bool LoadPointsAndIndexMapping(BAState* state, const char* path) {
 
 // ---- the state directory --------------------------------------------------------------------------------
 // APP/io:432-464
+// ---- PNG (8-bit grey or RGB) ------------------------------------------------------------------------------------
+// One IDAT chunk holding a zlib stream of stored (uncompressed) deflate blocks of at most 65535 bytes, filter type 0
+// on every row: no compression library needed. io.py's EncodePNG writes the same bytes.
+namespace io_detail {
+inline uint32_t png_crc32(const std::string& data, size_t begin) {
+  static uint32_t table[256];
+  static bool init = false;
+  if (!init) {
+    for (uint32_t n = 0; n < 256; ++n) {
+      uint32_t c = n;
+      for (int k = 0; k < 8; ++k) c = (c & 1) ? 0xedb88320u ^ (c >> 1) : c >> 1;
+      table[n] = c;
+    }
+    init = true;
+  }
+  uint32_t c = 0xffffffffu;
+  for (size_t i = begin; i < data.size(); ++i) c = table[(c ^ static_cast<uint8_t>(data[i])) & 0xff] ^ (c >> 8);
+  return c ^ 0xffffffffu;
+}
+inline void put_be32(std::string* out, uint32_t v) {
+  const char b[4] = {static_cast<char>(v >> 24), static_cast<char>(v >> 16), static_cast<char>(v >> 8), static_cast<char>(v)};
+  out->append(b, 4);
+}
+inline void png_chunk(std::string* out, const char* kind, const std::string& data) {
+  put_be32(out, static_cast<uint32_t>(data.size()));
+  const size_t start = out->size();
+  out->append(kind, 4);
+  out->append(data);
+  put_be32(out, png_crc32(*out, start));
+}
+}  // namespace io_detail
+
+// channels: 1 (grey) or 3 (RGB); pixels [height * width * channels], row-major. Returns false if the file cannot be
+// written or the arguments are invalid.
+inline bool WritePNG(const std::string& path, int width, int height, int channels, const uint8_t* pixels) {
+  if (width < 1 || height < 1 || (channels != 1 && channels != 3)) return false;
+  const size_t row = static_cast<size_t>(width) * channels;
+  std::string raw;
+  raw.reserve((row + 1) * height);
+  for (int y = 0; y < height; ++y) {
+    raw.push_back(0);
+    raw.append(reinterpret_cast<const char*>(pixels + y * row), row);
+  }
+  std::string z("\x78\x01", 2);
+  size_t pos = 0;
+  do {
+    const size_t len = std::min<size_t>(65535, raw.size() - pos);
+    const bool final = pos + len >= raw.size();
+    z.push_back(final ? 1 : 0);
+    const uint16_t l = static_cast<uint16_t>(len), nl = static_cast<uint16_t>(~l);
+    const char hdr[4] = {static_cast<char>(l & 0xff), static_cast<char>(l >> 8), static_cast<char>(nl & 0xff), static_cast<char>(nl >> 8)};
+    z.append(hdr, 4);
+    z.append(raw, pos, len);
+    pos += len;
+  } while (pos < raw.size());
+  uint32_t a = 1, b = 0;  // Adler-32
+  for (char ch : raw) {
+    a = (a + static_cast<uint8_t>(ch)) % 65521u;
+    b = (b + a) % 65521u;
+  }
+  io_detail::put_be32(&z, (b << 16) | a);
+  std::string ihdr;
+  io_detail::put_be32(&ihdr, static_cast<uint32_t>(width));
+  io_detail::put_be32(&ihdr, static_cast<uint32_t>(height));
+  const char rest[5] = {8, static_cast<char>(channels == 1 ? 0 : 2), 0, 0, 0};
+  ihdr.append(rest, 5);
+  std::string out("\x89PNG\r\n\x1a\n", 8);
+  io_detail::png_chunk(&out, "IHDR", ihdr);
+  io_detail::png_chunk(&out, "IDAT", z);
+  io_detail::png_chunk(&out, "IEND", std::string());
+  return io_detail::write_file(path, out);
+}
+
 inline bool SaveBAState(const char* base_path, const BAState& state) {
   using namespace io_detail;
   make_directories(base_path);

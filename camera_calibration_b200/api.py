@@ -1007,3 +1007,37 @@ def CompareModels(model_a: CameraModel, model_b: CameraModel, with_errors: bool 
                                      None if dir_err is None else _dp(dir_err),
                                      None if rep_err is None else _dp(rep_err), C.byref(ms)))
     return report, dir_err, rep_err, ms.value
+
+
+def LineObjCount(model: CameraModel, obj_step: int = 20) -> int:
+    """Number of lines in the .obj models of the centre-point analysis: every obj_step-th pixel of the calibrated
+    area from calibration_min in x and in y (calibration_report.cc:945-946)."""
+    rw = model.calibration_max_x() - model.calibration_min_x() + 1
+    rh = model.calibration_max_y() - model.calibration_min_y() + 1
+    if obj_step < 1 or rw < 1 or rh < 1:
+        return 0
+    return ((rw - 1) // obj_step + 1) * ((rh - 1) // obj_step + 1)
+
+
+def LineOffsets(model: CameraModel, obj_step: int = 20, device: int = -1):
+    """The centre-point analysis of a non-central camera (the NoncentralGenericModel branch of
+    CreateCalibrationReportForCamera, APP/calibration_report.cc:839-982) on the device (``b200ba_line_offsets``).
+    Returns (report, image, offsets, obj_lines, device_ms): a ``cabi.LineOffsetsReport``; the [h, w, 3] uint8
+    ``_line_offsets.png`` image; the [h, w, 3] offsets closest point - centre (NaN where there is no line); the
+    [n_obj, 4, 3] point_a, point_b, closest point and origin of every obj_step-th line (``io.WriteLineVisualizationOBJ``
+    writes the .obj files from them)."""
+    lib = cabi.load_library()
+    cam = model.c_camera()
+    intr = np.ascontiguousarray(model.flat_intrinsics(), dtype=np.float64)
+    h, w = model.height(), model.width()
+    image = np.zeros((h, w, 3), np.uint8)
+    offsets = np.empty((h, w, 3))
+    n_expected = LineObjCount(model, obj_step)
+    obj = np.empty((max(n_expected, 1), 4, 3))
+    n_obj = C.c_int64(0)
+    report = cabi.LineOffsetsReport()
+    ms = C.c_double(0)
+    _check(lib.b200ba_line_offsets(device, C.byref(cam), _dp(intr), C.byref(report), _u8p(image), _dp(offsets),
+                                   int(obj_step), _dp(obj), C.byref(n_obj), C.byref(ms)))
+    assert n_obj.value == n_expected, (n_obj.value, n_expected)
+    return report, image, offsets, obj[:n_obj.value], ms.value

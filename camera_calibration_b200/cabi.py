@@ -228,6 +228,22 @@ class FittingReport(C.Structure):
     ]
 
 
+class LineOffsetsReport(C.Structure):
+    """b200ba_line_offsets_report: the centre-point analysis of a non-central camera."""
+    _fields_ = [
+        ("center", C.c_double * 3),
+        ("line_count", C.c_int64),
+        ("line_distance_sum", C.c_double),
+        ("line_distance_max", C.c_double),
+        ("line_distance_median", C.c_double),
+        ("max_line_offset_extent", C.c_double),
+        ("initial_cost", C.c_double),
+        ("final_cost", C.c_double),
+        ("num_iterations_performed", C.c_int32),
+        ("lm_attempts", C.c_int32),
+    ]
+
+
 class FitReport(C.Structure):
     """b200ba_fit_report."""
     _fields_ = [
@@ -395,6 +411,8 @@ SYMBOLS = {
                                         C.POINTER(FitReport)]),
     "b200ba_compare_models": (C.c_int, [C.c_int, C.POINTER(Camera), _D, C.POINTER(Camera), _D, C.POINTER(FittingReport),
                                         _D, _D, _D]),
+    "b200ba_line_offsets": (C.c_int, [C.c_int, C.POINTER(Camera), _D, C.POINTER(LineOffsetsReport), C.POINTER(C.c_uint8),
+                                      _D, C.c_int32, _D, C.POINTER(C.c_int64), _D]),
     "b200ba_nccl_unique_id": (C.c_int, [C.POINTER(C.c_uint8)]),
     "b200ba_comm_init": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint8), C.c_int, C.c_int]),
     "b200ba_get_timings": (C.c_int, [C.c_void_p, C.POINTER(Timings)]),

@@ -145,6 +145,24 @@ struct CompareDev {
   ReportCam* stats;             // count / sum / max / median
 };
 
+// Centre-point analysis of a non-central camera (b200ba_line_offsets): device buffers of one call. The n lines are
+// those of the pixels of the calibrated rectangle, p = (y - min_y) * rw + (x - min_x).
+constexpr int kLineSums = 10;  // per LM pass: cost, b (3), H (6: 00 01 02 11 12 22)
+struct LineOffsetsDev {
+  double* lines;               // [6 * n] SoA: origin x, y, z, direction x, y, z
+  double* partial;             // line_system_partial_size(): first stage of the LM sums
+  double* sums;                // [kLineSums]
+  double* mag;                 // [n] line distance |closest - centre|
+  unsigned long long* extent;  // bit pattern of max_line_offset_extent
+  int64_t* range;              // [2] {0, n}: the one range of launch_report_statistics
+  double* stat_partial;        // report_partial_size(1)
+  unsigned int* select_hist;   // [256]
+  ReportCam* stats;            // count / sum / max / median of the line distances
+  double* offsets;             // [3 * w * h] or NULL
+  uint8_t* image;              // [3 * w * h] or NULL
+  double* obj;                 // [12 * n_obj] or NULL
+};
+
 // Voronoi coverage renderer (b200ba_render_voronoi, b200ba_report_images). Sites are integer points in
 // quarter-pixel units; a site whose x is kVoronoiNoSite is ignored. The sites are binned into a uniform
 // grid of square buckets that covers the image and every site: bucket (bx, by) holds the sites with

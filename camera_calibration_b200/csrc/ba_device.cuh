@@ -240,6 +240,51 @@ __device__ __forceinline__ void noncentral_eval(const CamDev& c, const double* _
   e.ox = c.sx * ox;
   e.oy = c.sy * oy;
 }
+// Value-only B-spline weights and 3-vector surface value (the w / v parts of bspline_basis / spline3), for passes
+// that need no pixel derivatives.
+__device__ __forceinline__ void bspline_weights(double u, double w[4]) {
+  const double u2 = u * u, u3 = u2 * u;
+  const double omu = 1.0 - u;
+  constexpr double k6 = 1.0 / 6.0;
+  w[0] = omu * omu * omu * k6;
+  w[1] = (3.0 * u3 - 6.0 * u2 + 4.0) * k6;
+  w[2] = (-3.0 * u3 + 3.0 * u2 + 3.0 * u + 1.0) * k6;
+  w[3] = u3 * k6;
+}
+__device__ __forceinline__ d3 spline3_value(const double* __restrict__ g, int gw, int x0, int y0, const double wx[4],
+                                            const double wy[4]) {
+  d3 v = mk3(0, 0, 0);
+  const double* row = g + 3 * (static_cast<int64_t>(y0) * gw + x0);
+#pragma unroll 1
+  for (int r = 0; r < 4; ++r) {
+    d3 a = mk3(0, 0, 0);
+#pragma unroll
+    for (int cidx = 0; cidx < 4; ++cidx) a = fma3(wx[cidx], ld3(row + 3 * cidx), a);
+    v = fma3(sel4(wy, r), a, v);
+    row += 3 * static_cast<int64_t>(gw);
+  }
+  return v;
+}
+// NoncentralGenericModel::UnprojectFromGrid (noncentral_generic.h:100-105) at pixel (x, y), value only: origin o and
+// the direction normalised as Eigen's normalize() does, d = v / sqrt(|v|^2) (|v|^2 without FMA; v unchanged if 0).
+__device__ __forceinline__ void noncentral_line(const CamDev& c, const double* __restrict__ dgrid,
+                                                const double* __restrict__ pgrid, double x, double y, d3& o, d3& d) {
+  int x0, y0;
+  double fu, fv;
+  locate(c, x, y, x0, y0, fu, fv);
+  double wx[4], wy[4];
+  bspline_weights(fu, wx);
+  bspline_weights(fv, wy);
+  const d3 v = spline3_value(dgrid, c.gw, x0, y0, wx, wy);
+  o = spline3_value(pgrid, c.gw, x0, y0, wx, wy);
+  const double n2 = __dadd_rn(__dadd_rn(__dmul_rn(v.x, v.x), __dmul_rn(v.y, v.y)), __dmul_rn(v.z, v.z));
+  if (n2 > 0) {
+    const double n = sqrt(n2);
+    d = mk3(v.x / n, v.y / n, v.z / n);
+  } else {
+    d = v;
+  }
+}
 // residual r = (t1 . (o - p), t2 . (o - p)) (noncentral_generic.cc:166-172)
 __device__ __forceinline__ void noncentral_residual(const NoncentralEval& e, d3 p, double& r0, double& r1,
                                                     d3& t1, d3& t2) {

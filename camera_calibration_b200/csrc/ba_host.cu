@@ -20,6 +20,7 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <limits>
 #include <string>
 #include <vector>
 
@@ -2681,6 +2682,209 @@ int b200ba_render_voronoi(int device, int32_t width, int32_t height, int64_t n_s
   }
   vr.release();
   cudaFree(d_sites); cudaFree(d_colors); cudaFree(d_img);
+  if (e0) cudaEventDestroy(e0);
+  if (e1) cudaEventDestroy(e1);
+  return rc;
+}
+
+// Eigen::LDLT<MatrixXd, Lower>(A.selfadjointView<Upper>()).solve(b) for n = 3 (SolveDensely, LV/lm_optimizer.h:1022-1023):
+// symmetric pivoting on the largest remaining |diagonal| entry as Eigen's left-looking factorisation sees it (the
+// ORIGINAL values of the trailing diagonal), then x = P^T L^-T D^-1 L^-1 P b with 1 / d_i taken as 0 where
+// |d_i| <= 1 / DBL_MAX. A is symmetric, row-major.
+static void ldlt_solve3(const double A[3][3], const double b[3], double x[3]) {
+  double L[3][3], od[3], col[3];
+  int transp[3];
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j <= i; ++j) L[i][j] = A[j][i];
+  for (int i = 0; i < 3; ++i) od[i] = L[i][i];
+  for (int k = 0; k < 3; ++k) {
+    int piv = k;
+    for (int i = k + 1; i < 3; ++i)
+      if (std::fabs(od[i]) > std::fabs(od[piv])) piv = i;
+    transp[k] = piv;
+    if (piv != k) {  // symmetric row / column swap k <-> piv on the lower triangle
+      std::swap(od[k], od[piv]);
+      for (int j = 0; j < k; ++j) std::swap(L[k][j], L[piv][j]);
+      for (int i = piv + 1; i < 3; ++i) std::swap(L[i][k], L[i][piv]);
+      std::swap(L[k][k], L[piv][piv]);
+      for (int i = k + 1; i < piv; ++i) std::swap(L[i][k], L[piv][i]);
+    }
+    const double dk = L[k][k];
+    if (std::fabs(dk) > 0) {
+      for (int i = k + 1; i < 3; ++i) {
+        col[i] = L[i][k];
+        L[i][k] = col[i] / dk;
+      }
+      for (int i = k + 1; i < 3; ++i)
+        for (int j = k + 1; j <= i; ++j) L[i][j] -= L[i][k] * col[j];
+    }
+  }
+  double y[3] = {b[0], b[1], b[2]};
+  for (int k = 0; k < 3; ++k) std::swap(y[k], y[transp[k]]);
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < i; ++j) y[i] -= L[i][j] * y[j];
+  const double tolerance = 1.0 / std::numeric_limits<double>::max();
+  for (int i = 0; i < 3; ++i) y[i] = std::fabs(L[i][i]) > tolerance ? y[i] / L[i][i] : 0.0;
+  for (int i = 2; i >= 0; --i)
+    for (int j = 0; j < i; ++j) y[j] -= L[i][j] * y[i];
+  for (int k = 2; k >= 0; --k) std::swap(y[k], y[transp[k]]);
+  for (int i = 0; i < 3; ++i) x[i] = y[i];
+}
+
+// The NoncentralGenericModel branch of CreateCalibrationReportForCamera (APP/calibration_report.cc:839-982). The
+// argument checks come first and touch no CUDA state. The LM loop restates LMOptimizer::OptimizeImpl
+// (LV/lm_optimizer.h:628-991) as b200ba_fit_directions does; H = sum t1 t1^T + t2 t2^T does not depend on the centre,
+// so it is summed once (the reference rebuilds the same matrix every iteration), and every iteration then needs one
+// pass for b and the cost and every attempt one pass for the trial cost, each a sum of per-line costs.
+int b200ba_line_offsets(int device, const b200ba_camera* cam, const double* intrinsics, b200ba_line_offsets_report* report,
+                        uint8_t* image, double* offsets, int32_t obj_step, double* obj_lines, int64_t* n_obj,
+                        double* device_ms) {
+  if (!cam || !intrinsics || !report) {
+    g_create_error = "b200ba_line_offsets: a required argument is NULL";
+    return 2;
+  }
+  if (cam->model_type != B200BA_MODEL_NONCENTRAL_GENERIC) {
+    g_create_error = "b200ba_line_offsets: the centre-point analysis is only defined for NoncentralGenericModel";
+    return 2;
+  }
+  if (cam->grid_width < 4 || cam->grid_height < 4) {
+    g_create_error = "b200ba_line_offsets: the grid is smaller than 4 x 4";
+    return 2;
+  }
+  if (obj_step < 1 || (obj_lines && !n_obj)) {
+    g_create_error = "b200ba_line_offsets: obj_step must be >= 1, and obj_lines needs n_obj";
+    return 2;
+  }
+  // the reference writes every line's offset into an image of the camera's size (:870, :889)
+  if (cam->calibration_min_x < 0 || cam->calibration_min_y < 0 || cam->calibration_max_x < cam->calibration_min_x ||
+      cam->calibration_max_y < cam->calibration_min_y || cam->calibration_max_x >= cam->width ||
+      cam->calibration_max_y >= cam->height) {
+    g_create_error = "b200ba_line_offsets: the calibrated area is empty or not inside the image";
+    return 2;
+  }
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
+    g_create_error = "no CUDA device available (this library has no CPU fallback)";
+    return 3;
+  }
+  if (device >= 0) cudaSetDevice(device);
+  CamDev c{};
+  fill_camdev(*cam, &c);
+  const int rw = cam->calibration_max_x - cam->calibration_min_x + 1, rh = cam->calibration_max_y - cam->calibration_min_y + 1;
+  const int64_t n = static_cast<int64_t>(rw) * rh, npx = static_cast<int64_t>(cam->width) * cam->height;
+  const int nx = (rw - 1) / obj_step + 1, ny = (rh - 1) / obj_step + 1;
+  const int64_t nobj = static_cast<int64_t>(nx) * ny;
+  const int64_t ni = intrinsics_size(*cam);
+  const int64_t range[2] = {0, n};
+  double* dintr = nullptr;
+  LineOffsetsDev d{};
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  int rc = 0;
+  auto ok = [&](cudaError_t e) {
+    if (e != cudaSuccess && rc == 0) {
+      g_create_error = cudaGetErrorString(e);
+      rc = 1;
+    }
+  };
+  ok(cudaMalloc(&dintr, sizeof(double) * ni));
+  ok(cudaMalloc(&d.lines, sizeof(double) * 6 * n));
+  ok(cudaMalloc(&d.partial, sizeof(double) * line_system_partial_size()));
+  ok(cudaMalloc(&d.sums, sizeof(double) * kLineSums));
+  ok(cudaMalloc(&d.mag, sizeof(double) * n));
+  ok(cudaMalloc(&d.extent, sizeof(unsigned long long)));
+  ok(cudaMalloc(&d.range, sizeof(range)));
+  ok(cudaMalloc(&d.stat_partial, sizeof(double) * report_partial_size(1)));
+  ok(cudaMalloc(&d.select_hist, 256 * sizeof(unsigned int)));
+  ok(cudaMalloc(&d.stats, sizeof(ReportCam)));
+  if (offsets) ok(cudaMalloc(&d.offsets, sizeof(double) * 3 * npx));
+  if (image) ok(cudaMalloc(&d.image, 3 * npx));
+  if (obj_lines) ok(cudaMalloc(&d.obj, sizeof(double) * 12 * nobj));
+  ok(cudaEventCreate(&e0));
+  ok(cudaEventCreate(&e1));
+  if (rc == 0) {
+    ok(cudaMemcpy(dintr, intrinsics, sizeof(double) * ni, cudaMemcpyHostToDevice));
+    ok(cudaMemcpy(d.range, range, sizeof(range), cudaMemcpyHostToDevice));
+  }
+  b200ba_line_offsets_report rep{};
+  double center[3] = {0, 0, 0};  // Vec3d::Zero() (:858)
+  ReportCam stats{};
+  unsigned long long extent_bits = 0;
+  if (rc == 0) {
+    cudaEventRecord(e0, 0);
+    launch_line_pass(c, dintr, d, 0);
+    auto pass = [&](int mode, const double* at, double* out) {
+      launch_line_system(mode, n, at, d, 0);
+      ok(cudaMemcpy(out, d.sums, sizeof(double) * kLineSums, cudaMemcpyDeviceToHost));
+    };
+    // Optimize(&center, cost, max_iteration_count = 100, max_lm_attempts = 10, init_lambda = -1,
+    // init_lambda_factor = 0.001f) (:859-867)
+    double H[3][3] = {}, lambda = 0, last_cost = 0;
+    const double init_lambda_factor = static_cast<double>(0.001f);
+    for (int iteration = 0; rc == 0 && iteration < 100; ++iteration) {
+      double s[kLineSums];
+      pass(iteration == 0 ? 2 : 1, center, s);
+      if (rc) break;
+      last_cost = s[0];
+      if (iteration == 0) {
+        rep.initial_cost = last_cost;
+        H[0][0] = s[4]; H[0][1] = H[1][0] = s[5]; H[0][2] = H[2][0] = s[6];
+        H[1][1] = s[7]; H[1][2] = H[2][1] = s[8]; H[2][2] = s[9];
+      }
+      if (last_cost == 0) break;
+      if (iteration == 0) lambda = init_lambda_factor * (((0.0 + H[0][0]) + H[1][1]) + H[2][2]) / 3;
+      bool applied = false;
+      for (int attempt = 0; rc == 0 && attempt < 10; ++attempt) {
+        rep.lm_attempts++;
+        double A[3][3], x[3];
+        for (int i = 0; i < 3; ++i)
+          for (int j = 0; j < 3; ++j) A[i][j] = H[i][j] + (i == j ? lambda : 0.0);
+        ldlt_solve3(A, s + 1, x);
+        if (std::isnan(x[0])) {  // the reference's NaN-update branch
+          lambda = 2.f * lambda;
+          continue;
+        }
+        const double trial[3] = {center[0] - x[0], center[1] - x[1], center[2] - x[2]};
+        double t[kLineSums];
+        pass(0, trial, t);
+        if (rc) break;
+        if (t[0] < last_cost) {  // CostIsSmallerThan: every residual is valid in both states
+          std::copy(trial, trial + 3, center);
+          lambda = 0.5f * lambda;
+          applied = true;
+          rep.num_iterations_performed += 1;
+          last_cost = t[0];
+          break;
+        }
+        lambda = 2.f * lambda;
+      }
+      if (!applied || last_cost == 0) break;
+    }
+    rep.final_cost = last_cost;
+    launch_line_outputs(c, center, d, obj_step, nx, nobj, 0);
+    cudaEventRecord(e1, 0);
+    ok(cudaGetLastError());
+    ok(cudaMemcpy(&stats, d.stats, sizeof(ReportCam), cudaMemcpyDeviceToHost));
+    ok(cudaMemcpy(&extent_bits, d.extent, sizeof(extent_bits), cudaMemcpyDeviceToHost));
+    if (offsets) ok(cudaMemcpy(offsets, d.offsets, sizeof(double) * 3 * npx, cudaMemcpyDeviceToHost));
+    if (image) ok(cudaMemcpy(image, d.image, 3 * npx, cudaMemcpyDeviceToHost));
+    if (obj_lines) ok(cudaMemcpy(obj_lines, d.obj, sizeof(double) * 12 * nobj, cudaMemcpyDeviceToHost));
+  }
+  if (rc == 0) {
+    float ms = 0;
+    ok(cudaEventElapsedTime(&ms, e0, e1));
+    if (device_ms) *device_ms = ms;
+    std::copy(center, center + 3, rep.center);
+    rep.line_count = stats.count;
+    rep.line_distance_sum = stats.sum;
+    rep.line_distance_max = stats.max;  // max is order-independent: the fixed-order reduction's max is exact
+    rep.line_distance_median = stats.median;
+    memcpy(&rep.max_line_offset_extent, &extent_bits, sizeof(double));
+    *report = rep;
+    if (n_obj) *n_obj = nobj;
+  }
+  cudaFree(dintr); cudaFree(d.lines); cudaFree(d.partial); cudaFree(d.sums); cudaFree(d.mag); cudaFree(d.extent);
+  cudaFree(d.range); cudaFree(d.stat_partial); cudaFree(d.select_hist); cudaFree(d.stats); cudaFree(d.offsets);
+  cudaFree(d.image); cudaFree(d.obj);
   if (e0) cudaEventDestroy(e0);
   if (e1) cudaEventDestroy(e1);
   return rc;

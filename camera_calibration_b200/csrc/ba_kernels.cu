@@ -2185,6 +2185,225 @@ void launch_compare_models(const CamDev& a, const double* ga, const CamDev& b, c
 }
 
 // ------------------------------------------------------------------------------------------
+// centre-point analysis of a non-central camera (CreateCalibrationReportForCamera, APP/calibration_report.cc:839-982)
+// ------------------------------------------------------------------------------------------
+// The lines are evaluated once and stored (48 B per line: 55 MB for 1200 x 950, 576 MB for 4000 x 3000); every LM
+// pass then streams them instead of re-evaluating two B-spline surfaces per line. DESIGN.md section 4 has the
+// measured times of both: about equal, since a streaming pass is bound by the tangent frame's FP64 arithmetic. Each pixel of the calibrated rectangle lies in the calibrated area, so every Unproject
+// of :847-856 succeeds and there is one line per rectangle pixel.
+constexpr int kLineTileX = 16, kLineTileY = 8;
+__global__ void __launch_bounds__(kLineTileX * kLineTileY)
+    line_pass_kernel(CamDev c, const double* __restrict__ intr, double* __restrict__ lines) {
+  const int rw = c.max_x - c.min_x + 1, rh = c.max_y - c.min_y + 1;
+  const int lx = blockIdx.x * kLineTileX + threadIdx.x, ly = blockIdx.y * kLineTileY + threadIdx.y;
+  if (lx >= rw || ly >= rh) return;
+  // the reference passes x + 0.5f (a float) where Unproject takes a double
+  const double px = static_cast<double>((c.min_x + lx) + 0.5f), py = static_cast<double>((c.min_y + ly) + 0.5f);
+  d3 o, d;
+  noncentral_line(c, intr, intr + 3 * static_cast<int64_t>(c.gw) * c.gh, px, py, o, d);
+  const int64_t n = static_cast<int64_t>(rw) * rh, p = static_cast<int64_t>(ly) * rw + lx;
+  lines[p] = o.x;
+  lines[n + p] = o.y;
+  lines[2 * n + p] = o.z;
+  lines[3 * n + p] = d.x;
+  lines[4 * n + p] = d.y;
+  lines[5 * n + p] = d.z;
+}
+__device__ __forceinline__ void load_line(const double* __restrict__ lines, int64_t n, int64_t p, d3& o, d3& d) {
+  o = mk3(lines[p], lines[n + p], lines[2 * n + p]);
+  d = mk3(lines[3 * n + p], lines[4 * n + p], lines[5 * n + p]);
+}
+
+// One pass of CenterPointCostFunction::Compute (:56-80) at the centre c: sum over the lines of the per-line cost
+// 1/2 (r1^2 + r2^2) (mode >= 0), of b = t1 r1 + t2 r2 (mode >= 1) and of H = t1 t1^T + t2 t2^T (mode 2), in the
+// fixed two-stage order of report_reduce_stage1/2. The cost is written with non-fused operations, so that every mode
+// computes the same bits for it: the trial cost of an accepted step IS the next iteration's cost, as in the reference.
+template <int kMode>
+__global__ void __launch_bounds__(kReportThreads)
+    line_system_stage1(int64_t n, const double* __restrict__ lines, double cx, double cy, double cz,
+                       double* __restrict__ partial) {
+  double s[kLineSums];
+#pragma unroll
+  for (int k = 0; k < kLineSums; ++k) s[k] = 0;
+  for (int64_t p = blockIdx.x * static_cast<int64_t>(kReportThreads) + threadIdx.x; p < n;
+       p += static_cast<int64_t>(kReportBlocks) * kReportThreads) {
+    d3 o, d, t1, t2;
+    load_line(lines, n, p, o, d);
+    compute_tangents(d, t1, t2);
+    const d3 q = mk3(__dsub_rn(cx, o.x), __dsub_rn(cy, o.y), __dsub_rn(cz, o.z));
+    const double r1 = dot3(t1, q), r2 = dot3(t2, q);
+    s[0] += __dmul_rn(0.5, __dadd_rn(__dmul_rn(r1, r1), __dmul_rn(r2, r2)));
+    if (kMode >= 1) {
+      s[1] += t1.x * r1 + t2.x * r2;
+      s[2] += t1.y * r1 + t2.y * r2;
+      s[3] += t1.z * r1 + t2.z * r2;
+    }
+    if (kMode >= 2) {
+      s[4] += t1.x * t1.x + t2.x * t2.x;
+      s[5] += t1.x * t1.y + t2.x * t2.y;
+      s[6] += t1.x * t1.z + t2.x * t2.z;
+      s[7] += t1.y * t1.y + t2.y * t2.y;
+      s[8] += t1.y * t1.z + t2.y * t2.z;
+      s[9] += t1.z * t1.z + t2.z * t2.z;
+    }
+  }
+  constexpr int kUsed = kMode == 0 ? 1 : (kMode == 1 ? 4 : kLineSums);
+  __shared__ double sh[kUsed][kReportThreads];
+#pragma unroll
+  for (int k = 0; k < kUsed; ++k) sh[k][threadIdx.x] = s[k];
+  __syncthreads();
+  for (int st = kReportThreads / 2; st > 0; st >>= 1) {
+    if (threadIdx.x < st) {
+#pragma unroll
+      for (int k = 0; k < kUsed; ++k) sh[k][threadIdx.x] += sh[k][threadIdx.x + st];
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x < kLineSums) partial[blockIdx.x * kLineSums + threadIdx.x] = threadIdx.x < kUsed ? sh[threadIdx.x][0] : 0.0;
+}
+__global__ void line_system_stage2(const double* __restrict__ partial, double* __restrict__ sums) {
+  const int k = threadIdx.x;
+  if (k >= kLineSums) return;
+  double v = 0;
+  for (int b = 0; b < kReportBlocks; ++b) v += partial[b * kLineSums + k];
+  sums[k] = v;
+}
+int line_system_partial_size() { return kReportBlocks * kLineSums; }
+void launch_line_pass(const CamDev& c, const double* intr, const LineOffsetsDev& d, cudaStream_t s) {
+  const int rw = c.max_x - c.min_x + 1, rh = c.max_y - c.min_y + 1;
+  const dim3 grid((rw + kLineTileX - 1) / kLineTileX, (rh + kLineTileY - 1) / kLineTileY);
+  line_pass_kernel<<<grid, dim3(kLineTileX, kLineTileY), 0, s>>>(c, intr, d.lines);
+}
+void launch_line_system(int mode, int64_t n, const double c[3], const LineOffsetsDev& d, cudaStream_t s) {
+  if (mode == 0) line_system_stage1<0><<<kReportBlocks, kReportThreads, 0, s>>>(n, d.lines, c[0], c[1], c[2], d.partial);
+  else if (mode == 1) line_system_stage1<1><<<kReportBlocks, kReportThreads, 0, s>>>(n, d.lines, c[0], c[1], c[2], d.partial);
+  else line_system_stage1<2><<<kReportBlocks, kReportThreads, 0, s>>>(n, d.lines, c[0], c[1], c[2], d.partial);
+  line_system_stage2<<<1, 32, 0, s>>>(d.partial, d.sums);
+}
+
+// :884-888 with no fused operation: parameter = d . (c - o), closest = o + parameter d, offset = closest - c
+__device__ __forceinline__ d3 line_offset(d3 o, d3 d, d3 c, d3& closest) {
+  const d3 q = mk3(__dsub_rn(c.x, o.x), __dsub_rn(c.y, o.y), __dsub_rn(c.z, o.z));
+  const double t = __dadd_rn(__dadd_rn(__dmul_rn(d.x, q.x), __dmul_rn(d.y, q.y)), __dmul_rn(d.z, q.z));
+  closest = mk3(__dadd_rn(o.x, __dmul_rn(t, d.x)), __dadd_rn(o.y, __dmul_rn(t, d.y)), __dadd_rn(o.z, __dmul_rn(t, d.z)));
+  return mk3(__dsub_rn(closest.x, c.x), __dsub_rn(closest.y, c.y), __dsub_rn(closest.z, c.z));
+}
+// Vector3d::norm() in Eigen's order, no fused multiply-add
+__device__ __forceinline__ double line_norm(d3 v) {
+  return sqrt(__dadd_rn(__dadd_rn(__dmul_rn(v.x, v.x), __dmul_rn(v.y, v.y)), __dmul_rn(v.z, v.z)));
+}
+
+// :880-902: the line distance of every line into mag (statistics by launch_report_statistics) and the extent, an exact
+// block maximum followed by one atomicMax per block on the bit pattern (non-negative doubles order like their uint64
+// patterns; fmax skips NaN as the reference's std::max(extent, NaN) keeps extent)
+__global__ void __launch_bounds__(kReportThreads)
+    line_distances_kernel(int64_t n, const double* __restrict__ lines, double cx, double cy, double cz,
+                          double* __restrict__ mag, unsigned long long* __restrict__ extent) {
+  const int64_t p = blockIdx.x * static_cast<int64_t>(kReportThreads) + threadIdx.x;
+  double ext = 0;
+  if (p < n) {
+    d3 o, d, closest;
+    load_line(lines, n, p, o, d);
+    const d3 off = line_offset(o, d, mk3(cx, cy, cz), closest);
+    mag[p] = line_norm(off);
+    ext = fmax(fabs(off.x), fmax(fabs(off.y), fabs(off.z)));
+  }
+  for (int o = 16; o > 0; o >>= 1) ext = fmax(ext, __shfl_xor_sync(0xffffffffu, ext, o));
+  __shared__ double sh[kReportThreads / 32];
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = ext;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double v = 0;
+    for (int w = 0; w < kReportThreads / 32; ++w) v = fmax(v, sh[w]);
+    if (v > 0) atomicMax(extent, static_cast<unsigned long long>(__double_as_longlong(v)));
+  }
+}
+
+// :870-871, :913-926 per image pixel: the offset (NaN outside the calibrated rectangle) and the colour
+// 127 + 127 * offset_k / extent in double, converted as x86-64 converts double to u8 (truncation to int32, low byte;
+// with extent 0 every channel is NaN and gives 0); black where the offset has a NaN
+__global__ void __launch_bounds__(kLineTileX * kLineTileY)
+    line_offsets_image_kernel(CamDev c, const double* __restrict__ lines, double cx, double cy, double cz,
+                              const unsigned long long* __restrict__ extent, double* __restrict__ offsets,
+                              uint8_t* __restrict__ img) {
+  const int x = blockIdx.x * kLineTileX + threadIdx.x, y = blockIdx.y * kLineTileY + threadIdx.y;
+  if (x >= c.width || y >= c.height) return;
+  const double nan_v = nan("");
+  d3 off = mk3(nan_v, nan_v, nan_v);
+  if (x >= c.min_x && x <= c.max_x && y >= c.min_y && y <= c.max_y) {
+    const int rw = c.max_x - c.min_x + 1;
+    const int64_t n = static_cast<int64_t>(rw) * (c.max_y - c.min_y + 1);
+    d3 o, d, closest;
+    load_line(lines, n, static_cast<int64_t>(y - c.min_y) * rw + (x - c.min_x), o, d);
+    off = line_offset(o, d, mk3(cx, cy, cz), closest);
+  }
+  const int64_t q = 3 * (static_cast<int64_t>(y) * c.width + x);
+  if (offsets) {
+    offsets[q] = off.x;
+    offsets[q + 1] = off.y;
+    offsets[q + 2] = off.z;
+  }
+  if (img) {
+    uint8_t out[3] = {0, 0, 0};
+    if (!isnan(off.x) && !isnan(off.y) && !isnan(off.z)) {
+      const double e = __longlong_as_double(static_cast<long long>(*extent));
+      out[0] = static_cast<uint8_t>(report_trunc(__dadd_rn(127.0, __ddiv_rn(__dmul_rn(127.0, off.x), e))));
+      out[1] = static_cast<uint8_t>(report_trunc(__dadd_rn(127.0, __ddiv_rn(__dmul_rn(127.0, off.y), e))));
+      out[2] = static_cast<uint8_t>(report_trunc(__dadd_rn(127.0, __ddiv_rn(__dmul_rn(127.0, off.z), e))));
+    }
+    img[q] = out[0];
+    img[q + 1] = out[1];
+    img[q + 2] = out[2];
+  }
+}
+
+// :945-973: line i = iy * nx + ix of the .obj models is the pixel (min_x + ix * step, min_y + iy * step);
+// obj[12 i ..]: point_a, point_b, closest point, origin
+__global__ void line_obj_kernel(CamDev c, const double* __restrict__ lines, double cx, double cy, double cz, int step,
+                                int nx, int64_t n_obj, double* __restrict__ obj) {
+  const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (i >= n_obj) return;
+  const int rw = c.max_x - c.min_x + 1;
+  const int64_t n = static_cast<int64_t>(rw) * (c.max_y - c.min_y + 1);
+  const int64_t p = (i / nx) * step * static_cast<int64_t>(rw) + (i % nx) * step;
+  d3 o, d, closest;
+  load_line(lines, n, p, o, d);
+  const d3 off = line_offset(o, d, mk3(cx, cy, cz), closest);
+  const double half = fmax(10.0, __dmul_rn(10.0, line_norm(off)));  // std::max<double>(10, 10 * norm)
+  const d3 hd = mk3(__dmul_rn(half, d.x), __dmul_rn(half, d.y), __dmul_rn(half, d.z));
+  double* out = obj + 12 * i;
+  out[0] = __dadd_rn(closest.x, hd.x);
+  out[1] = __dadd_rn(closest.y, hd.y);
+  out[2] = __dadd_rn(closest.z, hd.z);
+  out[3] = __dsub_rn(closest.x, hd.x);
+  out[4] = __dsub_rn(closest.y, hd.y);
+  out[5] = __dsub_rn(closest.z, hd.z);
+  out[6] = closest.x;
+  out[7] = closest.y;
+  out[8] = closest.z;
+  out[9] = o.x;
+  out[10] = o.y;
+  out[11] = o.z;
+}
+
+void launch_line_outputs(const CamDev& c, const double center[3], const LineOffsetsDev& d, int obj_step, int nx,
+                         int64_t n_obj, cudaStream_t s) {
+  const int64_t n = static_cast<int64_t>(c.max_x - c.min_x + 1) * (c.max_y - c.min_y + 1);
+  cudaMemsetAsync(d.extent, 0, sizeof(unsigned long long), s);  // the bits of +0.0
+  line_distances_kernel<<<static_cast<unsigned>((n + kReportThreads - 1) / kReportThreads), kReportThreads, 0, s>>>(
+      n, d.lines, center[0], center[1], center[2], d.mag, d.extent);
+  launch_report_statistics(1, d.range, d.mag, d.stat_partial, d.select_hist, d.stats, s);
+  if (d.offsets || d.image) {
+    const dim3 grid((c.width + kLineTileX - 1) / kLineTileX, (c.height + kLineTileY - 1) / kLineTileY);
+    line_offsets_image_kernel<<<grid, dim3(kLineTileX, kLineTileY), 0, s>>>(c, d.lines, center[0], center[1], center[2],
+                                                                            d.extent, d.offsets, d.image);
+  }
+  if (d.obj && n_obj > 0)
+    line_obj_kernel<<<static_cast<unsigned>((n_obj + 127) / 128), 128, 0, s>>>(c, d.lines, center[0], center[1], center[2],
+                                                                                obj_step, nx, n_obj, d.obj);
+}
+
+// ------------------------------------------------------------------------------------------
 // report images (CreateCalibrationReportForCamera, APP/calibration_report.cc:713-838)
 // ------------------------------------------------------------------------------------------
 // Error maps (:354-603): every feature site owns its Voronoi cell; a pixel's colour is the sum over the

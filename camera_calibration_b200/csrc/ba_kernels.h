@@ -59,6 +59,15 @@ int report_partial_size(int n_cameras);
 // on the device
 void launch_compare_models(const CamDev& a, const double* ga, const CamDev& b, const double* gb, const CompareDev& d,
                            cudaStream_t s);
+// centre-point analysis of a non-central camera (b200ba_line_offsets); intr on the device. launch_line_pass stores
+// the line of every calibrated-rectangle pixel in d.lines; launch_line_system sums (mode 0) the cost, (1) + b,
+// (2) + H at the centre c into d.sums; launch_line_outputs computes the distances and their statistics, the
+// extent, and whichever of d.offsets / d.image / d.obj is set (obj: every obj_step-th pixel, nx per row, n_obj)
+void launch_line_pass(const CamDev& c, const double* intr, const LineOffsetsDev& d, cudaStream_t s);
+void launch_line_system(int mode, int64_t n, const double c[3], const LineOffsetsDev& d, cudaStream_t s);
+int line_system_partial_size();
+void launch_line_outputs(const CamDev& c, const double center[3], const LineOffsetsDev& d, int obj_step, int nx,
+                         int64_t n_obj, cudaStream_t s);
 // re-projection errors of every observation into r.err / r.mag (the first kernel of launch_calibration_report)
 void launch_report_errors(const ProblemDev& pb, int n_cameras, const StateDev& st, const ReportDev& r, cudaStream_t s);
 // Voronoi coverage rendering of n sites (quarter-pixel int2, kVoronoiNoSite.x = skipped) with nch = 3 or 6 float

@@ -559,6 +559,44 @@ def GridPointLocationsImage(model: CentralGenericModel) -> np.ndarray:
     return img
 
 
+def _obj_number(v: float) -> str:
+    """std::ostream << double with setprecision(14), NaN written ``nan`` whatever its sign bit (as the C++ writer)."""
+    return "nan" if v != v else _g(v)
+
+
+def WriteLineVisualizationOBJ(base_path: str, obj_lines) -> bool:
+    """The three .obj models of a non-central camera (APP/calibration_report.cc:932-981) from the [n, 4, 3] lines
+    point_a, point_b, closest point, origin of ``api.LineOffsets``: ``<base>_line_visualization.obj`` (a - b),
+    ``<base>_line_visualization_cutoff.obj`` (a - closest point) and ``<base>_line_visualization_origins.obj``
+    (a, b, origin; the segment a - b), each with its ``v`` lines followed by its ``l`` lines, numbers with 14
+    significant digits. The C++ writer (b200ba_pipeline.hpp) produces the same bytes. Returns False if a file cannot
+    be written."""
+    lines = np.asarray(obj_lines, dtype=np.float64).reshape(-1, 4, 3)
+
+    def v(p):
+        return f"v {_obj_number(p[0])} {_obj_number(p[1])} {_obj_number(p[2])}\n"
+
+    full, cutoff, origins = [], [], []
+    for a, b, closest, origin in lines:
+        full += [v(a), v(b)]
+        cutoff += [v(a), v(closest)]
+        origins += [v(a), v(b), v(origin)]
+    vertex_index = 1  # vertex indexing starts at 1 in .obj files
+    for _ in range(len(lines)):
+        full.append(f"l {vertex_index} {vertex_index + 1}\n")
+        cutoff.append(f"l {vertex_index} {vertex_index + 1}\n")
+        origins.append(f"l {3 * (vertex_index // 2) + 1} {3 * (vertex_index // 2) + 2}\n")
+        vertex_index += 2
+    try:
+        for suffix, text in (("_line_visualization.obj", full), ("_line_visualization_cutoff.obj", cutoff),
+                             ("_line_visualization_origins.obj", origins)):
+            with open(base_path + suffix, "w") as f:
+                f.write("".join(text))
+    except OSError:
+        return False
+    return True
+
+
 def WriteFittingInfoFile(path: str, report) -> bool:
     """``<base>_fitting_info.txt`` (APP/fitting_report.h:186-200) from a ``cabi.FittingReport``. The
     reference sorts its error vector for the median; here the median comes in (it is computed on the

@@ -381,14 +381,17 @@ def BundleAdjustment(state_directory: str, model_input_directory: str, model_out
     return 0
 
 
-def CreateCalibrationReport(dataset: Dataset, state: BAState, report_base_path: str, visualizations: bool = False):
+def CreateCalibrationReport(dataset: Dataset, state: BAState, report_base_path: str, visualizations: bool = False,
+                            line_offsets: bool = False):
     """calibration_report.cc:83-98: the per-camera numbers of CreateCalibrationReportForCamera (:713-817)
     computed on the device (``b200ba_calibration_report``) and written to ``<report_base_path>_camera<i>_info.txt``
     (WriteReportInfoFile, :648-710). With ``visualizations``, every camera also gets the reference's images
     (``b200ba_report_images``): ``_observation_directions.png`` (central- and non-central-generic cameras; OpenCV
     cameras have no device un-projection), ``_errors_histogram.png``, ``_error_directions.png``,
-    ``_error_magnitudes.png`` and, for central-generic cameras, ``_grid_point_locations.png``; the C++ pipeline
-    writes the same bytes. Returns one ``cabi.CameraReport`` per camera."""
+    ``_error_magnitudes.png`` and, for central-generic cameras, ``_grid_point_locations.png``. With ``line_offsets``,
+    every non-central camera also gets the centre-point analysis of :839-982 (``api.LineOffsets`` on
+    ``state.intrinsics[i]``): ``_line_offsets.png`` and the three ``_line_visualization*.obj`` models. The C++
+    pipeline writes the same bytes. Returns one ``cabi.CameraReport`` per camera."""
     import os
     from . import io
     reports, _, _ = api.CalibrationReports(dataset, state)
@@ -411,6 +414,14 @@ def CreateCalibrationReport(dataset: Dataset, state: BAState, report_base_path: 
         io.WritePNG(base + "_error_magnitudes.png", imgs["error_magnitudes"])
         if isinstance(cam, CentralGenericModel):
             io.WritePNG(base + "_grid_point_locations.png", io.GridPointLocationsImage(cam))
+    for c in range(len(reports) if line_offsets else 0):
+        cam = state.intrinsics[c]
+        if not isinstance(cam, api.NoncentralGenericModel):
+            continue
+        base = f"{report_base_path}_camera{c}"
+        _, image, _, obj_lines, _ = api.LineOffsets(cam)
+        if not io.WritePNG(base + "_line_offsets.png", image) or not io.WriteLineVisualizationOBJ(base, obj_lines):
+            raise OSError(f"CreateCalibrationReport: cannot write the line-offset files of {base}")
     return reports
 
 

@@ -355,6 +355,38 @@ B200BA_API int b200ba_compare_models(int device, const b200ba_camera* cam_a, con
                                      const b200ba_camera* cam_b, const double* intr_b, b200ba_fitting_report* report,
                                      double* direction_errors, double* reprojection_errors, double* device_ms);
 
+/* ---- centre-point analysis of a non-central camera: the NoncentralGenericModel branch of
+ * CreateCalibrationReportForCamera (APP/calibration_report.cc:839-982, with CenterPointCostFunction of :56-80).
+ *   1. every pixel (x + 0.5f, y + 0.5f) of the calibrated area is un-projected to a line (o, d) (:847-856);
+ *   2. the centre c closest to all lines: LMOptimizer<double>::Optimize(c = 0, max_iteration_count = 100,
+ *      max_lm_attempts = 10, init_lambda = -1, init_lambda_factor = 0.001f) (:858-867) with two residuals per line,
+ *      t1 . (c - o) and t2 . (c - o) in the line's tangent frame, quadratic loss (cost = 1/2 sum r^2);
+ *   3. per line the offset closest - c, closest = o + (d . (c - o)) d, its norm (the line distance) and the largest
+ *      |component| (:869-902); the statistics the reference computes but does not print (:904-911) are returned here;
+ *   4. _line_offsets.png (:913-930): 127 + 127 * offset_k / max_line_offset_extent per channel in double, converted to
+ *      u8 as x86-64 does (truncation to int32, low byte); black where there is no line;
+ *   5. the lines of the .obj models (:932-973): every obj_step-th pixel from calibration_min in x and in y, half
+ *      = max(10, 10 |closest - c|), point_a = closest + half d, point_b = closest - half d.
+ * The model must be non-central-generic with grids of at least 4 x 4 and a calibrated area inside the image. */
+typedef struct b200ba_line_offsets_report {
+  double center[3];
+  int64_t line_count;                      /* calibrated-area pixels whose Unproject succeeds */
+  double line_distance_sum, line_distance_max, line_distance_median;  /* median NaN if count == 0 */
+  double max_line_offset_extent;           /* max |component| of the offsets; 0 if none */
+  double initial_cost, final_cost;         /* of the centre-point fit (quadratic loss: 1/2 sum r^2) */
+  int32_t num_iterations_performed, lm_attempts;
+} b200ba_line_offsets_report;
+/* Stand-alone (allocates, computes, frees); intrinsics [6 * grid_width * grid_height] (direction grid, then point
+ * grid) are not modified. image (nullable): [h*w*3] RGB row-major, _line_offsets.png. offsets (nullable): [3*w*h]
+ * row-major (y, x), closest point on the line - centre, NaN where there is no line. obj_lines (nullable):
+ * [n_obj][4][3] point_a, point_b, closest point, origin, in the reference's order (y outer, x inner); it must hold
+ * ((max_x - min_x) / obj_step + 1) * ((max_y - min_y) / obj_step + 1) lines, and that count is written to n_obj
+ * (nullable unless obj_lines is given). device_ms (nullable): device time of the analysis. Returns 2 for a bad
+ * argument, 3 without a device. */
+B200BA_API int b200ba_line_offsets(int device, const b200ba_camera* cam, const double* intrinsics,
+                                   b200ba_line_offsets_report* report, uint8_t* image, double* offsets, int32_t obj_step,
+                                   double* obj_lines, int64_t* n_obj, double* device_ms);
+
 /* ---- multi-GPU: imagesets sharded over ranks, one NCCL all-reduce per H/b build --- */
 #define B200BA_NCCL_UNIQUE_ID_BYTES 128
 B200BA_API int b200ba_nccl_unique_id(uint8_t id[B200BA_NCCL_UNIQUE_ID_BYTES]);

@@ -467,16 +467,48 @@ inline std::vector<uint8_t> GridPointLocationsImage(const CentralGenericModel& m
   return img;
 }
 
+// calibration_report.cc:932-981 -- the three .obj models of a non-central camera from the n_obj lines
+// [n_obj][4][3] point_a, point_b, closest point, origin of b200ba_line_offsets: <base>_line_visualization.obj (a - b),
+// <base>_line_visualization_cutoff.obj (a - closest point) and <base>_line_visualization_origins.obj (a, b, origin;
+// the segment a - b), each with its "v" lines followed by its "l" lines, numbers with setprecision(14) (NaN written
+// "nan" as in report_number). io.py's WriteLineVisualizationOBJ writes the same bytes. Returns false if a file cannot
+// be opened.
+inline bool WriteLineVisualizationOBJ(const std::string& base_path, const double* obj_lines, int64_t n_obj) {
+  std::ofstream obj_stream(base_path + "_line_visualization.obj", std::ios::out);
+  std::ofstream obj_stream_cutoff(base_path + "_line_visualization_cutoff.obj", std::ios::out);
+  std::ofstream obj_stream_origins(base_path + "_line_visualization_origins.obj", std::ios::out);
+  if (!obj_stream || !obj_stream_cutoff || !obj_stream_origins) return false;
+  using detail::report_number;
+  auto v = [](const double* p) {
+    return "v " + report_number(p[0]) + " " + report_number(p[1]) + " " + report_number(p[2]) + "\n";
+  };
+  for (int64_t i = 0; i < n_obj; ++i) {
+    const double* line = obj_lines + 12 * i;
+    obj_stream << v(line) << v(line + 3);
+    obj_stream_cutoff << v(line) << v(line + 6);
+    obj_stream_origins << v(line) << v(line + 3) << v(line + 9);
+  }
+  int64_t vertex_index = 1;  // vertex indexing starts at 1 in .obj files
+  for (int64_t i = 0; i < n_obj; ++i) {
+    obj_stream << "l " << vertex_index << " " << (vertex_index + 1) << "\n";
+    obj_stream_cutoff << "l " << vertex_index << " " << (vertex_index + 1) << "\n";
+    obj_stream_origins << "l " << (3 * (vertex_index / 2) + 1) << " " << (3 * (vertex_index / 2) + 2) << "\n";
+    vertex_index += 2;
+  }
+  return static_cast<bool>(obj_stream) && static_cast<bool>(obj_stream_cutoff) && static_cast<bool>(obj_stream_origins);
+}
+
 // calibration_report.cc:83-98: the numbers of CreateCalibrationReportForCamera (:713-817) for every camera, computed
 // in the library (b200ba_calibration_report) on the flattening that OptimizeJointly uses, and written to
 // <report_base_path>_camera<i>_info.txt. With visualizations, every camera also gets the reference's images
 // (b200ba_report_images): _observation_directions.png (central- and non-central-generic cameras; OpenCV cameras have
 // no device un-projection), _errors_histogram.png, _error_directions.png, _error_magnitudes.png and, for
-// central-generic cameras, _grid_point_locations.png. Neither argument is modified. Returns the per-camera numbers;
-// throws on a library error.
+// central-generic cameras, _grid_point_locations.png. With line_offsets, every non-central camera also gets the
+// centre-point analysis of :839-982 (b200ba_line_offsets): _line_offsets.png and the three _line_visualization*.obj
+// models. Neither argument is modified. Returns the per-camera numbers; throws on a library error.
 inline std::vector<b200ba_camera_report> CreateCalibrationReport(const Dataset& dataset, const BAState& state,
                                                                  const std::string& report_base_path,
-                                                                 bool visualizations = false) {
+                                                                 bool visualizations = false, bool line_offsets = false) {
   detail::Flat f;
   // flatten() only reads; it takes mutable references because flat_intrinsics() hands out the model's storage
   detail::flatten(const_cast<Dataset&>(dataset), const_cast<BAState*>(&state), &f);
@@ -540,6 +572,23 @@ inline std::vector<b200ba_camera_report> CreateCalibrationReport(const Dataset& 
                              r.reprojection_error_count, r.reprojection_error_sum, r.reprojection_error_max,
                              r.reprojection_error_median, r.biasedness))
       throw std::runtime_error("CreateCalibrationReport: cannot write " + path);
+  }
+  for (size_t c = 0; line_offsets && c < reports.size(); ++c) {
+    const CameraModel& cam = *state.intrinsics[c];
+    if (cam.type() != CameraModel::Type::NoncentralGeneric) continue;
+    constexpr int kStepForOBJ = 20;  // :933
+    const int rw = cam.calibration_max_x() - cam.calibration_min_x() + 1, rh = cam.calibration_max_y() - cam.calibration_min_y() + 1;
+    int64_t n_obj = (rw >= 1 && rh >= 1) ? static_cast<int64_t>((rw - 1) / kStepForOBJ + 1) * ((rh - 1) / kStepForOBJ + 1) : 0;
+    std::vector<uint8_t> image(3 * static_cast<size_t>(cam.width()) * cam.height());
+    std::vector<double> obj(12 * static_cast<size_t>(std::max<int64_t>(n_obj, 1)));
+    b200ba_line_offsets_report rep{};
+    if (b200ba_line_offsets(-1, &f.cams[c], f.intr[c], &rep, image.data(), nullptr, kStepForOBJ, obj.data(), &n_obj,
+                            nullptr) != 0)
+      throw std::runtime_error(std::string("b200ba_line_offsets: ") + b200ba_last_error(nullptr));
+    const std::string base = report_base_path + "_camera" + std::to_string(c);
+    if (!WritePNG(base + "_line_offsets.png", cam.width(), cam.height(), 3, image.data()) ||
+        !WriteLineVisualizationOBJ(base, obj.data(), n_obj))
+      throw std::runtime_error("CreateCalibrationReport: cannot write the line-offset files of " + base);
   }
   return reports;
 }

@@ -10,6 +10,7 @@ import numpy as np
 import pytest
 
 from camera_calibration_b200 import api, cabi, synthetic
+from tests import helpers
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -73,6 +74,36 @@ def test_fails_loudly_without_gpu():
         api.BundleAdjuster(sp.problem)
     with pytest.raises(api.B200BAError):
         api.schur_solve(2, np.zeros((1, 2, 2)), np.zeros((2, 1)), np.ones((1, 1)), [0, 0], [1])
+    # every stand-alone entry point, called with valid arguments, passes its argument checks and then fails with 3
+    lib = _lib()
+    d = lambda a: a.ctypes.data_as(C.POINTER(C.c_double))  # noqa: E731
+    central = helpers.make_camera(cabi.MODEL_CENTRAL_GENERIC, 64, 48, (0, 0, 63, 47), 6, 5)
+    noncentral = helpers.make_camera(cabi.MODEL_NONCENTRAL_GENERIC, 64, 48, (0, 0, 63, 47), 6, 5)
+    grid = helpers.xy1_grid(6, 5).reshape(-1)
+    lines = np.concatenate([grid, np.zeros_like(grid)])
+    spd, rhs, x = np.eye(2), np.ones(2), np.zeros(2)
+    points, pixels, out3, ok = np.ones((1, 3)), np.full((1, 2), 8.0), np.zeros((1, 3)), np.zeros(1, np.int32)
+    okp = ok.ctypes.data_as(C.POINTER(C.c_int32))
+    sites, colors, image = np.array([[8, 8]], np.int32), np.ones((1, 3), np.float32), np.zeros((8, 8, 3), np.uint8)
+    calls = {
+        "dense_cholesky_solve": lambda: lib.b200ba_dense_cholesky_solve(-1, 2, 128, d(spd), d(rhs), d(x), None, None),
+        "project": lambda: lib.b200ba_project(-1, C.byref(central), d(grid), 1, d(points), d(pixels), okp),
+        "unproject": lambda: lib.b200ba_unproject(-1, C.byref(central), d(grid), 1, d(pixels), d(out3), d(out3), okp),
+        "fit_directions": lambda: lib.b200ba_fit_directions(-1, 6, 5, d(grid.copy()), 1, d(np.full((1, 2), 1.5)),
+                                                            d(points), 1, C.byref(cabi.FitReport())),
+        "compare_models": lambda: lib.b200ba_compare_models(-1, C.byref(central), d(grid), C.byref(central), d(grid),
+                                                            C.byref(cabi.FittingReport()), None, None, None),
+        "render_voronoi": lambda: lib.b200ba_render_voronoi(-1, 8, 8, 1, sites.ctypes.data_as(C.POINTER(C.c_int32)),
+                                                            colors.ctypes.data_as(C.POINTER(C.c_float)),
+                                                            image.ctypes.data_as(C.POINTER(C.c_uint8)), None),
+        "line_offsets": lambda: lib.b200ba_line_offsets(-1, C.byref(noncentral), d(lines),
+                                                        C.byref(cabi.LineOffsetsReport()), None, None, 20, None, None,
+                                                        None),
+    }
+    for name, call in calls.items():
+        rc = call()
+        msg = lib.b200ba_last_error(None).decode()
+        assert rc == 3 and "no CUDA device" in msg, (name, rc, msg)
 
 
 def test_missing_library_is_an_error(tmp_path):

@@ -3,8 +3,8 @@
 // The reduced system of the Schur-complement solve (LV/lm_optimizer.h:1246-1369) is formed and
 // factorised with the kernels of this file instead of library calls:
 //
-//   dgemm_nt_kernel     C (+)= alpha * A B^T on 128 x 128 tiles, FP64 `mma.sync.m8n8k4` (SASS DMMA.8x8x4),
-//                       operands staged through shared memory
+//   dgemm_nt_kernel     C (+)= alpha * A B^T on 128 x 64 (default) or 128 x 128 tiles, 32 x 32 warp tiles, FP64
+//                       `mma.sync.m16n8k4` (SASS DMMA.16x8x4), operands staged through shared memory
 //                       by a 4-stage cp.async pipeline. One kernel, three uses:
 //                         * LOWER + plain epilogue: trailing update S22 -= L21 L21^T of the blocked Cholesky
 //                           (the reference factors with Eigen's LDLT, LV/lm_optimizer.h:1361);
@@ -52,10 +52,13 @@ template <int N>
 __device__ __forceinline__ void cp_async_wait() {
   asm volatile("cp.async.wait_group %0;\n" ::"n"(N));
 }
-__device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b) {
-  asm("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
-      : "+d"(c0), "+d"(c1)
-      : "d"(a), "d"(b));
+// One m16n8k4 FP64 MMA (SASS DMMA.16x8x4: twice the FMAs per instruction of m8n8k4, which H100 issues at the
+// same rate, so half the tensor pipe's peak is out of reach with m8n8k4). Fragments (lane = 4 lr + lc):
+// a0 = A(m = lr, k = lc), a1 = A(lr + 8, lc), b = B(n = lr, k = lc), c[v0 + 2 v1] = C(m = lr + 8 v1, n = 2 lc + v0).
+__device__ __forceinline__ void dmma1684(double& c0, double& c1, double& c2, double& c3, double a0, double a1, double b) {
+  asm("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};\n"
+      : "+d"(c0), "+d"(c1), "+d"(c2), "+d"(c3)
+      : "d"(a0), "d"(a1), "d"(b));
 }
 
 // Loader of one operand's BK x W tiles (pitch W + 4): rows k0 .. k0 + BK of the k-strided matrix X (leading
@@ -73,18 +76,15 @@ struct TileLoader {
   static constexpr int KS8 = THREADS / W;        // ... (unaligned path)
   static constexpr int Q16 = BK / KS16, Q8 = BK / KS8;
   static_assert(THREADS % CH == 0 && THREADS % W == 0 && BK % KS16 == 0 && BK % KS8 == 0, "tile / thread count mismatch");
-  // all chunks of a thread sit in the same column(s) and KS rows apart: one pointer, one byte count
+  // all chunks of a thread sit in the same column(s) and KS rows apart: one pointer, one byte count. X and ldx
+  // are not kept: issue() takes them from the kernel arguments, which stay in the constant bank instead of
+  // holding six registers through the main loop.
   const double* src;   // chunk of row k0 + kk0
-  const double* base;
-  int64_t row_step;    // KS * ldx
-  int64_t tile_step;   // BK * ldx
   int off0, kk0, bytes;
   bool aligned;
 
   __device__ __forceinline__ void init(const double* __restrict__ X, int64_t ldx, int rows, int i0, bool al) {
     aligned = al;
-    base = X;
-    tile_step = static_cast<int64_t>(BK) * ldx;
     int i;
     if (al) {
       kk0 = threadIdx.x / CH;
@@ -92,36 +92,34 @@ struct TileLoader {
       i = i0 + 2 * ch;
       off0 = kk0 * LD + 2 * ch;
       bytes = (i + 1 < rows) ? 16 : ((i < rows) ? 8 : 0);
-      row_step = static_cast<int64_t>(KS16) * ldx;
     } else {
       kk0 = threadIdx.x / W;
       const int ii = threadIdx.x % W;
       i = i0 + ii;
       off0 = kk0 * LD + ii;
       bytes = (i < rows) ? 8 : 0;
-      row_step = static_cast<int64_t>(KS8) * ldx;
     }
     src = X + static_cast<int64_t>(kk0) * ldx + min(i, max(rows - 1, 0));
   }
-  // copies the tile whose first row is k0 into dst and advances to the next tile
-  __device__ __forceinline__ void issue(double* dst, int k0, int K) {
+  // copies the tile whose first row is k0 into dst and advances to the next tile (X, ldx: those of init())
+  __device__ __forceinline__ void issue(double* dst, int k0, int K, const double* __restrict__ X, int64_t ldx) {
     const double* p = src;
     if (aligned) {
 #pragma unroll
       for (int q = 0; q < Q16; ++q) {
         const int nb = (k0 + kk0 + q * KS16 < K) ? bytes : 0;
-        cp_async16(dst + off0 + q * KS16 * LD, nb ? p : base, nb);
-        p += row_step;
+        cp_async16(dst + off0 + q * KS16 * LD, nb ? p : X, nb);
+        p += KS16 * ldx;
       }
     } else {
 #pragma unroll
       for (int q = 0; q < Q8; ++q) {
         const int nb = (k0 + kk0 + q * KS8 < K) ? bytes : 0;
-        cp_async8(dst + off0 + q * KS8 * LD, nb ? p : base, nb);
-        p += row_step;
+        cp_async8(dst + off0 + q * KS8 * LD, nb ? p : X, nb);
+        p += KS8 * ldx;
       }
     }
-    src += tile_step;
+    src += BK * ldx;
   }
 };
 
@@ -190,8 +188,8 @@ __global__ void __launch_bounds__(gemm_threads(BN_), BN_ == 64 ? 2 : 1) dgemm_nt
 #pragma unroll
     for (int s = 0; s < STAGES - 1; ++s) {
       if (s < nk) {
-        la.issue(As + s * BK * LDT, s * BK, g.K);
-        if (!same) lb.issue(Bs + s * BK * LDB, s * BK, g.K);
+        la.issue(As + s * BK * LDT, s * BK, g.K, g.A, g.lda);
+        if (!same) lb.issue(Bs + s * BK * LDB, s * BK, g.K, g.B, g.ldb);
       }
       cp_async_commit();
     }
@@ -203,8 +201,8 @@ __global__ void __launch_bounds__(gemm_threads(BN_), BN_ == 64 ? 2 : 1) dgemm_nt
         const int nt = kt + STAGES - 1;
         if (nt < nk) {
           const int s = nt % STAGES;
-          la.issue(As + s * BK * LDT, nt * BK, g.K);
-          if (!same) lb.issue(Bs + s * BK * LDB, nt * BK, g.K);
+          la.issue(As + s * BK * LDT, nt * BK, g.K, g.A, g.lda);
+          if (!same) lb.issue(Bs + s * BK * LDB, nt * BK, g.K, g.B, g.ldb);
         }
         cp_async_commit();
       }
@@ -213,17 +211,21 @@ __global__ void __launch_bounds__(gemm_threads(BN_), BN_ == 64 ? 2 : 1) dgemm_nt
       const int ldb_s = same ? LDT : LDB;
 #pragma unroll
       for (int ks = 0; ks < BK / 4; ++ks) {
-        double af[4], bf[4];
+        // af[i] = A(row wm + 8 i + lr, k = 4 ks + lc), bf = B(column wn + 8 j + lr, same k). Rows 16 b .. 16 b + 15
+        // of the warp tile are accumulator rows 2 b (m = lr) and 2 b + 1 (m = lr + 8): one m16n8k4 per (b, j).
+        double af[4];
         const double* ap = a_s + (ks * 4 + lc) * LDT + wm + lr;
         const double* bp = b_s + (ks * 4 + lc) * ldb_s + wn + lr;
 #pragma unroll
         for (int i = 0; i < 4; ++i) af[i] = ap[8 * i];
 #pragma unroll
-        for (int j = 0; j < 4; ++j) bf[j] = bp[8 * j];
+        for (int j = 0; j < 4; ++j) {
+          const double bf = bp[8 * j];
 #pragma unroll
-        for (int i = 0; i < 4; ++i)
-#pragma unroll
-          for (int j = 0; j < 4; ++j) dmma884(acc[i][j][0], acc[i][j][1], af[i], bf[j]);
+          for (int b = 0; b < 2; ++b)
+            dmma1684(acc[2 * b][j][0], acc[2 * b][j][1], acc[2 * b + 1][j][0], acc[2 * b + 1][j][1], af[2 * b],
+                     af[2 * b + 1], bf);
+        }
       }
     }
     cp_async_wait<0>();

@@ -1041,3 +1041,29 @@ def LineOffsets(model: CameraModel, obj_step: int = 20, device: int = -1):
                                    int(obj_step), _dp(obj), C.byref(n_obj), C.byref(ms)))
     assert n_obj.value == n_expected, (n_obj.value, n_expected)
     return report, image, offsets, obj[:n_obj.value], ms.value
+
+
+def LocalizationAccuracy(gt_model: CameraModel, compared_model: CameraModel, trials: int = 10000, seed: int = 0,
+                         with_trials: bool = False, device: int = -1):
+    """The localization accuracy test (APP/tools/localization_accuracy_test.cc:47-131) on the device
+    (``b200ba_localization_accuracy``; the sampling rule, the random stream and the pose fit are specified in
+    include/b200ba.h). Returns (report, trials, device_ms): a ``cabi.LocalizationReport`` (errors in metres); with
+    ``with_trials`` a dict of the per-trial arrays ``errors`` [trials] float32 (camera-centre offsets),
+    ``poses`` [trials, 6] (t, Cayley vector c) and ``samples`` [trials, 15, 3] float32 (pixel x, y and distance of
+    every point), else None."""
+    lib = cabi.load_library()
+    cg, cc = gt_model.c_camera(), compared_model.c_camera()
+    ig = np.ascontiguousarray(gt_model.flat_intrinsics(), dtype=np.float64)
+    ic = np.ascontiguousarray(compared_model.flat_intrinsics(), dtype=np.float64)
+    arrays = None
+    if with_trials:
+        arrays = {"errors": np.empty(trials, np.float32), "poses": np.empty((trials, 6)),
+                  "samples": np.empty((trials, 15, 3), np.float32)}
+    fp = lambda a: a.ctypes.data_as(C.POINTER(C.c_float))
+    report = cabi.LocalizationReport()
+    ms = C.c_double(0)
+    _check(lib.b200ba_localization_accuracy(device, C.byref(cg), _dp(ig), C.byref(cc), _dp(ic), int(trials), int(seed),
+                                            C.byref(report), None if arrays is None else fp(arrays["errors"]),
+                                            None if arrays is None else _dp(arrays["poses"]),
+                                            None if arrays is None else fp(arrays["samples"]), C.byref(ms)))
+    return report, arrays, ms.value

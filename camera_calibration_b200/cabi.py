@@ -228,6 +228,19 @@ class FittingReport(C.Structure):
     ]
 
 
+class LocalizationReport(C.Structure):
+    """b200ba_localization_report: the localization accuracy test of one calibration against another."""
+    _fields_ = [
+        ("trial_count", C.c_int64),
+        ("average_error", C.c_double),
+        ("median_error", C.c_double),
+        ("max_error", C.c_double),
+        ("total_iterations", C.c_int64),
+        ("redraws", C.c_int64),
+        ("max_iterations", C.c_int32),
+    ]
+
+
 class LineOffsetsReport(C.Structure):
     """b200ba_line_offsets_report: the centre-point analysis of a non-central camera."""
     _fields_ = [
@@ -413,6 +426,9 @@ SYMBOLS = {
                                         _D, _D, _D]),
     "b200ba_line_offsets": (C.c_int, [C.c_int, C.POINTER(Camera), _D, C.POINTER(LineOffsetsReport), C.POINTER(C.c_uint8),
                                       _D, C.c_int32, _D, C.POINTER(C.c_int64), _D]),
+    "b200ba_localization_accuracy": (C.c_int, [C.c_int, C.POINTER(Camera), _D, C.POINTER(Camera), _D, C.c_int64,
+                                               C.c_uint64, C.POINTER(LocalizationReport), C.POINTER(C.c_float), _D,
+                                               C.POINTER(C.c_float), _D]),
     "b200ba_nccl_unique_id": (C.c_int, [C.POINTER(C.c_uint8)]),
     "b200ba_comm_init": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint8), C.c_int, C.c_int]),
     "b200ba_get_timings": (C.c_int, [C.c_void_p, C.POINTER(Timings)]),

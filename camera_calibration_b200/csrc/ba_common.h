@@ -145,6 +145,23 @@ struct CompareDev {
   ReportCam* stats;             // count / sum / max / median
 };
 
+// Localization accuracy test (b200ba_localization_accuracy): device buffers of one call.
+constexpr int kLocPoints = 15;        // kPointCount (localization_accuracy_test.cc:77)
+constexpr int kLocMaxDraws = 4096;    // draws per point before the call gives up (return code 4)
+struct LocalizationDev {
+  double* p;                   // [trials * 15 * 3] ground-truth points
+  double* f;                   // [trials * 15 * 3] compared bearings
+  float* samples;              // [trials * 15 * 3] x, y, distance, or NULL
+  double* poses;               // [trials * 6] t, c, or NULL
+  double* mag;                 // [trials] (double)(float)|t|
+  unsigned long long* counts;  // [3] redraws, total iterations, max iterations
+  int* capped;                 // 1 if some point was not drawn within kLocMaxDraws
+  int64_t* range;              // [2] {0, trials}: the one range of launch_report_statistics
+  double* partial;             // report_partial_size(1)
+  unsigned int* select_hist;   // [256]
+  ReportCam* stats;            // count / sum / max / median of the errors
+};
+
 // Centre-point analysis of a non-central camera (b200ba_line_offsets): device buffers of one call. The n lines are
 // those of the pixels of the calibrated rectangle, p = (y - min_y) * rw + (x - min_x).
 constexpr int kLineSums = 10;  // per LM pass: cost, b (3), H (6: 00 01 02 11 12 22)

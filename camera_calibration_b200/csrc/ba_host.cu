@@ -2593,6 +2593,109 @@ int b200ba_compare_models(int device, const b200ba_camera* cam_a, const double* 
   return cs.rc;
 }
 
+// The localization accuracy test (APP/tools/localization_accuracy_test.cc:47-131). The argument checks come first
+// and touch no CUDA state. The sampling kernel runs first; a point that is not drawn within kLocMaxDraws ends the call
+// with 4 before any fit, where the reference would loop forever.
+int b200ba_localization_accuracy(int device, const b200ba_camera* gt_cam, const double* gt_intr, const b200ba_camera* cam,
+                                 const double* intr, int64_t trials, uint64_t seed, b200ba_localization_report* report,
+                                 float* errors, double* poses, float* samples, double* device_ms) {
+  if (!gt_cam || !gt_intr || !cam || !intr || !report) {
+    g_create_error = "b200ba_localization_accuracy: a required argument is NULL";
+    return 2;
+  }
+  if (gt_cam->model_type != B200BA_MODEL_CENTRAL_GENERIC || cam->model_type != B200BA_MODEL_CENTRAL_GENERIC) {
+    g_create_error = "b200ba_localization_accuracy: the localization accuracy test is only implemented for "
+                     "CentralGenericModel";
+    return 2;
+  }
+  if (gt_cam->width != cam->width || gt_cam->height != cam->height || gt_cam->width < 1 || gt_cam->height < 1) {
+    g_create_error = "b200ba_localization_accuracy: The ground truth and compared camera models do not have the same "
+                     "image size.";
+    return 2;
+  }
+  if (gt_cam->grid_width < 4 || gt_cam->grid_height < 4 || cam->grid_width < 4 || cam->grid_height < 4) {
+    g_create_error = "b200ba_localization_accuracy: a grid is smaller than 4 x 4";
+    return 2;
+  }
+  if (trials < 1 || trials > (int64_t(1) << 32)) {
+    g_create_error = "b200ba_localization_accuracy: trials must be in [1, 2^32]";
+    return 2;
+  }
+  // pixels are drawn in [0, w] x [0, h]; a calibrated area is [min, max + 1) in x and y
+  const double lo_x = std::max({0.0, double(gt_cam->calibration_min_x), double(cam->calibration_min_x)});
+  const double lo_y = std::max({0.0, double(gt_cam->calibration_min_y), double(cam->calibration_min_y)});
+  const double hi_x = std::min({double(gt_cam->width), gt_cam->calibration_max_x + 1.0, cam->calibration_max_x + 1.0});
+  const double hi_y = std::min({double(gt_cam->height), gt_cam->calibration_max_y + 1.0, cam->calibration_max_y + 1.0});
+  if (!(lo_x < hi_x && lo_y < hi_y)) {
+    g_create_error = "b200ba_localization_accuracy: the calibrated areas of the two models do not intersect in the image";
+    return 2;
+  }
+  CallScope cs(&g_create_error);
+  if (int rc = cs.use_device(device)) return rc;
+  CamDev cg{}, cc{};
+  fill_camdev(*gt_cam, &cg);
+  fill_camdev(*cam, &cc);
+  const int64_t n = trials * kLocPoints;
+  const int64_t ng = intrinsics_size(*gt_cam), nc = intrinsics_size(*cam);
+  double *dgg = nullptr, *dgc = nullptr;
+  LocalizationDev d{};
+  cs.alloc(&dgg, ng);
+  cs.alloc(&dgc, nc);
+  cs.alloc(&d.p, 3 * n);
+  cs.alloc(&d.f, 3 * n);
+  if (samples) cs.alloc(&d.samples, 3 * n);
+  if (poses) cs.alloc(&d.poses, 6 * trials);
+  cs.alloc(&d.mag, trials);
+  cs.alloc(&d.counts, 3);
+  cs.alloc(&d.capped, 1);
+  alloc_range_statistics(cs, trials, &d.range, &d.partial, &d.select_hist, &d.stats);
+  if (cs.rc == 0) {
+    cs.ok(cudaMemcpy(dgg, gt_intr, sizeof(double) * ng, cudaMemcpyHostToDevice));
+    cs.ok(cudaMemcpy(dgc, intr, sizeof(double) * nc, cudaMemcpyHostToDevice));
+  }
+  int capped = 0;
+  if (cs.rc == 0) {
+    cs.record(0, 0);
+    launch_localization_sample(cg, dgg, cc, dgc, trials, seed, d, 0);
+    cs.ok(cudaGetLastError());
+    cs.ok(cudaMemcpy(&capped, d.capped, sizeof(int), cudaMemcpyDeviceToHost));
+  }
+  if (cs.rc == 0 && capped) {
+    g_create_error = "b200ba_localization_accuracy: a point was not un-projected by both models within " +
+                     std::to_string(kLocMaxDraws) + " draws";
+    return 4;
+  }
+  ReportCam stats{};
+  unsigned long long counts[3] = {0, 0, 0};
+  if (cs.rc == 0) {
+    launch_localization_pose(trials, d, 0);
+    cs.record(1, 0);
+    cs.ok(cudaGetLastError());
+    cs.ok(cudaMemcpy(&stats, d.stats, sizeof(ReportCam), cudaMemcpyDeviceToHost));
+    cs.ok(cudaMemcpy(counts, d.counts, sizeof(counts), cudaMemcpyDeviceToHost));
+    if (errors) {
+      std::vector<double> mag(trials);
+      cs.ok(cudaMemcpy(mag.data(), d.mag, sizeof(double) * trials, cudaMemcpyDeviceToHost));
+      for (int64_t i = 0; i < trials; ++i) errors[i] = static_cast<float>(mag[i]);  // exact: mag holds floats
+    }
+    if (poses) cs.ok(cudaMemcpy(poses, d.poses, sizeof(double) * 6 * trials, cudaMemcpyDeviceToHost));
+    if (samples) cs.ok(cudaMemcpy(samples, d.samples, sizeof(float) * 3 * n, cudaMemcpyDeviceToHost));
+  }
+  if (cs.rc == 0) {
+    if (device_ms) *device_ms = cs.elapsed_ms(0, 1);
+    b200ba_localization_report r{};
+    r.trial_count = stats.count;
+    r.average_error = stats.count > 0 ? stats.sum / static_cast<double>(stats.count) : std::nan("");
+    r.median_error = stats.median;
+    r.max_error = stats.max;
+    r.total_iterations = static_cast<int64_t>(counts[1]);
+    r.redraws = static_cast<int64_t>(counts[0]);
+    r.max_iterations = static_cast<int32_t>(counts[2]);
+    *report = r;
+  }
+  return cs.rc;
+}
+
 // Stand-alone Voronoi coverage rendering (allocates, computes, frees): what b200ba_report_images renders its
 // error maps with.
 int b200ba_render_voronoi(int device, int32_t width, int32_t height, int64_t n_sites, const int32_t* sites_q,

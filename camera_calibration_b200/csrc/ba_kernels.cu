@@ -2185,6 +2185,331 @@ void launch_compare_models(const CamDev& a, const double* ga, const CamDev& b, c
 }
 
 // ------------------------------------------------------------------------------------------
+// localization accuracy test (tools/localization_accuracy_test.cc:47-131): the draws of the 15 points of every
+// trial, then one pose fit per trial (opengv's absolute_pose::optimize_nonlinear cost; the iteration and the random
+// stream are specified in include/b200ba.h)
+// ------------------------------------------------------------------------------------------
+__host__ __device__ __forceinline__ uint64_t loc_splitmix64(uint64_t z) {
+  z += 0x9E3779B97F4A7C15ull;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+// (float)(h >> 40) * 2^-24f * extent: the first product is exact, the second rounds once
+__device__ __forceinline__ float loc_coordinate(uint64_t h, float extent) {
+  return __fmul_rn(static_cast<float>(h >> 40) * 0x1p-24f, extent);
+}
+// Eigen's normalized() without fused operations, v / sqrt((x^2 + y^2) + z^2), and v * s: the sample kernel and
+// the pose kernel build p, f and u with these, so that u = f bit for bit where both models agree
+__device__ __forceinline__ double loc_norm(d3 v) {
+  return __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(v.x, v.x), __dmul_rn(v.y, v.y)), __dmul_rn(v.z, v.z)));
+}
+__device__ __forceinline__ d3 loc_unit(d3 v, double n) { return mk3(__ddiv_rn(v.x, n), __ddiv_rn(v.y, n), __ddiv_rn(v.z, n)); }
+__device__ __forceinline__ d3 loc_scaled(d3 v, double s) { return mk3(__dmul_rn(v.x, s), __dmul_rn(v.y, s), __dmul_rn(v.z, s)); }
+
+// One thread per (trial, point): the draws until both models un-project the pixel (CentralGenericModel::Unproject
+// succeeds exactly inside the calibrated area, central_generic.h:97-105), then p = s n and f.
+constexpr int kLocSampleThreads = 128;
+__global__ void __launch_bounds__(kLocSampleThreads)
+    localization_sample_kernel(CamDev gt, const double* __restrict__ ggt, CamDev cm, const double* __restrict__ gcm,
+                               int64_t trials, uint64_t seed_hash, double* __restrict__ p, double* __restrict__ f,
+                               float* __restrict__ samples, unsigned long long* __restrict__ counts,
+                               int* __restrict__ capped) {
+  const int64_t i = blockIdx.x * static_cast<int64_t>(kLocSampleThreads) + threadIdx.x;
+  unsigned long long redraws = 0;
+  if (i < trials * kLocPoints) {
+    const uint64_t trial = static_cast<uint64_t>(i / kLocPoints), point = static_cast<uint64_t>(i % kLocPoints);
+    const uint64_t key = (trial << 20) | (point << 16);
+    const float w = static_cast<float>(gt.width), h = static_cast<float>(gt.height);
+    int a = 0;
+    float x = 0, y = 0;
+    for (; a < kLocMaxDraws; ++a) {
+      const uint64_t k = seed_hash ^ (key | (static_cast<uint64_t>(a) << 4));
+      x = loc_coordinate(loc_splitmix64(k), w);
+      y = loc_coordinate(loc_splitmix64(k ^ 1), h);
+      if (in_area(gt, x, y) && in_area(cm, x, y)) break;
+    }
+    redraws = static_cast<unsigned long long>(a);
+    const double nan_v = nan("");
+    d3 pv = mk3(nan_v, nan_v, nan_v), fv = pv;
+    float s = nan_v;
+    if (a == kLocMaxDraws) {
+      *capped = 1;
+    } else {
+      const uint64_t k = seed_hash ^ (key | (static_cast<uint64_t>(a) << 4) | 2);
+      // kMinDistance + ((rand() % 10000) / 10000.f) * (kMaxDistance - kMinDistance) (:99), in float
+      s = __fadd_rn(1.5f, __fmul_rn(__fdiv_rn(static_cast<float>(loc_splitmix64(k) % 10000), 10000.f), 1.0f));
+      CentralEval e;
+      central_eval(gt, ggt, x, y, e);
+      const d3 n = loc_unit(e.u, loc_norm(e.u));  // gt_direction.normalize() (:96)
+      central_eval(cm, gcm, x, y, e);
+      const d3 m = loc_unit(e.u, loc_norm(e.u));  // compared_direction.normalized() (:103)
+      pv = loc_scaled(n, static_cast<double>(s));
+      const d3 sm = loc_scaled(m, static_cast<double>(s));
+      fv = loc_unit(sm, loc_norm(sm));
+    }
+    p[3 * i] = pv.x;
+    p[3 * i + 1] = pv.y;
+    p[3 * i + 2] = pv.z;
+    f[3 * i] = fv.x;
+    f[3 * i + 1] = fv.y;
+    f[3 * i + 2] = fv.z;
+    if (samples) {
+      samples[3 * i] = x;
+      samples[3 * i + 1] = y;
+      samples[3 * i + 2] = s;
+    }
+  }
+  for (int o = 16; o > 0; o >>= 1) redraws += __shfl_xor_sync(0xffffffffu, redraws, o);
+  if ((threadIdx.x & 31) == 0 && redraws) atomicAdd(counts, redraws);
+}
+
+// Residual of one point at x = (t, c): v = p - t, q = R(c)' v = ((1 - c'c) v + 2 c (c'v) - 2 c x v) / (1 + c'c),
+// u = normalize(q), e = u - f. With J = 1: also dq/dx (3 x 6) through A = [-R(c)' | dq/dc] and
+// du/dx = (A - u (u'A)) / |q|, dq/dc = (-2 v c' + 2 (c'v) I + 2 c v' + 2 [v]x - 2 q c') / (1 + c'c).
+// e is computed with explicitly rounded operations in the oracle's order: the cost of the system (J = 1) and the
+// trial cost (J = 0) at the same x are then the same number, as the LM's acceptance test assumes (with contractions
+// chosen per call site, a trial could win by rounding alone and the fit would run to its iteration limit).
+__device__ __forceinline__ double loc_dot(d3 a, d3 b) {
+  return __dadd_rn(__dadd_rn(__dmul_rn(a.x, b.x), __dmul_rn(a.y, b.y)), __dmul_rn(a.z, b.z));
+}
+__device__ __forceinline__ double loc_q(double one_m, double va, double cv2, double ca, double cxva, double inv_s) {
+  return __dmul_rn(inv_s, __dsub_rn(__dadd_rn(__dmul_rn(one_m, va), __dmul_rn(cv2, ca)), __dmul_rn(2.0, cxva)));
+}
+template <bool J>
+__device__ __forceinline__ void loc_residual(const double (&x)[6], d3 p, d3 f, d3& e, double (&du)[3][6]) {
+  const d3 v = mk3(__dsub_rn(p.x, x[0]), __dsub_rn(p.y, x[1]), __dsub_rn(p.z, x[2]));
+  const d3 c = mk3(x[3], x[4], x[5]);
+  const double cc = loc_dot(c, c), cv = loc_dot(c, v), inv_s = __ddiv_rn(1.0, __dadd_rn(1.0, cc));
+  const d3 cxv = mk3(__dsub_rn(__dmul_rn(c.y, v.z), __dmul_rn(c.z, v.y)), __dsub_rn(__dmul_rn(c.z, v.x), __dmul_rn(c.x, v.z)),
+                     __dsub_rn(__dmul_rn(c.x, v.y), __dmul_rn(c.y, v.x)));
+  const double one_m = __dsub_rn(1.0, cc), cv2 = 2.0 * cv;
+  const d3 q = mk3(loc_q(one_m, v.x, cv2, c.x, cxv.x, inv_s), loc_q(one_m, v.y, cv2, c.y, cxv.y, inv_s),
+                   loc_q(one_m, v.z, cv2, c.z, cxv.z, inv_s));
+  const double nq = loc_norm(q);
+  const d3 u = loc_unit(q, nq);
+  e = mk3(__dsub_rn(u.x, f.x), __dsub_rn(u.y, f.y), __dsub_rn(u.z, f.z));
+  if (!J) return;
+  const double cs[3] = {c.x, c.y, c.z}, vs[3] = {v.x, v.y, v.z}, qs[3] = {q.x, q.y, q.z};
+  const double inv_n = 1.0 / nq;
+#pragma unroll
+  for (int b = 0; b < 3; ++b) {
+    // column b of -R' = -((1 - c'c) I + 2 c c' - 2 [c]x) / s and of dq/dc
+    d3 rt = mk3(2.0 * c.x * cs[b], 2.0 * c.y * cs[b], 2.0 * c.z * cs[b]);
+    d3 m = mk3(2.0 * (c.x * vs[b] - v.x * cs[b] - qs[0] * cs[b]), 2.0 * (c.y * vs[b] - v.y * cs[b] - qs[1] * cs[b]),
+               2.0 * (c.z * vs[b] - v.z * cs[b] - qs[2] * cs[b]));
+    if (b == 0) {
+      rt.x += one_m;
+      rt.y -= 2.0 * c.z;
+      rt.z += 2.0 * c.y;
+      m.x += 2.0 * cv;
+      m.y += 2.0 * v.z;
+      m.z -= 2.0 * v.y;
+    } else if (b == 1) {
+      rt.x += 2.0 * c.z;
+      rt.y += one_m;
+      rt.z -= 2.0 * c.x;
+      m.x -= 2.0 * v.z;
+      m.y += 2.0 * cv;
+      m.z += 2.0 * v.x;
+    } else {
+      rt.x -= 2.0 * c.y;
+      rt.y += 2.0 * c.x;
+      rt.z += one_m;
+      m.x += 2.0 * v.y;
+      m.y -= 2.0 * v.x;
+      m.z += 2.0 * cv;
+    }
+    const d3 at = (-inv_s) * rt, ac = inv_s * m;
+    const d3 jt = inv_n * (at - dot3(u, at) * u), jc = inv_n * (ac - dot3(u, ac) * u);
+    du[0][b] = jt.x;
+    du[1][b] = jt.y;
+    du[2][b] = jt.z;
+    du[0][3 + b] = jc.x;
+    du[1][3 + b] = jc.y;
+    du[2][3 + b] = jc.z;
+  }
+}
+// r = 1/2 |e|^2 = 1 - f'u for unit vectors; the point's term of F is r^2
+__device__ __forceinline__ double loc_cost_term(d3 e) {
+  const double r = 0.5 * __dadd_rn(__dadd_rn(__dmul_rn(e.x, e.x), __dmul_rn(e.y, e.y)), __dmul_rn(e.z, e.z));
+  return r * r;
+}
+// sys = {F, grad F (6), H (21, lower triangle row by row)} of one point
+constexpr int kLocSums = 28;
+__device__ __forceinline__ int loc_h(int i, int j) { return 7 + i * (i + 1) / 2 + j; }
+__device__ __forceinline__ void loc_point_system(const double (&x)[6], d3 p, d3 f, double (&sys)[kLocSums]) {
+  d3 e;
+  double du[3][6];
+  loc_residual<true>(x, p, f, e, du);
+  sys[0] = loc_cost_term(e);
+  const double w = dot3(e, e);
+  double a[6];
+#pragma unroll
+  for (int j = 0; j < 6; ++j) {
+    a[j] = du[0][j] * e.x + du[1][j] * e.y + du[2][j] * e.z;  // (J'e)_j
+    sys[1 + j] = w * a[j];
+  }
+#pragma unroll
+  for (int i = 0; i < 6; ++i)
+#pragma unroll
+    for (int j = 0; j <= i; ++j)
+      sys[loc_h(i, j)] = w * (du[0][i] * du[0][j] + du[1][i] * du[1][j] + du[2][i] * du[2][j]) + 2.0 * a[i] * a[j];
+}
+// the same sum in every lane of the 16: a fixed xor butterfly (a + b == b + a, so all lanes agree bit for bit)
+template <int N>
+__device__ __forceinline__ void loc_reduce(double (&v)[N], unsigned mask) {
+#pragma unroll
+  for (int o = 8; o > 0; o >>= 1)
+#pragma unroll
+    for (int k = 0; k < N; ++k) v[k] += __shfl_xor_sync(mask, v[k], o);
+}
+// (H + lambda I) d = -g by Cholesky; false where H + lambda I is not positive definite
+__device__ __forceinline__ bool loc_solve(const double (&sys)[kLocSums], double lambda, double (&d)[6]) {
+  double L[21];
+  bool ok = true;
+#pragma unroll
+  for (int i = 0; i < 6; ++i)
+#pragma unroll
+    for (int j = 0; j <= i; ++j) {
+      double a = sys[loc_h(i, j)] + (i == j ? lambda : 0.0);
+#pragma unroll
+      for (int k = 0; k < j; ++k) a -= L[i * (i + 1) / 2 + k] * L[j * (j + 1) / 2 + k];
+      if (i == j) {
+        ok = ok && a > 0;
+        L[i * (i + 1) / 2 + i] = sqrt(a);
+      } else {
+        L[i * (i + 1) / 2 + j] = a / L[j * (j + 1) / 2 + j];
+      }
+    }
+  double y[6];
+#pragma unroll
+  for (int i = 0; i < 6; ++i) {
+    double a = -sys[1 + i];
+#pragma unroll
+    for (int k = 0; k < i; ++k) a -= L[i * (i + 1) / 2 + k] * y[k];
+    y[i] = a / L[i * (i + 1) / 2 + i];
+  }
+#pragma unroll
+  for (int i = 5; i >= 0; --i) {
+    double a = y[i];
+#pragma unroll
+    for (int k = i + 1; k < 6; ++k) a -= L[k * (k + 1) / 2 + i] * d[k];
+    d[i] = a / L[i * (i + 1) / 2 + i];
+  }
+  return ok;
+}
+
+// 16 lanes per trial, two trials per warp; lane i < 15 owns point i, lane 15 adds zeros. Every lane holds the whole
+// LM state (x, lambda, F, the reduced system) and factors H + lambda I itself, so the 16 lanes take the same branches.
+constexpr int kLocPoseThreads = 128;
+constexpr int kLocMaxIterations = 100;
+__global__ void __launch_bounds__(kLocPoseThreads)
+    localization_pose_kernel(int64_t trials, const double* __restrict__ p, const double* __restrict__ f,
+                             double* __restrict__ poses, double* __restrict__ mag,
+                             unsigned long long* __restrict__ counts) {
+  const int64_t trial = (blockIdx.x * static_cast<int64_t>(kLocPoseThreads) + threadIdx.x) >> 4;
+  const int lane = threadIdx.x & 15;
+  const unsigned mask = 0xffffu << (threadIdx.x & 16);
+  __shared__ unsigned long long block_iterations;
+  __shared__ unsigned int block_max;
+  if (threadIdx.x == 0) {
+    block_iterations = 0;
+    block_max = 0;
+  }
+  __syncthreads();
+  if (trial < trials) {
+    const bool own = lane < kLocPoints;
+    d3 pi = mk3(0, 0, 0), fi = mk3(0, 0, 0);
+    if (own) {
+      const int64_t o = 3 * (trial * kLocPoints + lane);
+      pi = ld3(p + o);
+      fi = ld3(f + o);
+    }
+    double x[6] = {0, 0, 0, 0, 0, 0};
+    double lambda = 0;
+    int iterations = 0;
+    for (int it = 0; it < kLocMaxIterations; ++it) {
+      double sys[kLocSums];
+      loc_point_system(x, pi, fi, sys);
+      if (!own)
+#pragma unroll
+        for (int k = 0; k < kLocSums; ++k) sys[k] = 0;
+      loc_reduce(sys, mask);
+      const double cost = sys[0];
+      if (cost == 0) break;
+      if (it == 0) {
+        double trace = 0;
+#pragma unroll
+        for (int i = 0; i < 6; ++i) trace += sys[loc_h(i, i)];
+        lambda = static_cast<double>(0.001f) * trace / 6;
+      }
+      bool applied = false;
+      double test_cost = cost;
+      for (int attempt = 0; attempt < 10; ++attempt) {
+        double d[6];
+        if (!loc_solve(sys, lambda, d)) {
+          lambda = 2.0 * lambda;
+          continue;
+        }
+        double xt[6];
+#pragma unroll
+        for (int k = 0; k < 6; ++k) xt[k] = x[k] + d[k];
+        d3 e;
+        double unused[3][6];
+        loc_residual<false>(xt, pi, fi, e, unused);
+        double tc[1] = {own ? loc_cost_term(e) : 0.0};
+        loc_reduce(tc, mask);
+        if (tc[0] < cost) {
+#pragma unroll
+          for (int k = 0; k < 6; ++k) x[k] = xt[k];
+          lambda = 0.5 * lambda;
+          applied = true;
+          ++iterations;
+          test_cost = tc[0];
+          break;
+        }
+        lambda = 2.0 * lambda;
+      }
+      if (!applied || test_cost == 0) break;
+    }
+    if (lane == 0) {
+      if (poses)
+#pragma unroll
+        for (int k = 0; k < 6; ++k) poses[6 * trial + k] = x[k];
+      // (float)translation.norm() (:115-116)
+      const float err = static_cast<float>(loc_norm(mk3(x[0], x[1], x[2])));
+      mag[trial] = static_cast<double>(err);
+      atomicAdd(&block_iterations, static_cast<unsigned long long>(iterations));
+      atomicMax(&block_max, static_cast<unsigned int>(iterations));
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    if (block_iterations) atomicAdd(counts + 1, block_iterations);
+    atomicMax(counts + 2, static_cast<unsigned long long>(block_max));
+  }
+}
+
+void launch_localization_sample(const CamDev& gt, const double* ggt, const CamDev& cmp, const double* gcmp,
+                                int64_t trials, uint64_t seed, const LocalizationDev& d, cudaStream_t s) {
+  cudaMemsetAsync(d.counts, 0, 3 * sizeof(unsigned long long), s);
+  cudaMemsetAsync(d.capped, 0, sizeof(int), s);
+  const int64_t n = trials * kLocPoints;
+  const uint64_t seed_hash = loc_splitmix64(seed);
+  localization_sample_kernel<<<static_cast<unsigned>((n + kLocSampleThreads - 1) / kLocSampleThreads),
+                               kLocSampleThreads, 0, s>>>(gt, ggt, cmp, gcmp, trials, seed_hash, d.p, d.f, d.samples,
+                                                          d.counts, d.capped);
+}
+
+void launch_localization_pose(int64_t trials, const LocalizationDev& d, cudaStream_t s) {
+  constexpr int kTrialsPerBlock = kLocPoseThreads / 16;
+  localization_pose_kernel<<<static_cast<unsigned>((trials + kTrialsPerBlock - 1) / kTrialsPerBlock), kLocPoseThreads,
+                             0, s>>>(trials, d.p, d.f, d.poses, d.mag, d.counts);
+  launch_report_statistics(1, d.range, d.mag, d.partial, d.select_hist, d.stats, s);
+}
+
+// ------------------------------------------------------------------------------------------
 // centre-point analysis of a non-central camera (CreateCalibrationReportForCamera, APP/calibration_report.cc:839-982)
 // ------------------------------------------------------------------------------------------
 // The lines are evaluated once and stored (48 B per line: 55 MB for 1200 x 950, 576 MB for 4000 x 3000); every LM

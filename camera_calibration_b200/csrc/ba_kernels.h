@@ -59,6 +59,11 @@ int report_partial_size(int n_cameras);
 // on the device
 void launch_compare_models(const CamDev& a, const double* ga, const CamDev& b, const double* gb, const CompareDev& d,
                            cudaStream_t s);
+// localization accuracy test (b200ba_localization_accuracy): the draws of every point (sets d.capped when a point
+// needs more than kLocMaxDraws draws), then, after the caller has checked d.capped, the pose fits and the statistics
+void launch_localization_sample(const CamDev& gt, const double* ggt, const CamDev& cmp, const double* gcmp,
+                                int64_t trials, uint64_t seed, const LocalizationDev& d, cudaStream_t s);
+void launch_localization_pose(int64_t trials, const LocalizationDev& d, cudaStream_t s);
 // centre-point analysis of a non-central camera (b200ba_line_offsets); intr on the device. launch_line_pass stores
 // the line of every calibrated-rectangle pixel in d.lines; launch_line_system sums (mode 0) the cost, (1) + b,
 // (2) + H at the centre c into d.sums; launch_line_outputs computes the distances and their statistics, the

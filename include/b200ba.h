@@ -355,6 +355,56 @@ B200BA_API int b200ba_compare_models(int device, const b200ba_camera* cam_a, con
                                      const b200ba_camera* cam_b, const double* intr_b, b200ba_fitting_report* report,
                                      double* direction_errors, double* reprojection_errors, double* device_ms);
 
+/* ---- localization accuracy test (APP/tools/localization_accuracy_test.cc:47-131, --localization_accuracy_test):
+ * what the difference between a ground-truth calibration and a compared calibration of one camera costs a camera
+ * that is localized with the compared one. Every trial:
+ *   1. draws 15 points: a float pixel (x, y) in [0, w] x [0, h] that BOTH models un-project (drawn again
+ *      otherwise), the ground-truth unit direction n = normalize(u_gt) at a distance s, p = s n, and the compared
+ *      bearing f = normalize(s normalize(u_cmp)) -- mathematically normalize(u_cmp); written with the operations
+ *      that normalise the transformed point, so that two identical models give f = normalize(p) bit for bit;
+ *   2. fits the pose x = (t, c) from x = 0, c the Cayley vector, R(c) = ((1 - c'c) I + 2 c c' + 2 [c]x) / (1 + c'c),
+ *      u_i = normalize(R(c)' (p_i - t)), minimising opengv's absolute_pose::optimize_nonlinear cost
+ *      F = sum_i (1 - f_i' u_i)^2, evaluated without cancellation as sum_i r_i^2, r_i = 1/2 |u_i - f_i|^2.
+ *      The iteration is Levenberg-Marquardt on H = sum_i J_i' (|e_i|^2 I + 2 e_i e_i') J_i (the Hessian of F
+ *      without its O(|e|^3) terms), e_i = u_i - f_i, J_i = du_i / d(t, c), step (H + lambda I) d = -grad F,
+ *      x <- x + d; lambda_0 = 0.001f tr(H) / 6, at most 10 attempts per iteration (x0.5 on an accepted step, x2
+ *      on a rejected step or a failed Cholesky factorisation), at most 100 iterations, stopping when an
+ *      iteration accepts nothing or F == 0. The result is the minimiser of the reference's cost, not the point
+ *      where the reference's MINPACK solver stops (that is reached early, at about twice the minimal cost);
+ *   3. records error = (float)|t|, the camera-centre offset in metres.
+ * The random stream is counter-based: with key = (trial << 20) | (point << 16) | (attempt << 4) | component and
+ * SplitMix64(z) = { z += 0x9E3779B97F4A7C15; z = (z ^ z >> 30) * 0xBF58476D1CE4E5B9;
+ *                   z = (z ^ z >> 27) * 0x94D049BB133111EB; return z ^ z >> 31; } (mod 2^64),
+ * a draw is h = SplitMix64(SplitMix64(seed) ^ key), so it depends only on (seed, trial, point, attempt,
+ * component). Attempt a of a point takes x = (float)(h_0 >> 40) * 2^-24f * (float)w and
+ * y = (float)(h_1 >> 40) * 2^-24f * (float)h (component 0 and 1, float products); the attempt that both models
+ * un-project takes the distance s = 1.5f + ((float)(h_2 % 10000) / 10000.f) * 1.0f (component 2). Examples, w = 640:
+ *   seed 0, trial 0, point 0, attempt 0:  h_0 = 0xa706dd2f4d197e6f, x = 417.5670166015625,
+ *                                         h_2 = 0xd7cc9674ff5ffa39, s = 1.7856999635696411 (k = 2857)
+ *   seed 7, trial 12345, point 14, attempt 3:  h_0 = 0xe273e8e0afcdd023, x = 566.1318969726562
+ * Both models must be central-generic (OpenCV models have no device un-projection; the reference never ends for a
+ * non-central model, whose Unproject(x, y, Vec3d*) always fails), of one image size, with grids of at least
+ * 4 x 4 and calibrated areas that intersect [0, w] x [0, h]. */
+typedef struct b200ba_localization_report {
+  int64_t trial_count;
+  double average_error; /* metres: the mean of the float errors, a fixed-order double sum (the reference sums in
+                           float, in order) */
+  double median_error;  /* metres: sorted(errors)[trial_count / 2] */
+  double max_error;     /* metres */
+  int64_t total_iterations; /* accepted LM steps over all pose fits */
+  int64_t redraws;          /* pixels drawn again because a model did not un-project them */
+  int32_t max_iterations;   /* accepted LM steps of the longest pose fit */
+} b200ba_localization_report;
+/* Stand-alone (allocates, computes, frees); the grids gt_intr / intr [3 * grid_width * grid_height] are not
+ * modified. errors (nullable): [trials] float. poses (nullable): [trials][6] t, c. samples (nullable):
+ * [trials][15][3] float x, y, distance of the accepted draws. device_ms (nullable): device time of the test.
+ * Returns 2 for a bad argument (before any CUDA call; also for trials < 1 or trials > 2^32), 3 without a device,
+ * 4 when a point of a trial is still not un-projected by both models after 4096 draws. */
+B200BA_API int b200ba_localization_accuracy(int device, const b200ba_camera* gt_cam, const double* gt_intr,
+                                            const b200ba_camera* cam, const double* intr, int64_t trials,
+                                            uint64_t seed, b200ba_localization_report* report, float* errors,
+                                            double* poses, float* samples, double* device_ms);
+
 /* ---- centre-point analysis of a non-central camera: the NoncentralGenericModel branch of
  * CreateCalibrationReportForCamera (APP/calibration_report.cc:839-982, with CenterPointCostFunction of :56-80).
  *   1. every pixel (x + 0.5f, y + 0.5f) of the calibrated area is un-projected to a line (o, d) (:847-856);

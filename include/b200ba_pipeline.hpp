@@ -1,6 +1,7 @@
 // b200ba_pipeline.hpp -- C++ host logic of the callers either side of the hot path (SURVEY.md 8f-3 / 8f-4):
 // the outlier deletion between bundle-adjustment rounds, the metric rescaling, the pyramid resampling of the generic
-// models, the calibration report's info files and the comparison of two calibrations, over the containers of
+// models, the calibration report's info files, the comparison of two calibrations and the localization accuracy test,
+// over the containers of
 // b200ba_shim.hpp. (RunBundleAdjustment itself -- 8f-2 -- is in b200ba_shim.hpp and runs device-resident in the
 // library.) The Python mirror is camera_calibration_b200/pipeline.py.
 //
@@ -668,6 +669,58 @@ inline int CompareCalibrations(const std::string& calibration_a, const std::stri
     std::cerr << "Cannot write file: " << path << "\n";
     return EXIT_FAILURE;
   }
+  return EXIT_SUCCESS;
+}
+
+// ---- localization accuracy test ---------------------------------------------------------------------------------
+// tools/localization_accuracy_test.cc:47-131: load both models, run b200ba_localization_accuracy (`trials` pose fits of
+// one seeded random stream; the reference seeds with the time) and print "Average error [mm]" and "Median error [mm]"
+// with std::ostream's default 6 significant digits, like the reference's LOG(INFO). Returns EXIT_SUCCESS /
+// EXIT_FAILURE with the reference's messages on stderr; models that are not central-generic are refused with
+// EXIT_FAILURE (the reference never ends for a non-central model). Throws on a library error.
+inline int LocalizationAccuracyTest(const std::string& gt_model_yaml_path, const std::string& compared_model_yaml_path,
+                                    int64_t trials = 10000, uint64_t seed = 0) {
+  std::shared_ptr<CameraModel> gt_model = LoadCameraModel(gt_model_yaml_path.c_str());
+  if (!gt_model) {
+    std::cerr << "Cannot load ground truth camera model: " << gt_model_yaml_path << "\n";
+    return EXIT_FAILURE;
+  }
+  std::shared_ptr<CameraModel> compared_model = LoadCameraModel(compared_model_yaml_path.c_str());
+  if (!compared_model) {
+    std::cerr << "Cannot load camera model to compare: " << compared_model_yaml_path << "\n";
+    return EXIT_FAILURE;
+  }
+  if (gt_model->width() != compared_model->width() || gt_model->height() != compared_model->height()) {
+    std::cerr << "The ground truth and compared camera models do not have the same image size.\n";
+    return EXIT_FAILURE;
+  }
+  auto* gt = dynamic_cast<CentralGenericModel*>(gt_model.get());
+  auto* compared = dynamic_cast<CentralGenericModel*>(compared_model.get());
+  if (!gt || !compared) {
+    std::cerr << "The localization accuracy test is only implemented for CentralGenericModel.\n";
+    return EXIT_FAILURE;
+  }
+  auto camera = [](const CentralGenericModel& m) {
+    b200ba_camera c{};
+    c.model_type = B200BA_MODEL_CENTRAL_GENERIC;
+    c.width = m.width();
+    c.height = m.height();
+    c.calibration_min_x = m.calibration_min_x();
+    c.calibration_min_y = m.calibration_min_y();
+    c.calibration_max_x = m.calibration_max_x();
+    c.calibration_max_y = m.calibration_max_y();
+    c.grid_width = m.gw;
+    c.grid_height = m.gh;
+    return c;
+  };
+  const b200ba_camera gt_cam = camera(*gt), cam = camera(*compared);
+  b200ba_localization_report report{};
+  if (b200ba_localization_accuracy(-1, &gt_cam, gt->grid.data(), &cam, compared->grid.data(), trials, seed, &report,
+                                   nullptr, nullptr, nullptr, nullptr) != 0)
+    throw std::runtime_error(std::string("b200ba_localization_accuracy: ") + b200ba_last_error(nullptr));
+  std::cout << "Average error [mm]: " << (1000 * report.average_error) << "\n";
+  std::cout << "Median error [mm]: " << (1000 * report.median_error) << "\n";
+  std::cout.flush();
   return EXIT_SUCCESS;
 }
 

@@ -1009,6 +1009,33 @@ def CompareModels(model_a: CameraModel, model_b: CameraModel, with_errors: bool 
     return report, dir_err, rep_err, ms.value
 
 
+# the images of FittingImages: (name, channels, file suffix), in the order the reference writes them
+# (fitting_report.h:180-184)
+FITTING_IMAGES = (("error_magnitudes", 1, "_fitting_error_magnitudes.png"),
+                  ("error_direction_angles", 3, "_fitting_error_direction_angles.png"),
+                  ("error_directions", 3, "_fitting_error_directions.png"),
+                  ("reprojection_magnitudes", 1, "_fitting_error_reprojection_magnitudes.png"),
+                  ("reprojections", 3, "_fitting_error_reprojections.png"))
+
+
+def FittingImages(model_a: CameraModel, model_b: CameraModel, device: int = -1):
+    """CreateFittingErrorReport(base = model_a, fitted = model_b, Identity) with its five images
+    (APP/fitting_report.h:135-184) on the device (``b200ba_fitting_images``; the colour rules are specified in
+    include/b200ba.h). Returns (report, images, device_ms): the same ``cabi.FittingReport`` as ``CompareModels``
+    and a dict name -> uint8 image, [h, w] or [h, w, 3], for every name of ``FITTING_IMAGES``."""
+    lib = cabi.load_library()
+    ca, cb = model_a.c_camera(), model_b.c_camera()
+    ia = np.ascontiguousarray(model_a.flat_intrinsics(), dtype=np.float64)
+    ib = np.ascontiguousarray(model_b.flat_intrinsics(), dtype=np.float64)
+    h, w = model_a.height(), model_a.width()
+    images = {name: np.empty((h, w, ch) if ch > 1 else (h, w), np.uint8) for name, ch, _ in FITTING_IMAGES}
+    report = cabi.FittingReport()
+    ms = C.c_double(0)
+    _check(lib.b200ba_fitting_images(device, C.byref(ca), _dp(ia), C.byref(cb), _dp(ib), C.byref(report),
+                                     *[_u8p(images[name]) for name, _, _ in FITTING_IMAGES], C.byref(ms)))
+    return report, images, ms.value
+
+
 def LineObjCount(model: CameraModel, obj_step: int = 20) -> int:
     """Number of lines in the .obj models of the centre-point analysis: every obj_step-th pixel of the calibrated
     area from calibration_min in x and in y (calibration_report.cc:945-946)."""

@@ -424,6 +424,9 @@ SYMBOLS = {
                                         C.POINTER(FitReport)]),
     "b200ba_compare_models": (C.c_int, [C.c_int, C.POINTER(Camera), _D, C.POINTER(Camera), _D, C.POINTER(FittingReport),
                                         _D, _D, _D]),
+    "b200ba_fitting_images": (C.c_int, [C.c_int, C.POINTER(Camera), _D, C.POINTER(Camera), _D, C.POINTER(FittingReport),
+                                        C.POINTER(C.c_uint8), C.POINTER(C.c_uint8), C.POINTER(C.c_uint8),
+                                        C.POINTER(C.c_uint8), C.POINTER(C.c_uint8), _D]),
     "b200ba_line_offsets": (C.c_int, [C.c_int, C.POINTER(Camera), _D, C.POINTER(LineOffsetsReport), C.POINTER(C.c_uint8),
                                       _D, C.c_int32, _D, C.POINTER(C.c_int64), _D]),
     "b200ba_localization_accuracy": (C.c_int, [C.c_int, C.POINTER(Camera), _D, C.POINTER(Camera), _D, C.c_int64,

@@ -143,6 +143,12 @@ struct CompareDev {
   double* partial;              // report_partial_size(1)
   unsigned int* select_hist;    // [256]
   ReportCam* stats;             // count / sum / max / median
+  // the five images of b200ba_fitting_images, row-major, or all NULL (then dir_err may be NULL too)
+  uint8_t* angles;              // [3 * w * h] _fitting_error_direction_angles.png, written by the comparison pass
+  uint8_t* magnitudes;          // [w * h]     _fitting_error_magnitudes.png
+  uint8_t* directions;          // [3 * w * h] _fitting_error_directions.png
+  uint8_t* rep_magnitudes;      // [w * h]     _fitting_error_reprojection_magnitudes.png
+  uint8_t* reprojections;       // [3 * w * h] _fitting_error_reprojections.png
 };
 
 // Localization accuracy test (b200ba_localization_accuracy): device buffers of one call.

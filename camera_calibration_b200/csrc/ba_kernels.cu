@@ -2095,6 +2095,8 @@ void launch_report_errors(const ProblemDev& pb, int n_cameras, const StateDev& s
 //   the two direction maxima over the pixels where both succeed;
 //   B.Project(dir_A) from the centre of B's calibrated area (no warm start): e = pixel - projection.
 // mag = |e| (NaN where A or Project fails) feeds launch_report_statistics.
+// With `angles` set, the pass also writes _fitting_error_direction_angles.png (fitting_report.h:144-157), the one
+// image that needs the two directions rather than their difference and depends on no maximum.
 constexpr int kCompareTileX = 16, kCompareTileY = 8;
 __device__ __forceinline__ bool compare_unproject(const CamDev& c, const double* __restrict__ grid, double x, double y,
                                                   d3& d) {
@@ -2104,10 +2106,19 @@ __device__ __forceinline__ bool compare_unproject(const CamDev& c, const double*
   d = e.u;
   return true;
 }
+// std::min<int>(255, std::max<int>(0, 127 + 127 / (M_PI / 180.f * 0.025) * (g - f) + 0.5)) (fitting_report.h:155-156):
+// evaluated left to right in double, converted to int as x86-64 does (INT_MIN for NaN, hence 0)
+__device__ __forceinline__ uint8_t fitting_angle(double g, double f) {
+  constexpr double kScale = 127 / (3.14159265358979323846 / static_cast<double>(180.f) * 0.025);
+  const double v = __dadd_rn(__dadd_rn(127.0, __dmul_rn(kScale, __dsub_rn(g, f))), 0.5);
+  return static_cast<uint8_t>(min(255, max(0, report_trunc(v))));
+}
+// kAngles: whether `angles` is set; a separate instance, so that the comparison alone keeps its register budget
+template <bool kAngles>
 __global__ void __launch_bounds__(kCompareTileX * kCompareTileY)
     compare_models_kernel(CamDev ca, const double* __restrict__ ga, CamDev cb, const double* __restrict__ gb,
                           double* __restrict__ mag, double* __restrict__ dir_err, double* __restrict__ rep_err,
-                          unsigned long long* __restrict__ dir_max) {
+                          unsigned long long* __restrict__ dir_max, uint8_t* __restrict__ angles) {
   const int x = blockIdx.x * kCompareTileX + threadIdx.x;
   const int y = blockIdx.y * kCompareTileY + threadIdx.y;
   const bool inside = x < ca.width && y < ca.height;
@@ -2119,6 +2130,7 @@ __global__ void __launch_bounds__(kCompareTileX * kCompareTileY)
     const double nan_v = nan("");
     double m = nan_v, ex = nan_v, ey = nan_v;
     d3 da;
+    uint8_t ang0 = 0, ang1 = 0, ang2 = 0;  // (0, 0, 0) where A fails (error.hasNaN())
     if (compare_unproject(ca, ga, px, py, da)) {
       d3 db, err;
       if (compare_unproject(cb, gb, px, py, db)) {
@@ -2130,6 +2142,13 @@ __global__ void __launch_bounds__(kCompareTileX * kCompareTileY)
         max_norm = sqrt(__dadd_rn(__dadd_rn(__dmul_rn(err.x, err.x), __dmul_rn(err.y, err.y)), __dmul_rn(err.z, err.z)));
       } else {
         err = mk3(INFINITY, INFINITY, INFINITY);
+        // the reference reads its uninitialised fitted direction here; pinned as NaN, which gives (0, 0, 127)
+        db = mk3(nan_v, nan_v, nan_v);
+      }
+      if (kAngles && !(isnan(err.x) || isnan(err.y) || isnan(err.z))) {
+        ang0 = fitting_angle(atan2(da.z, da.x), atan2(db.z, db.x));
+        ang1 = fitting_angle(atan2(da.y, da.z), atan2(db.y, db.z));
+        ang2 = 127;
       }
       if (dir_err) {
         dir_err[3 * p] = err.x;
@@ -2153,6 +2172,11 @@ __global__ void __launch_bounds__(kCompareTileX * kCompareTileY)
       rep_err[2 * p] = ex;
       rep_err[2 * p + 1] = ey;
     }
+    if (kAngles) {
+      angles[3 * p] = ang0;
+      angles[3 * p + 1] = ang1;
+      angles[3 * p + 2] = ang2;
+    }
   }
   // first stage of the maxima: the block's maximum, then one atomicMax per block on the bit patterns
   // (non-negative doubles order like their uint64 patterns; max is order-independent, so this is exact)
@@ -2175,13 +2199,71 @@ __global__ void __launch_bounds__(kCompareTileX * kCompareTileY)
   }
 }
 
+// The other four images of CreateFittingErrorReport (fitting_report.h:141-177), one thread per pixel, from the
+// comparison's dir_err and mag and the three maxima as the statistics left them on the device. Every value is
+// evaluated in the reference's order and float/double mix and converted to u8 as x86-64 does (report_trunc, then the
+// low byte):
+//   magnitude     255.99f * (|e| / max_error_norm); 0 where e = +inf (B fails) and where 0 / 0;
+//   direction     (255.99f / 2) * (min(max(e / max_error_component, -1), 1) + 1) per component, where std::min /
+//                 std::max (Eigen's cwiseMin / cwiseMax) keep their first argument when a comparison sees NaN;
+//   reprojection  max<float>(0, min<float>(255, 255.99f * |r| / reprojection_error_max)), |r| = 0 where A or
+//   magnitude     Project fails (the reference's image holds zero there; mag holds NaN);
+// and (0, 0, 0) for the first two where A fails (e = NaN). The reprojection-direction image is
+// 127 + s * 127 * (sin, cos)(atan2(-r.y, -r.x)), 127, + 0.5f with the strength s = max(0, min(1, |r| / -1)): the tool
+// passes max_visualization_extent_pixels = -1, so s = 0 for every |r| >= 0 and every pixel is (127, 127, 127).
+constexpr int kFittingImageThreads = 256;
+__global__ void __launch_bounds__(kFittingImageThreads)
+    fitting_images_kernel(int64_t n, const double* __restrict__ dir_err, const double* __restrict__ mag,
+                          const unsigned long long* __restrict__ dir_max, const ReportCam* __restrict__ stats,
+                          uint8_t* __restrict__ magnitudes, uint8_t* __restrict__ directions,
+                          uint8_t* __restrict__ rep_magnitudes, uint8_t* __restrict__ reprojections) {
+  const int64_t p = static_cast<int64_t>(blockIdx.x) * kFittingImageThreads + threadIdx.x;
+  if (p >= n) return;
+  const double max_norm = __longlong_as_double(static_cast<long long>(dir_max[0]));
+  const double max_comp = __longlong_as_double(static_cast<long long>(dir_max[1]));
+  const double rep_max = stats->max;
+  const double k = static_cast<double>(255.99f), k_half = static_cast<double>(255.99f / 2);
+  const double e[3] = {dir_err[3 * p], dir_err[3 * p + 1], dir_err[3 * p + 2]};
+  uint8_t m = 0, dir[3] = {0, 0, 0};
+  if (!(isnan(e[0]) || isnan(e[1]) || isnan(e[2]))) {
+    for (int c = 0; c < 3; ++c) {
+      double r = __ddiv_rn(e[c], max_comp);
+      r = r < -1.0 ? -1.0 : r;  // std::max(r, -1): r if the comparison is false, NaN included
+      r = 1.0 < r ? 1.0 : r;    // std::min(r, 1)
+      dir[c] = static_cast<uint8_t>(report_trunc(__dmul_rn(k_half, __dadd_rn(r, 1.0))));
+    }
+    const double norm = sqrt(__dadd_rn(__dadd_rn(__dmul_rn(e[0], e[0]), __dmul_rn(e[1], e[1])), __dmul_rn(e[2], e[2])));
+    m = static_cast<uint8_t>(report_trunc(__dmul_rn(k, __ddiv_rn(norm, max_norm))));
+  }
+  const double r_norm = isnan(mag[p]) ? 0.0 : mag[p];
+  float v = __double2float_rn(__ddiv_rn(__dmul_rn(k, r_norm), rep_max));
+  v = v < 255.f ? v : 255.f;  // std::min<float>(255, v): 255 for NaN
+  v = 0.f < v ? v : 0.f;      // std::max<float>(0, v)
+  magnitudes[p] = m;
+  directions[3 * p] = dir[0];
+  directions[3 * p + 1] = dir[1];
+  directions[3 * p + 2] = dir[2];
+  rep_magnitudes[p] = static_cast<uint8_t>(report_trunc(v));
+  reprojections[3 * p] = reprojections[3 * p + 1] = reprojections[3 * p + 2] = 127;
+}
+
 void launch_compare_models(const CamDev& a, const double* ga, const CamDev& b, const double* gb, const CompareDev& d,
                            cudaStream_t s) {
   cudaMemsetAsync(d.dir_max, 0, 2 * sizeof(unsigned long long), s);  // the bits of +0.0
   const dim3 grid((a.width + kCompareTileX - 1) / kCompareTileX, (a.height + kCompareTileY - 1) / kCompareTileY);
-  compare_models_kernel<<<grid, dim3(kCompareTileX, kCompareTileY), 0, s>>>(a, ga, b, gb, d.mag, d.dir_err, d.rep_err,
-                                                                           d.dir_max);
+  if (d.angles)
+    compare_models_kernel<true><<<grid, dim3(kCompareTileX, kCompareTileY), 0, s>>>(a, ga, b, gb, d.mag, d.dir_err,
+                                                                                 d.rep_err, d.dir_max, d.angles);
+  else
+    compare_models_kernel<false><<<grid, dim3(kCompareTileX, kCompareTileY), 0, s>>>(a, ga, b, gb, d.mag, d.dir_err,
+                                                                                  d.rep_err, d.dir_max, nullptr);
   launch_report_statistics(1, d.range, d.mag, d.partial, d.select_hist, d.stats, s);
+  if (d.magnitudes) {
+    const int64_t n = static_cast<int64_t>(a.width) * a.height;
+    fitting_images_kernel<<<static_cast<unsigned>((n + kFittingImageThreads - 1) / kFittingImageThreads),
+                            kFittingImageThreads, 0, s>>>(n, d.dir_err, d.mag, d.dir_max, d.stats, d.magnitudes,
+                                                          d.directions, d.rep_magnitudes, d.reprojections);
+  }
 }
 
 // ------------------------------------------------------------------------------------------

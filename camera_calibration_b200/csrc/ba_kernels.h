@@ -56,7 +56,7 @@ void launch_calibration_report(const ProblemDev& pb, int n_cameras, const StateD
                                cudaStream_t s);
 int report_partial_size(int n_cameras);
 // comparison of two central-generic models of the same image size (b200ba_compare_models); the grids a and b are
-// on the device
+// on the device. With d's images set (d.dir_err is then required), also the five images of b200ba_fitting_images.
 void launch_compare_models(const CamDev& a, const double* ga, const CamDev& b, const double* gb, const CompareDev& d,
                            cudaStream_t s);
 // localization accuracy test (b200ba_localization_accuracy): the draws of every point (sets d.capped when a point

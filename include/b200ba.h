@@ -354,6 +354,38 @@ typedef struct b200ba_fitting_report {
 B200BA_API int b200ba_compare_models(int device, const b200ba_camera* cam_a, const double* intr_a,
                                      const b200ba_camera* cam_b, const double* intr_b, b200ba_fitting_report* report,
                                      double* direction_errors, double* reprojection_errors, double* device_ms);
+/* The comparison of b200ba_compare_models (same arguments and checks, the same report bit for bit) together with the
+ * five images of CreateFittingErrorReport (fitting_report.h:135-184), row-major (y, x), all required:
+ *   error_magnitudes        [h*w]    _fitting_error_magnitudes.png: 255.99f * (|e| / max_error_norm), e = dir_B - dir_A
+ *   error_direction_angles  [h*w*3]  _fitting_error_direction_angles.png: per channel
+ *                                    min(255, max(0, (int)(127 + 127 / (M_PI / 180.f * 0.025) * (atan2(a.z, a.x) -
+ *                                    atan2(b.z, b.x)) + 0.5))), the same with atan2(.y, .z), and 127; a = dir_A, b = dir_B
+ *   error_directions        [h*w*3]  _fitting_error_directions.png: (255.99f / 2) * (clamp(e / max_error_component,
+ *                                    -1, 1) + 1) per component
+ *   reprojection_magnitudes [h*w]    _fitting_error_reprojection_magnitudes.png:
+ *                                    max<float>(0, min<float>(255, 255.99f * |r| / reprojection_error_max))
+ *   reprojections           [h*w*3]  _fitting_error_reprojections.png: (127, 127, 127) everywhere (below)
+ * with r = pixel - B.Project(dir_A). Every value is computed in the reference's order and float / double mix. Where the
+ * reference's C++ is undefined, the result is what its x86-64 build computes:
+ *   - every double / float -> u8 conversion, and the angle's double -> int, truncates to int32 with INT_MIN for NaN
+ *     and out-of-range values, then keeps the low byte: so the magnitude is 0 where B fails (e = +inf) and where
+ *     max_error_norm == 0 (0 / 0);
+ *   - std::min / std::max and Eigen's cwiseMin / cwiseMax keep their first argument when a comparison involves NaN:
+ *     where max_error_component == 0 a zero error gives NaN and the direction pixel is (0, 0, 0); where
+ *     reprojection_error_max == 0 every reprojection magnitude is 255;
+ *   - where B fails the reference reads an uninitialised fitted direction, pinned here as NaN: the angle pixel is
+ *     (0, 0, 127); the direction pixel is (255, 255, 255) (e = +inf clamps to 1);
+ *   - where A fails the magnitude, angle and direction pixels are 0 / (0, 0, 0), and the reprojection images see
+ *     r = 0, as in the reference's image, which holds zero wherever Project fails or is not tried;
+ *   - the reprojection-direction strength is max(0, min(1, |r| / -1)) = 0, because the tool passes
+ *     max_visualization_extent_pixels = -1, so that image is uniformly (127, 127, 127), as the reference writes it.
+ * device_ms (nullable): device time of the comparison and the images. Stand-alone; returns 2 for a bad argument
+ * (also a NULL image) before any CUDA call, 3 without a device. Repeated calls give identical bytes. */
+B200BA_API int b200ba_fitting_images(int device, const b200ba_camera* cam_a, const double* intr_a,
+                                     const b200ba_camera* cam_b, const double* intr_b, b200ba_fitting_report* report,
+                                     uint8_t* error_magnitudes, uint8_t* error_direction_angles,
+                                     uint8_t* error_directions, uint8_t* reprojection_magnitudes,
+                                     uint8_t* reprojections, double* device_ms);
 
 /* ---- localization accuracy test (APP/tools/localization_accuracy_test.cc:47-131, --localization_accuracy_test):
  * what the difference between a ground-truth calibration and a compared calibration of one camera costs a camera

@@ -160,6 +160,28 @@ class BundleAdjuster:
         _check(self.lib.b200ba_build_system(self._h, C.byref(opt), n, _dp(H), _dp(b), C.byref(cost)), self._h)
         return H, b, cost.value
 
+    def debug_solve_step(self, opt: Options, lam: float = -1.0, with_system: bool = True) -> Dict:
+        """One LM attempt's linear solve at the current state (``b200ba_debug_solve_step``): the reduced
+        system ``S`` (n_d x n_d, lower triangle valid) and right-hand side ``rhs`` the dense factorisation
+        receives, the update ``x``, and (``with_system``) ``H``, ``b`` of the same build. ``lam`` < 0: the LM's
+        first lambda. ``info`` names the path taken and the dense-phase variants in effect."""
+        n = self.degrees_of_freedom(opt)
+        H = np.zeros((n, n)) if with_system else None
+        b = np.zeros(n) if with_system else None
+        nbd = 3 * self.problem.n_points if opt.eliminate_points else 6 * self.problem.n_imagesets
+        nd = n - nbd
+        S = np.zeros((nd, nd), order="F")
+        rhs = np.zeros(nd)
+        x = np.zeros(n)
+        lam_used = C.c_double(0)
+        info = np.zeros(8, np.int32)
+        _check(self.lib.b200ba_debug_solve_step(self._h, C.byref(opt), float(lam), n, None if H is None else _dp(H),
+                                                None if b is None else _dp(b), _dp(S), _dp(rhs), _dp(x),
+                                                C.byref(lam_used), info.ctypes.data_as(C.POINTER(C.c_int32))), self._h)
+        names = ("spd", "use_grouped", "n_groups", "gemm", "panel", "trsv", "aux", "nb")
+        return {"H": H, "b": b, "S": S, "rhs": rhs, "x": x, "lambda": lam_used.value, "nbd": nbd,
+                "info": {k: int(v) for k, v in zip(names, info)}}
+
     def calibration_report(self, with_errors: bool = False):
         """CreateCalibrationReport's numbers (calibration_report.cc:83-98) for every camera on the device-resident
         state (``b200ba_calibration_report``). Returns (reports, errors, device_ms): one ``cabi.CameraReport``

@@ -449,6 +449,8 @@ SYMBOLS = {
     "b200ba_version": (C.c_char_p, []),
     "b200ba_debug_set_eval_budget": (None, [C.c_int]),
     "b200ba_debug_eval_counts": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint16)]),
+    "b200ba_debug_solve_step": (C.c_int, [C.c_void_p, C.POINTER(Options), C.c_double, C.c_int32, _D, _D, _D, _D, _D, _D,
+                                          _I32]),
 }
 
 

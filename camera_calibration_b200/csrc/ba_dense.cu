@@ -290,6 +290,13 @@ void launch_gemm_variant(const GemmArgs& g, bool lower, bool scatter, unsigned g
   else
     dgemm_nt_kernel<false, 0, BN_, BK, STAGES><<<grid, T, smem, s>>>(g);
 }
+// B200BA_GEMM=64 (default: 128 x 64 tiles, BK 16 x 4 stages, 2 CTAs / SM) | 128 (128 x 128 tiles, BK 32 x 3
+// stages, 1 CTA / SM) | 12816 (128 x 128, BK 16 x 4 stages). Read once per process.
+int gemm_variant() {
+  static int variant = -1;
+  if (variant < 0) variant = getenv("B200BA_GEMM") ? atoi(getenv("B200BA_GEMM")) : 64;
+  return variant;
+}
 }  // namespace
 
 int launch_dgemm_nt(const GemmArgs& g_in, bool lower, bool scatter, cudaStream_t s, bool leave_sms, bool one_tile_per_cta) {
@@ -299,10 +306,7 @@ int launch_dgemm_nt(const GemmArgs& g_in, bool lower, bool scatter, cudaStream_t
   int dev = 0;
   cudaGetDevice(&dev);
   bool& configured = configured_dev[dev & 63];  // function attributes are per device
-  // B200BA_GEMM=64 (default: 128 x 64 tiles, BK 16 x 4 stages, 2 CTAs / SM) | 128 (128 x 128 tiles, BK 32 x 3
-  // stages, 1 CTA / SM) | 12816 (128 x 128, BK 16 x 4 stages)
-  static int variant = -1;
-  if (variant < 0) variant = getenv("B200BA_GEMM") ? atoi(getenv("B200BA_GEMM")) : 64;
+  const int variant = gemm_variant();
   if (!configured) {
     configure_gemm_variant<64, 16, 4>();
     configure_gemm_variant<128, 32, 3>();
@@ -828,6 +832,24 @@ static int panel_version() {
   if (v < 0) v = getenv("B200BA_PANEL") ? atoi(getenv("B200BA_PANEL")) : 2;
   return v;
 }
+// B200BA_AUX=0 keeps the second look-ahead update of the single-GPU factorisation on the panel stream
+static bool aux_enabled() {
+  static const bool v = !(getenv("B200BA_AUX") && atoi(getenv("B200BA_AUX")) == 0);
+  return v;
+}
+// B200BA_TRSV=1: the first version of the triangular solves (one launch per tile, every CTA repeats the tile product)
+static int trsv_version() {
+  static int v = -1;
+  if (v < 0) v = getenv("B200BA_TRSV") ? atoi(getenv("B200BA_TRSV")) : 2;
+  return v;
+}
+
+void dense_variants(int* gemm, int* panel, int* trsv, int* aux) {
+  *gemm = gemm_variant();
+  *panel = panel_version();
+  *trsv = trsv_version();
+  *aux = aux_enabled() ? 1 : 0;
+}
 
 int dense_plan(DenseCtx* d, int n, int nb, int rank, int ranks) {
   d->n = n;
@@ -871,9 +893,7 @@ int dense_factor(DenseCtx* d) {
   const int sub_n = NB / PT;
   cudaStream_t sm = d->s_main, sp = d->s_panel;
   auto owner = [&](int k) { return k % R; };
-  // B200BA_AUX=0 keeps the second look-ahead update on the panel stream
-  static const bool aux_enabled = !(getenv("B200BA_AUX") && atoi(getenv("B200BA_AUX")) == 0);
-  const bool use_aux = aux_enabled && R == 1 && d->s_aux != nullptr;
+  const bool use_aux = aux_enabled() && R == 1 && d->s_aux != nullptr;
   // S is ready when everything queued on s_main so far has run
   cudaEventRecord(d->ev_misc, sm);
   cudaStreamWaitEvent(sp, d->ev_misc, 0);
@@ -1060,9 +1080,7 @@ int dense_solve(DenseCtx* d, double* b) {
     const int k = (t * PT) / NB, sub = (t * PT - k * NB) / PT;
     return d->Lpack + d->panel_off[k] + static_cast<int64_t>(d->panel_h[k]) * NB + static_cast<int64_t>(sub) * PT * PT;
   };
-  static int version = -1;  // B200BA_TRSV=1: the first version (one launch per tile, every CTA repeats the tile product)
-  if (version < 0) version = getenv("B200BA_TRSV") ? atoi(getenv("B200BA_TRSV")) : 2;
-  if (version == 2) {
+  if (trsv_version() == 2) {
     static bool configured_dev[64] = {};
     int dev = 0;
     cudaGetDevice(&dev);

@@ -163,6 +163,10 @@ struct b200ba_handle {
   cudaEvent_t ev_syrk[2] = {nullptr, nullptr}, ev_scatter[2] = {nullptr, nullptr}, ev_s_ready = nullptr;
   double* d_u = nullptr;
   bool use_grouped = false;
+  // b200ba_debug_solve_step: host buffers that receive S (n_d x n_d, column-major) and the reduced right-hand side
+  // between the Schur phase and the factorisation; null in every other call
+  double* capture_S = nullptr;
+  double* capture_rhs = nullptr;
   std::vector<double> grp_sums;           // [sx | sy | count] per Schur block (see build_groups)
   int force_grouped = -1;                 // B200BA_GROUPED=0|1 overrides the cost model
   bool compact_j = true;                  // B200BA_COMPACT_J=0: expanded Jacobian buffer also for central-generic cameras
@@ -832,6 +836,30 @@ int factor_dense(b200ba_handle* h) {
   return 0;
 }
 
+// b200ba_debug_solve_step (one rank): downloads S + lambda I as the factorisation will see it, un-mapped to a plain
+// column-major n_d x n_d array, and the reduced right-hand side.
+int capture_reduced_system(b200ba_handle* h) {
+  const Layout& L = h->L;
+  const int nd = L.nd;
+  if (nd > 0) {
+    if (h->own_dense) {
+      const DenseCtx& d = h->dn;
+      for (int j = 0; j < d.nblk; ++j) {
+        const int c0 = j * d.NB, w = std::min(d.NB, nd - c0);
+        CUDA_TRY(h, cudaMemcpy2DAsync(h->capture_S + static_cast<size_t>(c0) * nd, static_cast<size_t>(nd) * sizeof(double),
+                                      h->d_S + d.map.col_offset(c0), d.map.ld * sizeof(double),
+                                      static_cast<size_t>(nd) * sizeof(double), w, cudaMemcpyDeviceToHost, h->stream));
+      }
+    } else {
+      CUDA_TRY(h, cudaMemcpyAsync(h->capture_S, h->d_S, static_cast<size_t>(nd) * nd * sizeof(double), cudaMemcpyDeviceToHost,
+                                  h->stream));
+    }
+    CUDA_TRY(h, cudaMemcpyAsync(h->capture_rhs, h->d_x + L.nbd, static_cast<size_t>(nd) * sizeof(double),
+                                cudaMemcpyDeviceToHost, h->stream));
+  }
+  return sync_stream(h);
+}
+
 // Hot loop 2: Schur complement solve for a given lambda (LV/lm_optimizer.h:1246-1369).
 // Leaves x = [x_points | x_dense] in d_x. *spd = 0 when a factorisation met a non-positive pivot.
 int solve_system_own(b200ba_handle* h, double lambda, int* spd);
@@ -939,6 +967,7 @@ int solve_system(b200ba_handle* h, double lambda, int* spd) {
       h->timings.kernel_launches += 1;
     }
   }
+  if (h->capture_S && capture_reduced_system(h)) return 1;
   {
     ScopedPhase ph(h, PH_FACTOR);
     if (factor_dense(h)) return 1;
@@ -1084,6 +1113,7 @@ int solve_system_own(b200ba_handle* h, double lambda, int* spd) {
     if (L.nbd > 0 && nd > 0) launch_gemv_t(L.nbd, nd, nd, h->sys.B, h->d_u, -1.0, h->d_x + L.nbd, h->d_gemv_partial, h->stream);
     h->timings.kernel_launches += 4;
   }
+  if (h->capture_S && capture_reduced_system(h)) return 1;
   if (R > 1 && nd > 0) {
     // partial sums -> the block columns each rank owns (in place: rank r keeps chunk r)
     ScopedPhase ph(h, PH_ALLREDUCE);
@@ -1431,6 +1461,34 @@ LmResult small_lm(const int& rc, int max_iterations, System system, InitLambda i
     if (!applied || r.final_cost == 0) break;
   }
   return r;
+}
+
+// H (row-major upper triangle, the reference's variable order) and b of the last build_system.
+int download_system(b200ba_handle* h, double* H, double* b) {
+  const Layout& L = h->L;
+  const int n = L.dof;
+  std::vector<double> D(static_cast<size_t>(L.dsz) * L.nblocks), bp(L.nbd), B(static_cast<size_t>(L.nbd) * L.nd),
+      C(static_cast<size_t>(L.nd) * L.nd), bd(L.nd);
+  CUDA_TRY(h, cudaMemcpy(D.data(), h->sys.Dblk, D.size() * sizeof(double), cudaMemcpyDeviceToHost));
+  CUDA_TRY(h, cudaMemcpy(bp.data(), h->sys.bp, bp.size() * sizeof(double), cudaMemcpyDeviceToHost));
+  CUDA_TRY(h, cudaMemcpy(B.data(), h->sys.B, B.size() * sizeof(double), cudaMemcpyDeviceToHost));
+  CUDA_TRY(h, cudaMemcpy(C.data(), h->sys.C, C.size() * sizeof(double), cudaMemcpyDeviceToHost));
+  CUDA_TRY(h, cudaMemcpy(bd.data(), h->sys.bd, bd.size() * sizeof(double), cudaMemcpyDeviceToHost));
+  std::fill(H, H + static_cast<size_t>(n) * n, 0.0);
+  for (int p = 0; p < L.nblocks; ++p) {
+    const double* d = &D[static_cast<size_t>(L.dsz) * p];
+    const int o = L.bs * p;
+    for (int a2 = 0; a2 < L.bs; ++a2)
+      for (int b2 = a2; b2 < L.bs; ++b2)
+        H[static_cast<size_t>(o + a2) * n + o + b2] = d[a2 * L.bs - (a2 * (a2 - 1)) / 2 + (b2 - a2)];
+  }
+  for (int i = 0; i < L.nbd; ++i)
+    for (int k = 0; k < L.nd; ++k) H[static_cast<size_t>(i) * n + L.nbd + k] = B[static_cast<size_t>(i) * L.nd + k];
+  for (int i = 0; i < L.nd; ++i)
+    for (int k = i; k < L.nd; ++k) H[static_cast<size_t>(L.nbd + i) * n + L.nbd + k] = C[static_cast<size_t>(i) * L.nd + k];
+  for (int i = 0; i < L.nbd; ++i) b[i] = bp[i];
+  for (int i = 0; i < L.nd; ++i) b[L.nbd + i] = bd[i];
+  return 0;
 }
 
 }  // namespace
@@ -2215,27 +2273,40 @@ int b200ba_build_system(b200ba_handle* h, const b200ba_options* opt, int32_t n, 
   double c = 0, nv = 0;
   if (build_system(h, opt->huber_parameter, &c, &nv)) return 1;
   if (cost) *cost = c;
-  std::vector<double> D(static_cast<size_t>(L.dsz) * L.nblocks), bp(L.nbd), B(static_cast<size_t>(L.nbd) * L.nd),
-      C(static_cast<size_t>(L.nd) * L.nd), bd(L.nd);
-  CUDA_TRY(h, cudaMemcpy(D.data(), h->sys.Dblk, D.size() * sizeof(double), cudaMemcpyDeviceToHost));
-  CUDA_TRY(h, cudaMemcpy(bp.data(), h->sys.bp, bp.size() * sizeof(double), cudaMemcpyDeviceToHost));
-  CUDA_TRY(h, cudaMemcpy(B.data(), h->sys.B, B.size() * sizeof(double), cudaMemcpyDeviceToHost));
-  CUDA_TRY(h, cudaMemcpy(C.data(), h->sys.C, C.size() * sizeof(double), cudaMemcpyDeviceToHost));
-  CUDA_TRY(h, cudaMemcpy(bd.data(), h->sys.bd, bd.size() * sizeof(double), cudaMemcpyDeviceToHost));
-  std::fill(H, H + static_cast<size_t>(n) * n, 0.0);
-  for (int p = 0; p < L.nblocks; ++p) {
-    const double* d = &D[static_cast<size_t>(L.dsz) * p];
-    const int o = L.bs * p;
-    for (int a2 = 0; a2 < L.bs; ++a2)
-      for (int b2 = a2; b2 < L.bs; ++b2)
-        H[static_cast<size_t>(o + a2) * n + o + b2] = d[a2 * L.bs - (a2 * (a2 - 1)) / 2 + (b2 - a2)];
+  return download_system(h, H, b);
+}
+
+// Diagnostics / tests: one LM attempt's linear solve at the current state (see the header).
+int b200ba_debug_solve_step(b200ba_handle* h, const b200ba_options* opt, double lambda, int32_t n, double* H, double* b,
+                            double* S, double* rhs, double* x, double* lambda_used, int32_t info[8]) {
+  if (int rc = check_ready(h, opt)) return rc;
+  const Layout& L = h->L;
+  if (h->n_ranks > 1) {
+    h->error = "b200ba_debug_solve_step: the handle is joined to a communicator";
+    return 2;
   }
-  for (int i = 0; i < L.nbd; ++i)
-    for (int k = 0; k < L.nd; ++k) H[static_cast<size_t>(i) * n + L.nbd + k] = B[static_cast<size_t>(i) * L.nd + k];
-  for (int i = 0; i < L.nd; ++i)
-    for (int k = i; k < L.nd; ++k) H[static_cast<size_t>(L.nbd + i) * n + L.nbd + k] = C[static_cast<size_t>(i) * L.nd + k];
-  for (int i = 0; i < L.nbd; ++i) b[i] = bp[i];
-  for (int i = 0; i < L.nd; ++i) b[L.nbd + i] = bd[i];
+  if (n != L.dof || !S || !rhs || !x || !info) {
+    h->error = "b200ba_debug_solve_step: n does not equal the number of unknowns, or a required output is NULL";
+    return 2;
+  }
+  const bool any_fixed = opt->debug_fix_points || opt->debug_fix_poses || opt->debug_fix_rig_poses || opt->debug_fix_intrinsics;
+  double cost = 0, n_valid = 0;
+  if (build_system(h, opt->huber_parameter, &cost, &n_valid, any_fixed ? opt : nullptr)) return 1;
+  if (H && b && download_system(h, H, b)) return 1;
+  if (lambda < 0) lambda = opt->init_lambda_factor * h->trace_H / L.dof;
+  int spd = 1;
+  h->capture_S = S;
+  h->capture_rhs = rhs;
+  const int rc = solve_system(h, lambda, &spd);
+  h->capture_S = h->capture_rhs = nullptr;
+  if (rc) return rc;
+  CUDA_TRY(h, cudaMemcpy(x, h->d_x, static_cast<size_t>(L.dof) * sizeof(double), cudaMemcpyDeviceToHost));
+  if (lambda_used) *lambda_used = lambda;
+  info[0] = spd;
+  info[1] = h->use_grouped ? 1 : 0;
+  info[2] = h->n_groups;
+  dense_variants(&info[3], &info[4], &info[5], &info[6]);
+  info[7] = h->own_dense ? h->dn.NB : 0;
   return 0;
 }
 

@@ -186,5 +186,7 @@ struct DenseCtx {
 int dense_plan(DenseCtx* d, int n, int nb, int rank, int ranks);
 int dense_factor(DenseCtx* d);
 int dense_solve(DenseCtx* d, double* b);
+// the process-wide variants of the dense phase in effect (B200BA_GEMM, B200BA_PANEL, B200BA_TRSV, B200BA_AUX)
+void dense_variants(int* gemm, int* panel, int* trsv, int* aux);
 
 }  // namespace b200ba

@@ -517,6 +517,24 @@ B200BA_API void b200ba_debug_set_eval_budget(int budget);
 /* Spline evaluations the projection LM spent per observation in the last pass that wrote
  * Jacobians; counts [n_obs], caller's observation order. */
 B200BA_API int b200ba_debug_eval_counts(b200ba_handle* h, uint16_t* counts);
+/* One LM attempt's linear solve at the current state, with its intermediates: builds H, b (with the
+ * debug_fix_* masks of opt) and solves (H + lambda I) x = b with the kernels b200ba_optimize uses
+ * (B200BA_DENSE selects the in-tree or the cuBLAS / cuSOLVER dense phase). lambda < 0 means the LM's
+ * first lambda, init_lambda_factor * trace(H) / dof. n = the number of unknowns. Outputs (host):
+ *   H [n*n], b [n]   nullable; as b200ba_build_system returns them, from the same build
+ *   S [n_d*n_d]      the reduced system C + lambda I - B^T (D + lambda I)^-1 B as the factorisation
+ *                    receives it; column-major, lower triangle
+ *   rhs [n_d]        the reduced right-hand side b_d - B^T (D + lambda I)^-1 b_p
+ *   x [n]            the update, in b200ba_build_system's variable order
+ *   lambda_used      nullable
+ *   info [8]         positive definite (1 / 0), grouped contraction used, number of groups, and the
+ *                    dense-phase variants in effect: GEMM tile (64 | 128 | 12816), panel version,
+ *                    triangular-solve version, aux stream (1 / 0), block width (0 on the library path)
+ * n_d = n minus the unknowns of the eliminated blocks (points, or poses without eliminate_points).
+ * Returns 2 for a handle joined to a communicator. */
+B200BA_API int b200ba_debug_solve_step(b200ba_handle* h, const b200ba_options* opt, double lambda, int32_t n,
+                                       double* H, double* b, double* S, double* rhs, double* x,
+                                       double* lambda_used, int32_t info[8]);
 
 #ifdef __cplusplus
 }

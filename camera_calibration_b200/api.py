@@ -1116,3 +1116,29 @@ def LocalizationAccuracy(gt_model: CameraModel, compared_model: CameraModel, tri
                                             None if arrays is None else _dp(arrays["poses"]),
                                             None if arrays is None else fp(arrays["samples"]), C.byref(ms)))
     return report, arrays, ms.value
+
+
+def CompareReconstructions(state1: BAState, state2: BAState, pixel_step: int = 10, device: int = -1):
+    """The numbers of the ``--compare_reconstructions`` tool (tools/bundle_adjustment.cc:223-392) for two states of
+    one image sequence with one camera each (``b200ba_compare_reconstructions``; the steps and the deviations from
+    the reference are specified in include/b200ba.h): the direction sums over every ``pixel_step``-th pixel on the
+    device, Umeyama's scale, the intrinsics rotation and the endpoint drift on the host. Returns
+    (``cabi.ReconstructionComparison``, device_ms). Raises ``B200BAError`` for states that do not hold one camera
+    each or differ in image count, and for every library error (return code 4: the rotation is not determined)."""
+    if len(state1.intrinsics) != 1 or len(state2.intrinsics) != 1:
+        raise B200BAError("CompareReconstructions: each state must hold exactly one camera")
+    if len(state1.rig_tr_global) != len(state2.rig_tr_global):
+        raise B200BAError("CompareReconstructions: the states differ in image count")
+    lib = cabi.load_library()
+    m1, m2 = state1.intrinsics[0], state2.intrinsics[0]
+    c1, c2 = m1.c_camera(), m2.c_camera()
+    i1 = np.ascontiguousarray(m1.flat_intrinsics(), dtype=np.float64)
+    i2 = np.ascontiguousarray(m2.flat_intrinsics(), dtype=np.float64)
+    poses = [np.ascontiguousarray(a, dtype=np.float64) for a in
+             (state1.rig_tr_global, state1.camera_tr_rig[0], state2.rig_tr_global, state2.camera_tr_rig[0])]
+    report = cabi.ReconstructionComparison()
+    ms = C.c_double(0)
+    _check(lib.b200ba_compare_reconstructions(device, C.byref(c1), _dp(i1), C.byref(c2), _dp(i2),
+                                              len(state1.rig_tr_global), *[_dp(p) for p in poses], int(pixel_step),
+                                              C.byref(report), C.byref(ms)))
+    return report, ms.value

@@ -241,6 +241,22 @@ class LocalizationReport(C.Structure):
     ]
 
 
+class ReconstructionComparison(C.Structure):
+    """b200ba_reconstruction_comparison: the comparison of two bundle-adjusted reconstructions."""
+    _fields_ = [
+        ("direction_pairs", C.c_int64),
+        ("direction_sums", C.c_double * 9),
+        ("intrinsics1_r_intrinsics2", C.c_double * 9),
+        ("rotation_cost", C.c_double),
+        ("scale", C.c_double),
+        ("firstimage1_tr_firstimage2", C.c_double * 16),
+        ("endpoint_translation_difference", C.c_double),
+        ("trajectory_length1", C.c_double),
+        ("trajectory_length2", C.c_double),
+        ("relative_endpoint_difference", C.c_double),
+    ]
+
+
 class LineOffsetsReport(C.Structure):
     """b200ba_line_offsets_report: the centre-point analysis of a non-central camera."""
     _fields_ = [
@@ -432,6 +448,12 @@ SYMBOLS = {
     "b200ba_localization_accuracy": (C.c_int, [C.c_int, C.POINTER(Camera), _D, C.POINTER(Camera), _D, C.c_int64,
                                                C.c_uint64, C.POINTER(LocalizationReport), C.POINTER(C.c_float), _D,
                                                C.POINTER(C.c_float), _D]),
+    "b200ba_compare_reconstructions": (C.c_int, [C.c_int, C.POINTER(Camera), _D, C.POINTER(Camera), _D, C.c_int32, _D,
+                                                 _D, _D, _D, C.c_int32, C.POINTER(ReconstructionComparison), _D]),
+    "b200ba_reconstruction_directions": (C.c_int, [C.c_int, C.POINTER(Camera), _D, C.POINTER(Camera), _D, C.c_int32,
+                                                   C.POINTER(C.c_int32), _D]),
+    "b200ba_reconstruction_alignment": (C.c_int, [C.c_int64, _D, C.c_int32, _D, _D, _D, _D,
+                                                  C.POINTER(ReconstructionComparison)]),
     "b200ba_nccl_unique_id": (C.c_int, [C.POINTER(C.c_uint8)]),
     "b200ba_comm_init": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint8), C.c_int, C.c_int]),
     "b200ba_get_timings": (C.c_int, [C.c_void_p, C.POINTER(Timings)]),

@@ -168,6 +168,10 @@ struct LocalizationDev {
   ReportCam* stats;            // count / sum / max / median of the errors
 };
 
+// Reconstruction comparison (b200ba_compare_reconstructions): the count of sample pixels both models un-project and
+// the nine entries of M = sum d1 d2^T, row-major.
+constexpr int kSweepSums = 10;
+
 // Centre-point analysis of a non-central camera (b200ba_line_offsets): device buffers of one call. The n lines are
 // those of the pixels of the calibrated rectangle, p = (y - min_y) * rw + (x - min_x).
 constexpr int kLineSums = 10;  // per LM pass: cost, b (3), H (6: 00 01 02 11 12 22)

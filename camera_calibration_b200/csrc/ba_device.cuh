@@ -428,6 +428,82 @@ __device__ __forceinline__ void opencv_jacobians(const double* __restrict__ q, d
   Jy[10] = fy * (r2 + 2 * y2);
   Jy[11] = fy * 2 * xy;
 }
+// The distortion of normalised coordinates n -> (n radial + tangential) and its 2x2 derivative: the dxx, dxy, dyx,
+// dyy of opencv_jacobians, i.e. CentralOpenCVModel::ProjectInnerPartWithJacobian (central_opencv.cc:101-148) with
+// the derivative of the value it returns. (The reference's closed form of that Jacobian is not the derivative of its
+// value; the un-projection below only uses it as a search direction, and its accept / stop rules are the reference's.)
+__device__ __forceinline__ void opencv_distort(const double* __restrict__ q, double nx, double ny, double& ux,
+                                               double& uy, double J[2][2]) {
+  const double x2 = nx * nx, xy = nx * ny, y2 = ny * ny;
+  const double r2 = x2 + y2, r4 = r2 * r2, r6 = r4 * r2;
+  const double k1 = q[4], k2 = q[5], k3 = q[6], k4 = q[7], k5 = q[8], k6 = q[9], p1 = q[10], p2 = q[11];
+  const double num = 1 + k1 * r2 + k2 * r4 + k3 * r6;
+  const double den = 1 + k4 * r2 + k5 * r4 + k6 * r6;
+  const double iden = 1.0 / den;
+  const double radial = num * iden;
+  const double dnum = k1 + 2 * k2 * r2 + 3 * k3 * r4;
+  const double dden = k4 + 2 * k5 * r2 + 3 * k6 * r4;
+  const double drad = (dnum * den - num * dden) * iden * iden;
+  ux = nx * radial + (2.0 * p1 * xy + p2 * (r2 + 2.0 * x2));
+  uy = ny * radial + (2.0 * p2 * xy + p1 * (r2 + 2.0 * y2));
+  J[0][0] = radial + 2 * x2 * drad + 2 * p1 * ny + 6 * p2 * nx;
+  J[0][1] = 2 * xy * drad + 2 * p1 * nx + 2 * p2 * ny;
+  J[1][0] = 2 * xy * drad + 2 * p2 * ny + 2 * p1 * nx;
+  J[1][1] = radial + 2 * y2 * drad + 2 * p2 * nx + 6 * p1 * ny;
+}
+// CentralOpenCVModel::Unproject (central_opencv.cc:150-156): UnprojectWithGaussNewton (parametric.h:60-148) from the
+// normalised pixel, at most 100 iterations of up to 5 attempts (lambda_0 = 1.0 * 0.5 tr(H) at the first iteration,
+// x0.1 on an accepted attempt, x10 on a rejected one), stopping after an iteration that ends with cost < 1e-10f or
+// accepts nothing; then d = (x, y, 1) normalised. Returns false where the reference returns false.
+__device__ __forceinline__ bool opencv_unproject(const double* __restrict__ q, double x, double y, d3& d) {
+  const double dpx = (x - q[2]) / q[0], dpy = (y - q[3]) / q[1];
+  double cx = dpx, cy = dpy;
+  constexpr double kEpsilon = static_cast<double>(1e-10f);
+  double lambda = -1;
+  bool converged = false;
+  for (int i = 0; i < 100; ++i) {
+    double ux, uy, J[2][2];
+    opencv_distort(q, cx, cy, ux, uy, J);
+    double dx = ux - dpx, dy = uy - dpy;
+    double cost = dx * dx + dy * dy;
+    const double H00 = J[0][0] * J[0][0] + J[1][0] * J[1][0];
+    const double H01 = J[0][0] * J[0][1] + J[1][0] * J[1][1];
+    const double H11 = J[0][1] * J[0][1] + J[1][1] * J[1][1];
+    const double b0 = dx * J[0][0] + dy * J[1][0];
+    const double b1 = dx * J[0][1] + dy * J[1][1];
+    if (lambda < 0) lambda = 1.0 * (0.5 * (H00 + H11));
+    bool update_found = false;
+    for (int attempt = 0; attempt < 5; ++attempt) {
+      const double H00l = H00 + lambda, H11l = H11 + lambda;
+      const double x1 = (b1 - H01 / H00l * b0) / (H11l - H01 * H01 / H00l);
+      const double x0 = (b0 - H01 * x1) / H00l;
+      const double tx = cx - x0, ty = cy - x1;
+      double tux, tuy, TJ[2][2];
+      opencv_distort(q, tx, ty, tux, tuy, TJ);
+      dx = tux - dpx;
+      dy = tuy - dpy;
+      const double test_cost = dx * dx + dy * dy;
+      if (test_cost < cost) {
+        cost = test_cost;
+        cx = tx;
+        cy = ty;
+        lambda *= 0.1;
+        update_found = true;
+        break;
+      }
+      lambda *= 10;
+    }
+    if (cost < kEpsilon) {
+      converged = true;
+      break;
+    }
+    if (!update_found) break;
+  }
+  if (!converged) return false;
+  const double n = sqrt(cx * cx + cy * cy + 1.0);
+  d = mk3(cx / n, cy / n, 1.0 / n);
+  return true;
+}
 
 // ---- Huber (libvis loss_functions.h:94-133) ------------------------------------------------------
 __device__ __forceinline__ double huber_cost_sq(double h, double sq) {

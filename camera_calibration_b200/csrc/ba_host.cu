@@ -2822,6 +2822,374 @@ int b200ba_localization_accuracy(int device, const b200ba_camera* gt_cam, const 
   return cs.rc;
 }
 
+// ---- reconstruction comparison (APP/tools/bundle_adjustment.cc:223-392) -------------------------------------------
+// R(q) of a unit quaternion (w, x, y, z), row-major
+static void quat_matrix(const double* q, double R[9]) {
+  const double w = q[0], x = q[1], y = q[2], z = q[3];
+  R[0] = 1 - 2 * (y * y + z * z);
+  R[1] = 2 * (x * y - w * z);
+  R[2] = 2 * (x * z + w * y);
+  R[3] = 2 * (x * y + w * z);
+  R[4] = 1 - 2 * (x * x + z * z);
+  R[5] = 2 * (y * z - w * x);
+  R[6] = 2 * (x * z - w * y);
+  R[7] = 2 * (y * z + w * x);
+  R[8] = 1 - 2 * (x * x + y * y);
+}
+
+// image_tr_global = camera_tr_rig * rig_tr_global (Sophus: the product quaternion is normalised); its rotation R and
+// the centre -R^T t of its inverse G
+static void image_centre(const double* camera_tr_rig, const double* rig_tr_global, double R[9], double c[3]) {
+  const double* a = camera_tr_rig;
+  const double* b = rig_tr_global;
+  double q[4] = {a[0] * b[0] - a[1] * b[1] - a[2] * b[2] - a[3] * b[3],
+                 a[0] * b[1] + a[1] * b[0] + a[2] * b[3] - a[3] * b[2],
+                 a[0] * b[2] + a[2] * b[0] + a[3] * b[1] - a[1] * b[3],
+                 a[0] * b[3] + a[3] * b[0] + a[1] * b[2] - a[2] * b[1]};
+  const double n = std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
+  for (double& v : q) v /= n;
+  double Ra[9];
+  quat_matrix(a, Ra);
+  double t[3];
+  for (int r = 0; r < 3; ++r) t[r] = a[4 + r] + (Ra[3 * r] * b[4] + Ra[3 * r + 1] * b[5] + Ra[3 * r + 2] * b[6]);
+  quat_matrix(q, R);
+  for (int r = 0; r < 3; ++r) c[r] = -(R[r] * t[0] + R[3 + r] * t[1] + R[6 + r] * t[2]);
+}
+
+// Horn's quaternion method: for M = sum a b^T (a the targets, b the sources), the rotation R maximising tr(R^T M)
+// = sum a^T R b is R(q) for the unit eigenvector q of the largest eigenvalue of the symmetric 4 x 4 matrix N(M), and
+// that eigenvalue is the maximum. Cyclic Jacobi: a rotation is skipped where the off-diagonal entry is exactly zero, so
+// a block-diagonal N (M symmetric) keeps its first row untouched and gives q = (1, 0, 0, 0) exactly.
+static void horn_rotation(const double M[9], double R[9], double* lambda1, double* lambda2) {
+  // S = M^T: S_ij = sum b_i a_j (Horn 1987, eq. 28 ff.)
+  const double Sxx = M[0], Sxy = M[3], Sxz = M[6], Syx = M[1], Syy = M[4], Syz = M[7], Szx = M[2], Szy = M[5],
+               Szz = M[8];
+  double A[4][4] = {{Sxx + Syy + Szz, Syz - Szy, Szx - Sxz, Sxy - Syx},
+                    {Syz - Szy, Sxx - Syy - Szz, Sxy + Syx, Szx + Sxz},
+                    {Szx - Sxz, Sxy + Syx, -Sxx + Syy - Szz, Syz + Szy},
+                    {Sxy - Syx, Szx + Sxz, Syz + Szy, -Sxx - Syy + Szz}};
+  double V[4][4] = {{1, 0, 0, 0}, {0, 1, 0, 0}, {0, 0, 1, 0}, {0, 0, 0, 1}};
+  for (int sweep = 0; sweep < 64; ++sweep) {
+    bool rotated = false;
+    for (int p = 0; p < 3; ++p) {
+      for (int r = p + 1; r < 4; ++r) {
+        const double apq = A[p][r];
+        if (apq == 0) continue;
+        // negligible against both diagonal entries: set to zero (the classical Jacobi threshold)
+        if (std::fabs(A[p][p]) + 1e3 * std::fabs(apq) == std::fabs(A[p][p]) &&
+            std::fabs(A[r][r]) + 1e3 * std::fabs(apq) == std::fabs(A[r][r]) && sweep > 3) {
+          A[p][r] = A[r][p] = 0;
+          continue;
+        }
+        rotated = true;
+        const double theta = (A[r][r] - A[p][p]) / (2 * apq);
+        const double t = (theta >= 0 ? 1.0 : -1.0) / (std::fabs(theta) + std::sqrt(theta * theta + 1));
+        const double c = 1 / std::sqrt(t * t + 1), s = t * c;
+        for (int k = 0; k < 4; ++k) {  // A <- A J (columns p, r)
+          const double akp = A[k][p], akr = A[k][r];
+          A[k][p] = c * akp - s * akr;
+          A[k][r] = s * akp + c * akr;
+        }
+        for (int k = 0; k < 4; ++k) {  // A <- J^T A (rows p, r)
+          const double apk = A[p][k], ark = A[r][k];
+          A[p][k] = c * apk - s * ark;
+          A[r][k] = s * apk + c * ark;
+        }
+        A[p][r] = A[r][p] = 0;
+        for (int k = 0; k < 4; ++k) {
+          const double vkp = V[k][p], vkr = V[k][r];
+          V[k][p] = c * vkp - s * vkr;
+          V[k][r] = s * vkp + c * vkr;
+        }
+      }
+    }
+    if (!rotated) break;
+  }
+  int i1 = 0;
+  for (int k = 1; k < 4; ++k)
+    if (A[k][k] > A[i1][i1]) i1 = k;
+  int i2 = i1 == 0 ? 1 : 0;
+  for (int k = 0; k < 4; ++k)
+    if (k != i1 && A[k][k] > A[i2][i2]) i2 = k;
+  *lambda1 = A[i1][i1];
+  *lambda2 = A[i2][i2];
+  double q[4] = {V[0][i1], V[1][i1], V[2][i1], V[3][i1]};
+  const double n = std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
+  for (double& v : q) v /= n;
+  quat_matrix(q, R);
+}
+
+static double norm3(const double v[3]) { return std::sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]); }
+
+static bool centres_coincide(int32_t n, const double* rig_tr_global, const double* camera_tr_rig) {
+  double R[9], c0[3], c[3];
+  image_centre(camera_tr_rig, rig_tr_global, R, c0);
+  for (int32_t i = 1; i < n; ++i) {
+    image_centre(camera_tr_rig, rig_tr_global + 7 * static_cast<int64_t>(i), R, c);
+    if (c[0] != c0[0] || c[1] != c0[1] || c[2] != c0[2]) return false;
+  }
+  return true;
+}
+
+// argument checks of the host part; 0 or 2 (with g_create_error set)
+static int alignment_arguments(const char* who, int32_t n_images, const double* rtg1, const double* ctr1, const double* rtg2,
+                        const double* ctr2) {
+  const std::string prefix = std::string(who) + ": ";
+  if (!rtg1 || !ctr1 || !rtg2 || !ctr2) {
+    g_create_error = prefix + "a required argument is NULL";
+    return 2;
+  }
+  if (n_images < 2) {
+    g_create_error = prefix + "the reconstructions need at least two images";
+    return 2;
+  }
+  if (centres_coincide(n_images, rtg1, ctr1) || centres_coincide(n_images, rtg2, ctr2)) {
+    g_create_error = prefix + "all camera centres of a reconstruction coincide";
+    return 2;
+  }
+  return 0;
+}
+
+static int reconstruction_alignment(int64_t pairs, const double* M, int32_t n, const double* rtg1, const double* ctr1,
+                             const double* rtg2, const double* ctr2, b200ba_reconstruction_comparison* out) {
+  b200ba_reconstruction_comparison r{};
+  r.direction_pairs = pairs;
+  for (int k = 0; k < 9; ++k) r.direction_sums[k] = M[k];
+  // step 1: rotations of G_k[i]^-1 and the centres
+  std::vector<double> c1(3 * static_cast<size_t>(n)), c2(3 * static_cast<size_t>(n));
+  double R1_0[9], R2_0[9], Rtmp[9];
+  for (int32_t i = 0; i < n; ++i) {
+    image_centre(ctr1, rtg1 + 7 * static_cast<int64_t>(i), i == 0 ? R1_0 : Rtmp, &c1[3 * i]);
+    image_centre(ctr2, rtg2 + 7 * static_cast<int64_t>(i), i == 0 ? R2_0 : Rtmp, &c2[3 * i]);
+  }
+  // step 2: Umeyama's scale. Both sums are left undivided by n; their ratio is the same.
+  double m1[3] = {0, 0, 0}, m2[3] = {0, 0, 0};
+  for (int32_t i = 0; i < n; ++i)
+    for (int k = 0; k < 3; ++k) {
+      m1[k] += c1[3 * i + k];
+      m2[k] += c2[3 * i + k];
+    }
+  for (int k = 0; k < 3; ++k) {
+    m1[k] /= n;
+    m2[k] /= n;
+  }
+  double S[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}, V1[3] = {0, 0, 0};
+  for (int32_t i = 0; i < n; ++i) {
+    double a[3], b[3];
+    for (int k = 0; k < 3; ++k) {
+      a[k] = c2[3 * i + k] - m2[k];
+      b[k] = c1[3 * i + k] - m1[k];
+    }
+    for (int row = 0; row < 3; ++row)
+      for (int col = 0; col < 3; ++col) S[3 * row + col] += a[row] * b[col];
+    for (int k = 0; k < 3; ++k) V1[k] += b[k] * b[k];
+  }
+  double Rs[9], ls1, ls2;
+  horn_rotation(S, Rs, &ls1, &ls2);
+  const double s = ls1 / ((V1[0] + V1[1]) + V1[2]);
+  r.scale = s;
+  // step 4: the intrinsics rotation
+  double R[9], l1, l2;
+  horn_rotation(M, R, &l1, &l2);
+  for (int k = 0; k < 9; ++k) r.intrinsics1_r_intrinsics2[k] = R[k];
+  double trRM = 0;
+  for (int k = 0; k < 9; ++k) trRM += R[k] * M[k];
+  r.rotation_cost = static_cast<double>(pairs) - trRM;
+  if (pairs < 2 || !(l1 - l2 > 64 * std::numeric_limits<double>::epsilon() * std::fabs(l1))) {
+    *out = b200ba_reconstruction_comparison{};
+    out->direction_pairs = pairs;
+    for (int k = 0; k < 9; ++k) out->direction_sums[k] = M[k];
+    return 4;
+  }
+  // step 5: T = G1s[0] [R 0; 0 1] G2[0]^-1, G1s[0] = [R1_0^T | s c1[0]], G2[0]^-1 = [R2_0 | -R2_0 c2[0]]
+  double A[16] = {0}, B[16] = {0}, C[16] = {0};
+  for (int row = 0; row < 3; ++row) {
+    for (int col = 0; col < 3; ++col) {
+      A[4 * row + col] = R1_0[3 * col + row];
+      C[4 * row + col] = R2_0[3 * row + col];
+      B[4 * row + col] = R[3 * row + col];
+    }
+    A[4 * row + 3] = c1[row] * s;
+    C[4 * row + 3] = -(R2_0[3 * row] * c2[0] + R2_0[3 * row + 1] * c2[1] + R2_0[3 * row + 2] * c2[2]);
+  }
+  A[15] = B[15] = C[15] = 1;
+  double AB[16];
+  for (int i = 0; i < 4; ++i)
+    for (int j = 0; j < 4; ++j) {
+      double v = 0;
+      for (int k = 0; k < 4; ++k) v += A[4 * i + k] * B[4 * k + j];
+      AB[4 * i + j] = v;
+    }
+  for (int i = 0; i < 4; ++i)
+    for (int j = 0; j < 4; ++j) {
+      double v = 0;
+      for (int k = 0; k < 4; ++k) v += AB[4 * i + k] * C[4 * k + j];
+      r.firstimage1_tr_firstimage2[4 * i + j] = v;
+    }
+  // step 6
+  const double* c1b = &c1[3 * (n - 1)];
+  const double* c2b = &c2[3 * (n - 1)];
+  double d1[3], d2[3], e[3];
+  for (int k = 0; k < 3; ++k) {
+    d1[k] = c1b[k] - c1[k];
+    d2[k] = c2b[k] - c2[k];
+  }
+  double l1v[3], l2v[3];
+  for (int row = 0; row < 3; ++row) {
+    l1v[row] = R1_0[3 * row] * d1[0] + R1_0[3 * row + 1] * d1[1] + R1_0[3 * row + 2] * d1[2];
+    l2v[row] = R2_0[3 * row] * d2[0] + R2_0[3 * row + 1] * d2[1] + R2_0[3 * row + 2] * d2[2];
+  }
+  for (int row = 0; row < 3; ++row)
+    e[row] = (R[3 * row] * l2v[0] + R[3 * row + 1] * l2v[1] + R[3 * row + 2] * l2v[2]) - s * l1v[row];
+  r.endpoint_translation_difference = norm3(e);
+  double L1 = 0, L2 = 0;
+  for (int32_t i = 0; i + 1 < n; ++i) {
+    double a[3], b[3];
+    for (int k = 0; k < 3; ++k) {
+      a[k] = c1[3 * i + k] * s - c1[3 * (i + 1) + k] * s;
+      b[k] = c2[3 * i + k] - c2[3 * (i + 1) + k];
+    }
+    L1 += norm3(a);
+    L2 += norm3(b);
+  }
+  r.trajectory_length1 = L1;
+  r.trajectory_length2 = L2;
+  r.relative_endpoint_difference = r.endpoint_translation_difference / (0.5 * (L1 + L2));
+  *out = r;
+  return 0;
+}
+
+int b200ba_reconstruction_alignment(int64_t direction_pairs, const double* direction_sums, int32_t n_images,
+                                    const double* rig_tr_global1, const double* camera_tr_rig1,
+                                    const double* rig_tr_global2, const double* camera_tr_rig2,
+                                    b200ba_reconstruction_comparison* out) {
+  if (!direction_sums || !out) {
+    g_create_error = "b200ba_reconstruction_alignment: a required argument is NULL";
+    return 2;
+  }
+  if (int rc = alignment_arguments("b200ba_reconstruction_alignment", n_images, rig_tr_global1, camera_tr_rig1,
+                                   rig_tr_global2, camera_tr_rig2))
+    return rc;
+  const int rc = reconstruction_alignment(direction_pairs, direction_sums, n_images, rig_tr_global1, camera_tr_rig1,
+                                          rig_tr_global2, camera_tr_rig2, out);
+  if (rc == 4) g_create_error = "b200ba_reconstruction_alignment: the intrinsics rotation is not determined";
+  return rc;
+}
+
+// argument checks of the direction sweep; 0 or 2 (with g_create_error set)
+static int sweep_arguments(const std::string& prefix, const b200ba_camera* cam1, const double* intr1,
+                           const b200ba_camera* cam2, const double* intr2, int32_t pixel_step) {
+  if (!cam1 || !intr1 || !cam2 || !intr2) {
+    g_create_error = prefix + "a required argument is NULL";
+    return 2;
+  }
+  for (const b200ba_camera* c : {cam1, cam2}) {
+    if (c->model_type != B200BA_MODEL_CENTRAL_GENERIC && c->model_type != B200BA_MODEL_NONCENTRAL_GENERIC &&
+        c->model_type != B200BA_MODEL_CENTRAL_OPENCV) {
+      g_create_error = prefix + "the comparison is implemented for central-generic, non-central-generic and "
+                                "central-OpenCV models";
+      return 2;
+    }
+    if (c->model_type != B200BA_MODEL_CENTRAL_OPENCV && (c->grid_width < 4 || c->grid_height < 4)) {
+      g_create_error = prefix + "a grid is smaller than 4 x 4";
+      return 2;
+    }
+  }
+  if (cam1->width != cam2->width || cam1->height != cam2->height || cam1->width < 1 || cam1->height < 1) {
+    g_create_error = prefix + "the models differ in image size";
+    return 2;
+  }
+  if (pixel_step < 1) {
+    g_create_error = prefix + "pixel_step must be at least 1";
+    return 2;
+  }
+  return 0;
+}
+
+int b200ba_compare_reconstructions(int device, const b200ba_camera* cam1, const double* intr1,
+                                   const b200ba_camera* cam2, const double* intr2, int32_t n_images,
+                                   const double* rig_tr_global1, const double* camera_tr_rig1,
+                                   const double* rig_tr_global2, const double* camera_tr_rig2, int32_t pixel_step,
+                                   b200ba_reconstruction_comparison* out, double* device_ms) {
+  const std::string prefix = "b200ba_compare_reconstructions: ";
+  if (!out) {
+    g_create_error = prefix + "a required argument is NULL";
+    return 2;
+  }
+  if (int rc = sweep_arguments(prefix, cam1, intr1, cam2, intr2, pixel_step)) return rc;
+  if (int rc = alignment_arguments("b200ba_compare_reconstructions", n_images, rig_tr_global1, camera_tr_rig1,
+                                   rig_tr_global2, camera_tr_rig2))
+    return rc;
+  CallScope cs(&g_create_error);
+  if (int rc = cs.use_device(device)) return rc;
+  CamDev c1{}, c2{};
+  fill_camdev(*cam1, &c1);
+  fill_camdev(*cam2, &c2);
+  const int nx = (cam1->width + pixel_step - 1) / pixel_step, ny = (cam1->height + pixel_step - 1) / pixel_step;
+  const int64_t n1 = intrinsics_size(*cam1), n2 = intrinsics_size(*cam2);
+  double *d1 = nullptr, *d2 = nullptr, *partial = nullptr, *sums = nullptr;
+  cs.alloc(&d1, n1);
+  cs.alloc(&d2, n2);
+  cs.alloc(&partial, sweep_partial_blocks(nx, ny) * kSweepSums);
+  cs.alloc(&sums, kSweepSums);
+  double h[kSweepSums] = {};
+  if (cs.rc == 0) {
+    cs.ok(cudaMemcpy(d1, intr1, sizeof(double) * n1, cudaMemcpyHostToDevice));
+    cs.ok(cudaMemcpy(d2, intr2, sizeof(double) * n2, cudaMemcpyHostToDevice));
+  }
+  if (cs.rc == 0) {
+    cs.record(0, 0);
+    launch_reconstruction_sweep(c1, d1, c2, d2, pixel_step, nx, ny, partial, sums, 0);
+    cs.record(1, 0);
+    cs.ok(cudaGetLastError());
+    cs.ok(cudaMemcpy(h, sums, sizeof(h), cudaMemcpyDeviceToHost));
+  }
+  if (cs.rc != 0) return cs.rc;
+  if (device_ms) *device_ms = cs.elapsed_ms(0, 1);
+  const int rc = reconstruction_alignment(static_cast<int64_t>(h[0]), h + 1, n_images, rig_tr_global1, camera_tr_rig1,
+                                          rig_tr_global2, camera_tr_rig2, out);
+  if (rc == 4) {
+    g_create_error = prefix + "the intrinsics rotation is not determined (" + std::to_string(out->direction_pairs) +
+                     " sample pixels that both models un-project; rank of sum d1 d2^T below 2)";
+  }
+  return rc;
+}
+
+int b200ba_reconstruction_directions(int device, const b200ba_camera* cam1, const double* intr1,
+                                     const b200ba_camera* cam2, const double* intr2, int32_t pixel_step, int32_t* ok,
+                                     double* directions) {
+  const std::string prefix = "b200ba_reconstruction_directions: ";
+  if (!ok || !directions) {
+    g_create_error = prefix + "a required argument is NULL";
+    return 2;
+  }
+  if (int rc = sweep_arguments(prefix, cam1, intr1, cam2, intr2, pixel_step)) return rc;
+  CallScope cs(&g_create_error);
+  if (int rc = cs.use_device(device)) return rc;
+  CamDev c1{}, c2{};
+  fill_camdev(*cam1, &c1);
+  fill_camdev(*cam2, &c2);
+  const int nx = (cam1->width + pixel_step - 1) / pixel_step, ny = (cam1->height + pixel_step - 1) / pixel_step;
+  const int64_t n = static_cast<int64_t>(nx) * ny, n1 = intrinsics_size(*cam1), n2 = intrinsics_size(*cam2);
+  double *d1 = nullptr, *d2 = nullptr, *ddirs = nullptr;
+  int32_t* dok = nullptr;
+  cs.alloc(&d1, n1);
+  cs.alloc(&d2, n2);
+  cs.alloc(&ddirs, 6 * n);
+  cs.alloc(&dok, 2 * n);
+  if (cs.rc == 0) {
+    cs.ok(cudaMemcpy(d1, intr1, sizeof(double) * n1, cudaMemcpyHostToDevice));
+    cs.ok(cudaMemcpy(d2, intr2, sizeof(double) * n2, cudaMemcpyHostToDevice));
+  }
+  if (cs.rc == 0) {
+    launch_reconstruction_directions(c1, d1, c2, d2, pixel_step, nx, ny, dok, ddirs, 0);
+    cs.ok(cudaGetLastError());
+    cs.ok(cudaMemcpy(ok, dok, sizeof(int32_t) * 2 * n, cudaMemcpyDeviceToHost));
+    cs.ok(cudaMemcpy(directions, ddirs, sizeof(double) * 6 * n, cudaMemcpyDeviceToHost));
+  }
+  return cs.rc;
+}
+
 // Stand-alone Voronoi coverage rendering (allocates, computes, frees): what b200ba_report_images renders its
 // error maps with.
 int b200ba_render_voronoi(int device, int32_t width, int32_t height, int64_t n_sites, const int32_t* sites_q,

@@ -2592,6 +2592,125 @@ void launch_localization_pose(int64_t trials, const LocalizationDev& d, cudaStre
 }
 
 // ------------------------------------------------------------------------------------------
+// reconstruction comparison (b200ba_compare_reconstructions; the sample loop of APP/tools/bundle_adjustment.cc:280-294)
+// ------------------------------------------------------------------------------------------
+// Unproject(x, y, Line3d*) of a CG / NCG / OpenCV model followed by the tool's direction().normalized(); origins are
+// not used. The final normalisation is Eigen's: d / sqrt(|d|^2), |d|^2 without FMA.
+__device__ __forceinline__ bool sweep_unproject(const CamDev& c, const double* __restrict__ intr, double x, double y,
+                                                d3& d) {
+  d3 u;
+  if (c.model_type == B200BA_MODEL_CENTRAL_OPENCV) {
+    if (!opencv_unproject(intr, x, y, u)) return false;
+  } else {
+    if (!in_area(c, x, y)) return false;
+    if (c.model_type == B200BA_MODEL_CENTRAL_GENERIC) {
+      CentralEval e;
+      central_eval(c, intr, x, y, e);
+      u = e.u;
+    } else {
+      d3 o;
+      noncentral_line(c, intr, intr + 3 * static_cast<int64_t>(c.gw) * c.gh, x, y, o, u);
+    }
+  }
+  const double n = sqrt(__dadd_rn(__dadd_rn(__dmul_rn(u.x, u.x), __dmul_rn(u.y, u.y)), __dmul_rn(u.z, u.z)));
+  d = mk3(u.x / n, u.y / n, u.z / n);
+  return true;
+}
+// One thread per sample pixel (x, y) = (step i + 0.5, step j + 0.5) of the nx x ny sample grid, in 16 x 8 tiles. Pixels
+// that both models un-project add 1 and d1 d2^T to the block's kSweepSums sums; the block reduces them by a fixed
+// shared-memory tree into partial[block][kSweepSums] (the block's linear index), and sweep_stage2 adds the blocks in a
+// fixed order. Nothing depends on scheduling, so repeated calls give the same bits.
+constexpr int kSweepTileX = 16, kSweepTileY = 8, kSweepThreads = kSweepTileX * kSweepTileY;
+__global__ void __launch_bounds__(kSweepThreads)
+    reconstruction_sweep_kernel(CamDev c1, const double* __restrict__ intr1, CamDev c2,
+                                const double* __restrict__ intr2, int step, int nx, int ny,
+                                double* __restrict__ partial) {
+  const int i = blockIdx.x * kSweepTileX + threadIdx.x, j = blockIdx.y * kSweepTileY + threadIdx.y;
+  double s[kSweepSums];
+#pragma unroll
+  for (int k = 0; k < kSweepSums; ++k) s[k] = 0;
+  if (i < nx && j < ny) {
+    const double x = static_cast<double>(i) * step + 0.5, y = static_cast<double>(j) * step + 0.5;
+    d3 d1, d2;
+    if (sweep_unproject(c1, intr1, x, y, d1) && sweep_unproject(c2, intr2, x, y, d2)) {
+      s[0] = 1;
+      s[1] = d1.x * d2.x;
+      s[2] = d1.x * d2.y;
+      s[3] = d1.x * d2.z;
+      s[4] = d1.y * d2.x;
+      s[5] = d1.y * d2.y;
+      s[6] = d1.y * d2.z;
+      s[7] = d1.z * d2.x;
+      s[8] = d1.z * d2.y;
+      s[9] = d1.z * d2.z;
+    }
+  }
+  __shared__ double sh[kSweepSums][kSweepThreads];
+  const int t = threadIdx.y * kSweepTileX + threadIdx.x;
+#pragma unroll
+  for (int k = 0; k < kSweepSums; ++k) sh[k][t] = s[k];
+  __syncthreads();
+  for (int st = kSweepThreads / 2; st > 0; st >>= 1) {
+    if (t < st) {
+#pragma unroll
+      for (int k = 0; k < kSweepSums; ++k) sh[k][t] += sh[k][t + st];
+    }
+    __syncthreads();
+  }
+  if (t < kSweepSums) partial[(static_cast<int64_t>(blockIdx.y) * gridDim.x + blockIdx.x) * kSweepSums + t] = sh[t][0];
+}
+// sums[k] = sum over the blocks of partial[b][k]: block k of the grid, thread t adds blocks t, t + 256, ... in order,
+// then a fixed tree over the 256 threads.
+__global__ void __launch_bounds__(kReportThreads)
+    sweep_stage2(int64_t nblocks, const double* __restrict__ partial, double* __restrict__ sums) {
+  const int k = blockIdx.x;
+  double v = 0;
+  for (int64_t b = threadIdx.x; b < nblocks; b += kReportThreads) v += partial[b * kSweepSums + k];
+  __shared__ double sh[kReportThreads];
+  sh[threadIdx.x] = v;
+  __syncthreads();
+  for (int st = kReportThreads / 2; st > 0; st >>= 1) {
+    if (threadIdx.x < st) sh[threadIdx.x] += sh[threadIdx.x + st];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) sums[k] = sh[0];
+}
+// The per-pixel directions behind the sums: ok[2 p + k] and dirs[6 p + 3 k ..] of model k + 1 at sample p = j nx + i
+// (0 where the model does not un-project the pixel).
+__global__ void reconstruction_directions_kernel(CamDev c1, const double* __restrict__ intr1, CamDev c2,
+                                                 const double* __restrict__ intr2, int step, int nx, int ny,
+                                                 int32_t* __restrict__ ok, double* __restrict__ dirs) {
+  const int64_t p = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (p >= static_cast<int64_t>(nx) * ny) return;
+  const double x = static_cast<double>(p % nx) * step + 0.5, y = static_cast<double>(p / nx) * step + 0.5;
+#pragma unroll
+  for (int k = 0; k < 2; ++k) {
+    d3 d = mk3(0, 0, 0);
+    const bool r = sweep_unproject(k == 0 ? c1 : c2, k == 0 ? intr1 : intr2, x, y, d);
+    ok[2 * p + k] = r ? 1 : 0;
+    dirs[6 * p + 3 * k] = r ? d.x : 0.0;
+    dirs[6 * p + 3 * k + 1] = r ? d.y : 0.0;
+    dirs[6 * p + 3 * k + 2] = r ? d.z : 0.0;
+  }
+}
+void launch_reconstruction_directions(const CamDev& c1, const double* intr1, const CamDev& c2, const double* intr2,
+                                      int step, int nx, int ny, int32_t* ok, double* dirs, cudaStream_t s) {
+  const int64_t n = static_cast<int64_t>(nx) * ny;
+  reconstruction_directions_kernel<<<static_cast<unsigned>((n + 127) / 128), 128, 0, s>>>(c1, intr1, c2, intr2, step,
+                                                                                          nx, ny, ok, dirs);
+}
+int64_t sweep_partial_blocks(int nx, int ny) {
+  return static_cast<int64_t>((nx + kSweepTileX - 1) / kSweepTileX) * ((ny + kSweepTileY - 1) / kSweepTileY);
+}
+void launch_reconstruction_sweep(const CamDev& c1, const double* intr1, const CamDev& c2, const double* intr2,
+                                 int step, int nx, int ny, double* partial, double* sums, cudaStream_t s) {
+  const dim3 grid((nx + kSweepTileX - 1) / kSweepTileX, (ny + kSweepTileY - 1) / kSweepTileY);
+  reconstruction_sweep_kernel<<<grid, dim3(kSweepTileX, kSweepTileY), 0, s>>>(c1, intr1, c2, intr2, step, nx, ny,
+                                                                              partial);
+  sweep_stage2<<<kSweepSums, kReportThreads, 0, s>>>(sweep_partial_blocks(nx, ny), partial, sums);
+}
+
+// ------------------------------------------------------------------------------------------
 // centre-point analysis of a non-central camera (CreateCalibrationReportForCamera, APP/calibration_report.cc:839-982)
 // ------------------------------------------------------------------------------------------
 // The lines are evaluated once and stored (48 B per line: 55 MB for 1200 x 950, 576 MB for 4000 x 3000); every LM

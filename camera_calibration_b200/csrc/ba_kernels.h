@@ -64,6 +64,15 @@ void launch_compare_models(const CamDev& a, const double* ga, const CamDev& b, c
 void launch_localization_sample(const CamDev& gt, const double* ggt, const CamDev& cmp, const double* gcmp,
                                 int64_t trials, uint64_t seed, const LocalizationDev& d, cudaStream_t s);
 void launch_localization_pose(int64_t trials, const LocalizationDev& d, cudaStream_t s);
+// reconstruction comparison (b200ba_compare_reconstructions): over the nx x ny sample pixels (step i + 0.5,
+// step j + 0.5), sums[0] = pixels both models un-project, sums[1 + 3 r + c] = sum of d1[r] d2[c] over them;
+// partial holds sweep_partial_blocks(nx, ny) * kSweepSums doubles. intr1 / intr2 on the device.
+int64_t sweep_partial_blocks(int nx, int ny);
+void launch_reconstruction_sweep(const CamDev& c1, const double* intr1, const CamDev& c2, const double* intr2,
+                                 int step, int nx, int ny, double* partial, double* sums, cudaStream_t s);
+// the per-pixel un-projections of the same sample pixels: ok [2 nx ny], dirs [6 nx ny]
+void launch_reconstruction_directions(const CamDev& c1, const double* intr1, const CamDev& c2, const double* intr2,
+                                      int step, int nx, int ny, int32_t* ok, double* dirs, cudaStream_t s);
 // centre-point analysis of a non-central camera (b200ba_line_offsets); intr on the device. launch_line_pass stores
 // the line of every calibrated-rectangle pixel in d.lines; launch_line_system sums (mode 0) the cost, (1) + b,
 // (2) + H at the centre c into d.sums; launch_line_outputs computes the distances and their statistics, the

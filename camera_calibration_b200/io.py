@@ -618,3 +618,67 @@ def WriteFittingInfoFile(path: str, report) -> bool:
     except OSError:
         return False
     return True
+
+
+# ---------------------------------------------------------------------------------------
+# MeshLab project (the --compare_reconstructions output)
+# ---------------------------------------------------------------------------------------
+def _xml_attribute(b: bytes) -> bytes:
+    """tinyxml2's attribute escaping: & " ' < > become entities; every other byte is written as it is."""
+    return (b.replace(b"&", b"&amp;").replace(b'"', b"&quot;").replace(b"'", b"&apos;").replace(b"<", b"&lt;")
+            .replace(b">", b"&gt;"))
+
+
+def EncodeMeshLabProject(meshes) -> bytes:
+    """The bytes libvis' WriteMeshLabProject (external_io/meshlab_project.cc:81-111) saves through tinyxml2 for
+    ``meshes``, a list of (label, filename, 4 x 4 matrix): the matrix is cast to float32 and printed like std::ostream
+    prints a float (``%g``), every value followed by a space, every row by a newline. Labels and file names are str
+    (encoded like file names, os.fsencode) or bytes."""
+    out = [b"<MeshLabProject>\n    <MeshGroup>\n"]
+    for label, filename, matrix in meshes:
+        label = label if isinstance(label, bytes) else os.fsencode(label)
+        filename = filename if isinstance(filename, bytes) else os.fsencode(filename)
+        m = np.asarray(matrix, dtype=np.float32).reshape(4, 4)
+        rows = "".join("".join(f"{float(v):g} " for v in row) + "\n" for row in m)
+        out.append(b'        <MLMesh label="' + _xml_attribute(label) + b'" filename="' + _xml_attribute(filename)
+                   + b'">\n            <MLMatrix44>\n' + rows.encode() + b"</MLMatrix44>\n        </MLMesh>\n")
+    out.append(b"    </MeshGroup>\n</MeshLabProject>\n")
+    return b"".join(out)
+
+
+def WriteMeshLabProject(path, meshes) -> bool:
+    """Writes ``EncodeMeshLabProject(meshes)`` to ``path``; False if the file cannot be written."""
+    try:
+        with open(path, "wb") as f:
+            f.write(EncodeMeshLabProject(meshes))
+        return True
+    except OSError:
+        return False
+
+
+def _path_join(directory: bytes, name: bytes) -> bytes:
+    return directory + name if directory.endswith(b"/") else directory + b"/" + name
+
+
+def MeshLabProjectPaths(reconstruction_path_1, reconstruction_path_2, cwd=None):
+    """The path logic of tools/bundle_adjustment.cc:327-372, on the bytes of the two path strings: the longest common
+    prefix cut back to its last '/' is the project's directory; rest_k is path_k after the first differing byte (empty
+    when one path is a prefix of the other); a mesh file is absolute(path_k) + '/' + name (no '/' added after a
+    trailing one), absolute() prefixing cwd + '/' to a relative path without normalising it. Returns
+    (project_path, rest_1, rest_2, [points_1, poses_1, points_2, poses_2]) as bytes."""
+    p1, p2 = os.fsencode(reconstruction_path_1), os.fsencode(reconstruction_path_2)
+    cwd = os.fsencode(os.getcwd() if cwd is None else cwd)
+    n = 0
+    while n < min(len(p1), len(p2)) and p1[n] == p2[n]:
+        n += 1
+    prefix = p1[:n]
+    rest1 = rest2 = b""
+    if n < min(len(p1), len(p2)):
+        rest1, rest2 = p1[n:], p2[n:]
+    cut = prefix.rfind(b"/")
+    prefix = prefix[:cut + 1]
+    files = []
+    for p in (p1, p2):
+        absolute = p if p.startswith(b"/") else _path_join(cwd, p)
+        files += [_path_join(absolute, b"points.yaml.obj"), _path_join(absolute, b"rig_tr_global.yaml.obj")]
+    return prefix + b"reconstructions_aligned_at_start.mlp", rest1, rest2, files

@@ -437,6 +437,69 @@ B200BA_API int b200ba_localization_accuracy(int device, const b200ba_camera* gt_
                                             uint64_t seed, b200ba_localization_report* report, float* errors,
                                             double* poses, float* samples, double* device_ms);
 
+/* ---- reconstruction comparison (APP/tools/bundle_adjustment.cc:223-392, --compare_reconstructions): how far two
+ * bundle-adjusted reconstructions of one image sequence -- e.g. one per calibration of the camera -- drift apart.
+ * Poses are [qw qx qy qz tx ty tz] (Sophus order: (a * b).q = normalize(a.q b.q), (a * b).t = a.t + R(a.q) b.t).
+ *   1. G_k[i] = (camera_tr_rig_k * rig_tr_global_k[i])^-1 for every image i (image_used is not consulted); the
+ *      centre c_k[i] = G_k[i].t = -R^T t of the composed pose.
+ *   2. Scale: Umeyama with scaling from c_1 to c_2, in double (the reference runs it in float):
+ *      s = lambda_max(N(S)) / sum_i |c_1[i] - mean c_1|^2, S = sum_i (c_2[i] - mean c_2)(c_1[i] - mean c_1)^T, where
+ *      lambda_max(N(S)) is Horn's quaternion form of max over rotations R of tr(R^T S) (= Umeyama's tr(D S_sign)).
+ *   3. Directions: every sample pixel (x + 0.5, y + 0.5), x = 0, step, ... < width, y likewise, that BOTH models
+ *      un-project (Unproject(x, y, Line3d*): CG / NCG inside the calibrated area; OpenCV by the reference's
+ *      UnprojectWithGaussNewton, parametric.h:60-148, whose iteration uses the exact derivative of the distortion);
+ *      d_k = the unit line direction, normalised once more (origins are ignored). M = sum d1 d2^T on the device,
+ *      one thread per sample pixel, summed in a fixed order (repeated calls give the same bits).
+ *   4. R = intrinsics1_r_intrinsics2 = the exact minimiser of sum |R d2 - d1|^2 over rotations: the unit eigenvector
+ *      of the largest eigenvalue of Horn's symmetric 4 x 4 matrix N(M) (cyclic Jacobi in double), as a rotation
+ *      matrix. The reference reports the point where an LM run from the identity stops instead. rotation_cost is
+ *      evaluated as direction_pairs - sum_ij R_ij M_ij, the identity for unit directions (absolute rounding error
+ *      about direction_pairs * 2^-52).
+ *   5. T = firstimage1_tr_firstimage2 = G1s[0].matrix() * [R 0; 0 1] * G2[0]^-1.matrix(), G1s = G_1 with its
+ *      translations multiplied by s.
+ *   6. endpoint_translation_difference e = |(T G2[n-1]).t - G1s[n-1].t|, evaluated as
+ *      |R (R2_0^T (c_2[n-1] - c_2[0])) - s (R1_0^T (c_1[n-1] - c_1[0]))| with R_k0 the rotation of G_k[0]^-1 (the same
+ *      number without forming T, so that two identical states give exactly 0); trajectory_length1 = sum_i
+ *      |s c_1[i] - s c_1[i+1]|, trajectory_length2 = sum_i |c_2[i] - c_2[i+1]|; relative_endpoint_difference
+ *      = e / (0.5 (trajectory_length1 + trajectory_length2)). */
+typedef struct b200ba_reconstruction_comparison {
+  int64_t direction_pairs;             /* sample pixels both models un-project */
+  double direction_sums[9];            /* M = sum d1 d2^T, row-major */
+  double intrinsics1_r_intrinsics2[9]; /* row-major: the minimiser of sum |R d2 - d1|^2 */
+  double rotation_cost;                /* 1/2 sum |R d2 - d1|^2 at that R */
+  double scale;                        /* s */
+  double firstimage1_tr_firstimage2[16]; /* row-major 4 x 4 */
+  double endpoint_translation_difference, trajectory_length1, trajectory_length2, relative_endpoint_difference;
+} b200ba_reconstruction_comparison;
+/* Stand-alone (allocates, computes, frees). cam1 / intr1 and cam2 / intr2: the single camera of each reconstruction,
+ * central-generic, non-central-generic or central-OpenCV, of one image size. rig_tr_global1 / 2: [7 n_images];
+ * camera_tr_rig1 / 2: [7]. device_ms (nullable): device time of the direction sweep. Returns 2 for a bad argument
+ * before any CUDA call (a NULL pointer, another model type, a generic grid smaller than 4 x 4, different image sizes,
+ * n_images < 2, pixel_step < 1, or all centres of one reconstruction equal: the reference divides by zero there),
+ * 3 without a device, 4 when the rotation is not determined: fewer than two direction pairs or
+ * lambda_1 - lambda_2 <= 64 * 2^-52 * |lambda_1| for the two largest eigenvalues of N(M) (this includes rank M < 2).
+ * On 4, out holds the pairs and M. */
+B200BA_API int b200ba_compare_reconstructions(int device, const b200ba_camera* cam1, const double* intr1,
+                                              const b200ba_camera* cam2, const double* intr2, int32_t n_images,
+                                              const double* rig_tr_global1, const double* camera_tr_rig1,
+                                              const double* rig_tr_global2, const double* camera_tr_rig2,
+                                              int32_t pixel_step, b200ba_reconstruction_comparison* out,
+                                              double* device_ms);
+/* The sample-pixel directions behind direction_sums, pixel by pixel (inspection and tests): for sample p = j nx + i,
+ * nx = ceil(width / pixel_step), ok[2 p + k] = 1 where model k + 1 un-projects (step i + 0.5, step j + 0.5) and
+ * directions[6 p + 3 k + c] its direction as step 3 defines it (0 otherwise). ok [2 nx ny], directions [6 nx ny].
+ * The argument checks of b200ba_compare_reconstructions for the models and the step (2); 3 without a device. */
+B200BA_API int b200ba_reconstruction_directions(int device, const b200ba_camera* cam1, const double* intr1,
+                                                const b200ba_camera* cam2, const double* intr2, int32_t pixel_step,
+                                                int32_t* ok, double* directions);
+/* The host part of b200ba_compare_reconstructions (steps 1, 2 and 4-6) from given direction sums: fills every field
+ * of out from direction_pairs and M [9]. Needs no device; returns 2 for a NULL pointer, n_images < 2 or coinciding
+ * centres, 4 when the rotation is not determined (out then holds the pairs and M). */
+B200BA_API int b200ba_reconstruction_alignment(int64_t direction_pairs, const double* direction_sums, int32_t n_images,
+                                               const double* rig_tr_global1, const double* camera_tr_rig1,
+                                               const double* rig_tr_global2, const double* camera_tr_rig2,
+                                               b200ba_reconstruction_comparison* out);
+
 /* ---- centre-point analysis of a non-central camera: the NoncentralGenericModel branch of
  * CreateCalibrationReportForCamera (APP/calibration_report.cc:839-982, with CenterPointCostFunction of :56-80).
  *   1. every pixel (x + 0.5f, y + 0.5f) of the calibrated area is un-projected to a line (o, d) (:847-856);

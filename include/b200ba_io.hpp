@@ -677,4 +677,190 @@ inline bool LoadBAState(const char* base_path, BAState* state, Dataset* dataset)
   return true;
 }
 
+// ---- COLMAP text model (the --bundle_adjustment input) ---------------------------------------------------------
+// libvis/src/libvis/external_io/colmap_model.cc:96-142: two lines per image, "IMAGE_ID QW QX QY QZ TX TY TZ CAMERA_ID
+// NAME" then "X Y POINT3D_ID ..."; the pose is parsed into float like the reference's SE3f, the observations as double
+// and then cast to float (io.py reads them the same way). Lines that are empty or start with '#' are skipped.
+struct ColmapObservation {
+  Vec2f xy;
+  long long point3d_id;
+};
+struct ColmapImage {
+  int image_id = 0;
+  float q[4] = {1, 0, 0, 0};  // qw qx qy qz
+  float t[3] = {0, 0, 0};
+  int camera_id = 0;
+  std::string file_path;
+  std::vector<ColmapObservation> observations;
+};
+namespace io_detail {
+inline std::vector<std::string> split_lines(const std::string& text) {
+  std::vector<std::string> lines;
+  size_t begin = 0;
+  while (true) {
+    const size_t end = text.find('\n', begin);
+    lines.push_back(text.substr(begin, end == std::string::npos ? std::string::npos : end - begin));
+    if (end == std::string::npos) break;
+    begin = end + 1;
+  }
+  return lines;
+}
+inline std::vector<std::string> split_fields(const std::string& line) {
+  std::istringstream in(line);
+  std::vector<std::string> fields;
+  std::string f;
+  while (in >> f) fields.push_back(f);
+  return fields;
+}
+}  // namespace io_detail
+
+// Returns false if the file cannot be read or a line is malformed; `images` is keyed (and so ordered) by image id.
+inline bool ReadColmapImages(const std::string& images_txt_path, bool read_observations,
+                             std::map<int, ColmapImage>* images) {
+  using namespace io_detail;
+  std::string text;
+  if (!read_file(images_txt_path, &text)) return false;
+  const std::vector<std::string> lines = split_lines(text);
+  images->clear();
+  size_t i = 0;
+  while (i < lines.size()) {
+    const std::string& line = lines[i++];
+    if (line.empty() || line[0] == '#') continue;
+    const std::vector<std::string> f = split_fields(line);
+    if (f.size() < 9) return false;
+    ColmapImage image;
+    char* end = nullptr;
+    image.image_id = std::atoi(f[0].c_str());
+    for (int k = 0; k < 4; ++k) image.q[k] = std::strtof(f[1 + k].c_str(), &end);
+    for (int k = 0; k < 3; ++k) image.t[k] = std::strtof(f[5 + k].c_str(), &end);
+    image.camera_id = std::atoi(f[8].c_str());
+    if (f.size() > 9) image.file_path = f[9];
+    const std::string obs_line = i < lines.size() ? lines[i] : std::string();
+    ++i;
+    if (read_observations) {
+      const std::vector<std::string> v = split_fields(obs_line);
+      for (size_t k = 0; k + 2 < v.size(); k += 3) {
+        ColmapObservation o;
+        o.xy = Vec2f{static_cast<float>(std::strtod(v[k].c_str(), &end)),
+                     static_cast<float>(std::strtod(v[k + 1].c_str(), &end))};
+        o.point3d_id = static_cast<long long>(std::strtod(v[k + 2].c_str(), &end));
+        image.observations.push_back(o);
+      }
+    }
+    (*images)[image.image_id] = image;
+  }
+  return true;
+}
+
+// colmap_model.cc:265-299: "ID X Y Z R G B ERROR track..." (positions as float; colours, error and tracks ignored)
+inline bool ReadColmapPoints3D(const std::string& points3d_txt_path, std::map<int, Vec3d>* points) {
+  using namespace io_detail;
+  std::string text;
+  if (!read_file(points3d_txt_path, &text)) return false;
+  points->clear();
+  for (const std::string& line : split_lines(text)) {
+    if (line.empty() || line[0] == '#') continue;
+    const std::vector<std::string> f = split_fields(line);
+    if (f.size() < 4) return false;
+    char* end = nullptr;
+    (*points)[std::atoi(f[0].c_str())] = Vec3d{static_cast<double>(std::strtof(f[1].c_str(), &end)),
+                                               static_cast<double>(std::strtof(f[2].c_str(), &end)),
+                                               static_cast<double>(std::strtof(f[3].c_str(), &end))};
+  }
+  return true;
+}
+
+// tools/bundle_adjustment.cc:110-184: a COLMAP text model and the camera `model` -> (dataset, state). Images and
+// points are ordered by increasing id, observations without a 3D point (id -1) are dropped, the single rig pose is the
+// identity and every image is used; the float quaternion is normalised in double. Returns false if a file cannot be
+// read; throws std::out_of_range for an observation of an unknown point.
+inline bool LoadColmapProblem(const std::shared_ptr<CameraModel>& model, const std::string& model_input_directory,
+                              std::shared_ptr<Dataset>* dataset, BAState* state) {
+  using namespace io_detail;
+  std::map<int, ColmapImage> images;
+  std::map<int, Vec3d> points;
+  if (!ReadColmapImages(join(model_input_directory, "images.txt"), true, &images) ||
+      !ReadColmapPoints3D(join(model_input_directory, "points3D.txt"), &points))
+    return false;
+  auto ds = std::make_shared<Dataset>(1);
+  ds->SetImageSize(0, model->width(), model->height());
+  BAState st;
+  st.intrinsics = {model};
+  st.camera_tr_rig = {SE3d()};
+  st.image_used.assign(images.size(), true);
+  for (const auto& item : images) {
+    const ColmapImage& image = item.second;
+    const double q[4] = {image.q[0], image.q[1], image.q[2], image.q[3]};
+    const double n = std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
+    SE3d T;
+    T.qw = q[0] / n; T.qx = q[1] / n; T.qy = q[2] / n; T.qz = q[3] / n;
+    T.tx = image.t[0]; T.ty = image.t[1]; T.tz = image.t[2];
+    st.rig_tr_global.push_back(T);
+    std::shared_ptr<Imageset> set = ds->NewImageset();
+    set->SetFilename(image.file_path);
+    for (const ColmapObservation& o : image.observations) {
+      if (o.point3d_id < 0) continue;
+      PointFeature feature;
+      feature.xy = o.xy;
+      feature.id = static_cast<int>(o.point3d_id);
+      set->FeaturesOfCamera(0).push_back(feature);
+    }
+  }
+  for (const auto& item : points) {
+    st.feature_id_to_points_index[item.first] = static_cast<int>(st.points.size());
+    st.points.push_back(item.second);
+  }
+  st.ComputeFeatureIdToPointsIndex(ds.get());
+  *dataset = ds;
+  *state = st;
+  return true;
+}
+
+// ---- MeshLab project (the --compare_reconstructions output) -------------------------------------------------------
+// The bytes libvis' WriteMeshLabProject (external_io/meshlab_project.cc:81-111) saves through tinyxml2: one <MLMesh>
+// per mesh, attributes escaped as tinyxml2 escapes them (& " ' < >), the matrix cast to float and printed as
+// std::ostream prints a float (%g), each value followed by a space and each row by a newline. io.py's
+// EncodeMeshLabProject writes the same bytes.
+struct MeshLabMesh {
+  std::string label, filename;
+  double global_tr_mesh[16];  // row-major
+};
+namespace io_detail {
+inline std::string xml_attribute(const std::string& s) {
+  std::string out;
+  for (char ch : s) {
+    switch (ch) {
+      case '&': out += "&amp;"; break;
+      case '"': out += "&quot;"; break;
+      case '\'': out += "&apos;"; break;
+      case '<': out += "&lt;"; break;
+      case '>': out += "&gt;"; break;
+      default: out += ch;
+    }
+  }
+  return out;
+}
+}  // namespace io_detail
+inline std::string EncodeMeshLabProject(const std::vector<MeshLabMesh>& meshes) {
+  using namespace io_detail;
+  std::string out = "<MeshLabProject>\n    <MeshGroup>\n";
+  for (const MeshLabMesh& mesh : meshes) {
+    out += "        <MLMesh label=\"" + xml_attribute(mesh.label) + "\" filename=\"" + xml_attribute(mesh.filename) +
+           "\">\n            <MLMatrix44>\n";
+    for (int r = 0; r < 4; ++r) {
+      for (int c = 0; c < 4; ++c) {
+        char buf[64];
+        std::snprintf(buf, sizeof(buf), "%g ", static_cast<double>(static_cast<float>(mesh.global_tr_mesh[4 * r + c])));
+        out += buf;
+      }
+      out += "\n";
+    }
+    out += "</MLMatrix44>\n        </MLMesh>\n";
+  }
+  return out + "    </MeshGroup>\n</MeshLabProject>\n";
+}
+inline bool WriteMeshLabProject(const std::string& path, const std::vector<MeshLabMesh>& meshes) {
+  return io_detail::write_file(path, EncodeMeshLabProject(meshes));
+}
+
 }  // namespace b200ba_shim

@@ -1,7 +1,7 @@
 // b200ba_pipeline.hpp -- C++ host logic of the callers either side of the hot path (SURVEY.md 8f-3 / 8f-4):
 // the outlier deletion between bundle-adjustment rounds, the metric rescaling, the pyramid resampling of the generic
-// models, the calibration report's info files, the comparison of two calibrations and the localization accuracy test,
-// over the containers of
+// models, the calibration report's info files, the comparison of two calibrations, the localization accuracy test and
+// the --bundle_adjustment / --compare_reconstructions tools, over the containers of
 // b200ba_shim.hpp. (RunBundleAdjustment itself -- 8f-2 -- is in b200ba_shim.hpp and runs device-resident in the
 // library.) The Python mirror is camera_calibration_b200/pipeline.py.
 //
@@ -746,6 +746,153 @@ inline int LocalizationAccuracyTest(const std::string& gt_model_yaml_path, const
   std::cout << "Average error [mm]: " << (1000 * report.average_error) << "\n";
   std::cout << "Median error [mm]: " << (1000 * report.median_error) << "\n";
   std::cout.flush();
+  return EXIT_SUCCESS;
+}
+
+// ---- --bundle_adjustment and --compare_reconstructions (tools/bundle_adjustment.cc) --------------------------------
+// :50-220: load <state_directory>/intrinsics0.yaml and the COLMAP text model (LoadColmapProblem), run
+// max_iteration_count single LM iterations (localize_only, eliminate_points, dense Schur mode) and write the state
+// directory and cost.txt (14 significant digits) after every iteration. Returns EXIT_SUCCESS / EXIT_FAILURE; throws on
+// a library error. pipeline.BundleAdjustment is the Python mirror.
+inline int BundleAdjustment(const std::string& state_directory, const std::string& model_input_directory,
+                            const std::string& model_output_directory, int max_iteration_count = 30) {
+  std::shared_ptr<CameraModel> model = LoadCameraModel(io_detail::join(state_directory, "intrinsics0.yaml").c_str());
+  if (!model) return EXIT_FAILURE;
+  std::shared_ptr<Dataset> dataset;
+  BAState state;
+  if (!LoadColmapProblem(model, model_input_directory, &dataset, &state)) return EXIT_FAILURE;
+  double lambda = -1;
+  for (int iteration = 0; iteration < max_iteration_count; ++iteration) {
+    const double cost = OptimizeJointly(*dataset, &state, 1, lambda, 1e-4, 0, true, true, SchurMode::Dense, &lambda,
+                                        nullptr, false, false, false, false, false, /*print_progress*/ false);
+    SaveBAState(model_output_directory.c_str(), state);
+    io_detail::write_file(io_detail::join(model_output_directory, "cost.txt"), io_detail::num(cost) + "\n");
+  }
+  return EXIT_SUCCESS;
+}
+
+// The MeshLab project's paths (:327-372) on the bytes of the two path strings: the project's directory is their
+// longest common prefix cut back to its last '/'; rest_k is path_k from the first differing byte on (empty when one
+// path is a prefix of the other); a mesh file is absolute(path_k) + '/' + name, without a second '/' after a trailing
+// one, absolute() prefixing the working directory + '/' to a relative path without normalising it.
+struct MeshLabProjectPaths {
+  std::string project, rest1, rest2;
+  std::string files[4];  // points 1, poses 1, points 2, poses 2
+};
+inline MeshLabProjectPaths ReconstructionProjectPaths(const std::string& path1, const std::string& path2,
+                                                      const std::string& cwd) {
+  MeshLabProjectPaths r;
+  size_t n = 0;
+  while (n < std::min(path1.size(), path2.size()) && path1[n] == path2[n]) ++n;
+  if (n < std::min(path1.size(), path2.size())) {
+    r.rest1 = path1.substr(n);
+    r.rest2 = path2.substr(n);
+  }
+  const size_t cut = path1.substr(0, n).rfind('/');
+  r.project = (cut == std::string::npos ? std::string() : path1.substr(0, cut + 1)) + "reconstructions_aligned_at_start.mlp";
+  const std::string* paths[2] = {&path1, &path2};
+  for (int k = 0; k < 2; ++k) {
+    const std::string absolute = (!paths[k]->empty() && (*paths[k])[0] == '/') ? *paths[k] : io_detail::join(cwd, *paths[k]);
+    r.files[2 * k] = io_detail::join(absolute, "points.yaml.obj");
+    r.files[2 * k + 1] = io_detail::join(absolute, "rig_tr_global.yaml.obj");
+  }
+  return r;
+}
+
+// :223-392: load both state directories, compare them on the device (b200ba_compare_reconstructions, every
+// pixel_step-th pixel), print "intrinsics1_r_intrinsics2_4x4:", four rows of %.6g values separated by single spaces and
+// "relative endpoint difference: <%.6g of 100 rel>%" to stdout, and write reconstructions_aligned_at_start.mlp.
+// Returns EXIT_SUCCESS, also when the project cannot be written (a message on stderr, as in the reference), and
+// EXIT_FAILURE with a message on stderr where a state does not load, the states differ in image count, camera count
+// or image size (the reference aborts), or the library refuses them (return codes 2 and 4). pipeline.py's
+// CompareReconstructions prints and writes the same bytes.
+inline int CompareReconstructions(const std::string& reconstruction_path_1, const std::string& reconstruction_path_2,
+                                  int pixel_step = 10) {
+  BAState states[2];
+  const std::string* paths[2] = {&reconstruction_path_1, &reconstruction_path_2};
+  for (int k = 0; k < 2; ++k) {
+    if (!LoadBAState(paths[k]->c_str(), &states[k], nullptr)) {
+      std::cerr << "Cannot load reconstruction: " << *paths[k] << "\n";
+      return EXIT_FAILURE;
+    }
+  }
+  const BAState& s1 = states[0];
+  const BAState& s2 = states[1];
+  if (s1.rig_tr_global.size() != s2.rig_tr_global.size()) {
+    std::cerr << "The reconstructions differ in image count (" << s1.rig_tr_global.size() << " against "
+              << s2.rig_tr_global.size() << ").\n";
+    return EXIT_FAILURE;
+  }
+  if (s1.intrinsics.size() != 1 || s2.intrinsics.size() != 1) {
+    std::cerr << "Reconstruction comparison needs exactly one camera in each reconstruction.\n";
+    return EXIT_FAILURE;
+  }
+  CameraModel& m1 = *s1.intrinsics[0];
+  CameraModel& m2 = *s2.intrinsics[0];
+  if (m1.width() != m2.width() || m1.height() != m2.height()) {
+    std::cerr << "The cameras differ in image size (" << m1.width() << " x " << m1.height() << " against "
+              << m2.width() << " x " << m2.height() << ").\n";
+    return EXIT_FAILURE;
+  }
+  auto camera = [](CameraModel& m) {
+    b200ba_camera c{};
+    c.model_type = static_cast<int32_t>(m.type());
+    c.width = m.width();
+    c.height = m.height();
+    c.calibration_min_x = m.calibration_min_x();
+    c.calibration_min_y = m.calibration_min_y();
+    c.calibration_max_x = m.calibration_max_x();
+    c.calibration_max_y = m.calibration_max_y();
+    int rx = 0, ry = 0;
+    if (m.GetGridResolution(&rx, &ry)) {
+      c.grid_width = rx;
+      c.grid_height = ry;
+    }
+    return c;
+  };
+  auto flat = [](const std::vector<SE3d>& poses) {
+    std::vector<double> v;
+    for (const SE3d& T : poses) v.insert(v.end(), {T.qw, T.qx, T.qy, T.qz, T.tx, T.ty, T.tz});
+    return v;
+  };
+  const b200ba_camera c1 = camera(m1), c2 = camera(m2);
+  const std::vector<double> rtg1 = flat(s1.rig_tr_global), ctr1 = flat({s1.camera_tr_rig.at(0)});
+  const std::vector<double> rtg2 = flat(s2.rig_tr_global), ctr2 = flat({s2.camera_tr_rig.at(0)});
+  b200ba_reconstruction_comparison r{};
+  const int rc = b200ba_compare_reconstructions(-1, &c1, m1.flat_intrinsics().data(), &c2, m2.flat_intrinsics().data(),
+                                                static_cast<int32_t>(s1.rig_tr_global.size()), rtg1.data(), ctr1.data(),
+                                                rtg2.data(), ctr2.data(), pixel_step, &r, nullptr);
+  if (rc != 0) {
+    std::cerr << "libb200ba error " << rc << ": " << b200ba_last_error(nullptr) << "\n";
+    return EXIT_FAILURE;
+  }
+  std::string out = "intrinsics1_r_intrinsics2_4x4:\n";
+  for (int row = 0; row < 4; ++row) {
+    for (int col = 0; col < 4; ++col) {
+      const double v = (row < 3 && col < 3) ? r.intrinsics1_r_intrinsics2[3 * row + col] : (row == col ? 1.0 : 0.0);
+      char buf[64];
+      std::snprintf(buf, sizeof(buf), col ? " %.6g" : "%.6g", v);
+      out += buf;
+    }
+    out += "\n";
+  }
+  char buf[96];
+  std::snprintf(buf, sizeof(buf), "relative endpoint difference: %.6g%%\n", 100 * r.relative_endpoint_difference);
+  out += buf;
+  std::cout << out;
+  std::cout.flush();
+  const MeshLabProjectPaths p = ReconstructionProjectPaths(reconstruction_path_1, reconstruction_path_2,
+                                                           std::filesystem::current_path().string());
+  std::vector<MeshLabMesh> meshes(4);
+  const char* labels[4] = {"SfM cloud 1: ", "SfM camera poses 1: ", "SfM cloud 2: ", "SfM camera poses 2: "};
+  for (int k = 0; k < 4; ++k) {
+    meshes[k].label = labels[k] + (k < 2 ? p.rest1 : p.rest2);
+    meshes[k].filename = p.files[k];
+    for (int e = 0; e < 16; ++e)
+      meshes[k].global_tr_mesh[e] = k < 2 ? (e == 15 ? 1.0 : (e % 5 == 0 ? r.scale : 0.0)) : r.firstimage1_tr_firstimage2[e];
+  }
+  if (!WriteMeshLabProject(p.project, meshes))
+    std::cerr << "Failed to save MeshLab project to: " << p.project << "\n";
   return EXIT_SUCCESS;
 }
 

@@ -247,6 +247,25 @@ def RenderVoronoi(width: int, height: int, sites_q, colors, device: int = -1):
     return img, ms.value
 
 
+def VisualizeCameraModel(width: int, height: int, params, device: int = -1, directions: bool = False):
+    """VisualizeCameraModel (APP/tools/visualize_calibration.cc:39-96) of a libvis RadtanCamera8d on the device
+    (``b200ba_visualize_camera``; the steps are specified in include/b200ba.h): params = k1 k2 r1 r2 fx fy cx cy.
+    Returns (image [height, width, 3] uint8, rotation [3, 3], directions, device_ms); with ``directions`` the
+    [height, width, 3] rotated unit directions behind the image, else None."""
+    lib = cabi.load_library()
+    p = np.ascontiguousarray(np.asarray(params, dtype=np.float64).reshape(-1))
+    if p.size != 8:
+        raise ValueError("VisualizeCameraModel: params must hold k1 k2 r1 r2 fx fy cx cy")
+    w, h = max(int(width), 0), max(int(height), 0)
+    img = np.zeros((h, w, 3), np.uint8)
+    rot = np.zeros((3, 3))
+    dirs = np.zeros((h, w, 3)) if directions else None
+    ms = C.c_double(0)
+    _check(lib.b200ba_visualize_camera(device, int(width), int(height), _dp(p), _u8p(img), _dp(rot),
+                                       None if dirs is None else _dp(dirs), C.byref(ms)))
+    return img, rot, dirs, ms.value
+
+
 def nccl_unique_id() -> bytes:
     lib = cabi.load_library()
     buf = (C.c_uint8 * cabi.NCCL_UNIQUE_ID_BYTES)()

@@ -466,6 +466,7 @@ SYMBOLS = {
                                        C.POINTER(C.c_uint8), C.POINTER(C.c_int64), _D]),
     "b200ba_render_voronoi": (C.c_int, [C.c_int, C.c_int32, C.c_int32, C.c_int64, _I32, C.POINTER(C.c_float),
                                         C.POINTER(C.c_uint8), _D]),
+    "b200ba_visualize_camera": (C.c_int, [C.c_int, C.c_int32, C.c_int32, _D, C.POINTER(C.c_uint8), _D, _D, _D]),
     "b200ba_snapshot_state": (C.c_int, [C.c_void_p]),
     "b200ba_restore_state": (C.c_int, [C.c_void_p]),
     "b200ba_version": (C.c_char_p, []),

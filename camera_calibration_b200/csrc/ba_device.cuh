@@ -543,4 +543,60 @@ __device__ __forceinline__ d3 rot_apply(const double R[9], d3 p) {
              R[6] * p.x + R[7] * p.y + R[8] * p.z);
 }
 
+// ---- libvis RadtanCamera8d (libvis/camera.h: RadtanDistortion4 :500-591, PixelMapping4 :1011-1121) ---------------
+// p = k1 k2 r1 r2 fx fy cx cy. UnprojectFromPixelCornerConv(x, y): n = (fx_inv x + cx_inv, fy_inv y + cy_inv) with
+// fx_inv = 1 / fx, cx_inv = -cx / fx; then at most 5 Gauss-Newton steps from u = n: e = n - D(u),
+// u += (J^T J)^-1 J^T e with Eigen's closed-form 2 x 2 inverse (1 / det times the adjugate) and the products taken left
+// to right, stopping after the step whose e has |e|^2 < DBL_EPSILON. Returns (u.x, u.y), the direction being (u, 1).
+// Every operation is rounded on its own (no fused multiply-add) in the reference's order, so that a restatement in
+// double reproduces every bit; where the iteration diverges the values are whatever IEEE arithmetic gives (NaN, inf).
+__device__ __forceinline__ void radtan8_unproject(const double* __restrict__ p, double x, double y, double& ux,
+                                                  double& uy) {
+  const double k1 = p[0], k2 = p[1], r1 = p[2], r2 = p[3];
+  const double nx = __dadd_rn(__dmul_rn(__ddiv_rn(1.0, p[4]), x), __ddiv_rn(-p[6], p[4]));
+  const double ny = __dadd_rn(__dmul_rn(__ddiv_rn(1.0, p[5]), y), __ddiv_rn(-p[7], p[5]));
+  const double k1_2 = __dmul_rn(k1, 2.0), k2_4 = __dmul_rn(k2, 4.0);
+  const double r1_2 = __dmul_rn(2.0, r1), r2_2 = __dmul_rn(2.0, r2), r1_6 = __dmul_rn(6.0, r1), r2_6 = __dmul_rn(6.0, r2);
+  ux = nx;
+  uy = ny;
+  for (int i = 0; i < 5; ++i) {
+    const double mx2 = __dmul_rn(ux, ux), my2 = __dmul_rn(uy, uy), mxy = __dmul_rn(ux, uy);
+    const double rho2 = __dadd_rn(mx2, my2);
+    const double k2rho2 = __dmul_rn(k2, rho2);
+    const double rad = __dadd_rn(__dmul_rn(k1, rho2), __dmul_rn(k2rho2, rho2));
+    const double one_rad = __dadd_rn(1.0, rad);
+    const double k2rho2_4 = __dmul_rn(k2rho2, 4.0);
+    const double j00 = __dadd_rn(__dadd_rn(__dadd_rn(__dadd_rn(one_rad, __dmul_rn(k1_2, mx2)), __dmul_rn(k2rho2_4, mx2)),
+                                           __dmul_rn(r1_2, uy)),
+                                 __dmul_rn(r2_6, ux));
+    const double j10 = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(k1_2, mxy), __dmul_rn(__dmul_rn(k2_4, rho2), mxy)),
+                                           __dmul_rn(r1_2, ux)),
+                                 __dmul_rn(r2_2, uy));
+    const double j11 = __dadd_rn(__dadd_rn(__dadd_rn(__dadd_rn(one_rad, __dmul_rn(k1_2, my2)), __dmul_rn(k2rho2_4, my2)),
+                                           __dmul_rn(r1_6, uy)),
+                                 __dmul_rn(r2_2, ux));
+    const double dx = __dadd_rn(__dadd_rn(__dadd_rn(ux, __dmul_rn(ux, rad)), __dmul_rn(r1_2, mxy)),
+                                __dmul_rn(r2, __dadd_rn(rho2, __dmul_rn(2.0, mx2))));
+    const double dy = __dadd_rn(__dadd_rn(__dadd_rn(uy, __dmul_rn(uy, rad)), __dmul_rn(r2_2, mxy)),
+                                __dmul_rn(r1, __dadd_rn(rho2, __dmul_rn(2.0, my2))));
+    const double ex = __dsub_rn(nx, dx), ey = __dsub_rn(ny, dy);
+    // A = J^T J (J symmetric: J(0,1) = J(1,0) = j10)
+    const double a00 = __dadd_rn(__dmul_rn(j00, j00), __dmul_rn(j10, j10));
+    const double a01 = __dadd_rn(__dmul_rn(j00, j10), __dmul_rn(j10, j11));
+    const double a10 = __dadd_rn(__dmul_rn(j10, j00), __dmul_rn(j11, j10));
+    const double a11 = __dadd_rn(__dmul_rn(j10, j10), __dmul_rn(j11, j11));
+    const double invdet = __ddiv_rn(1.0, __dsub_rn(__dmul_rn(a00, a11), __dmul_rn(a10, a01)));
+    const double i00 = __dmul_rn(a11, invdet), i10 = __dmul_rn(-a10, invdet);
+    const double i01 = __dmul_rn(-a01, invdet), i11 = __dmul_rn(a00, invdet);
+    // M = A^-1 J^T, then M e
+    const double m00 = __dadd_rn(__dmul_rn(i00, j00), __dmul_rn(i01, j10));
+    const double m01 = __dadd_rn(__dmul_rn(i00, j10), __dmul_rn(i01, j11));
+    const double m10 = __dadd_rn(__dmul_rn(i10, j00), __dmul_rn(i11, j10));
+    const double m11 = __dadd_rn(__dmul_rn(i10, j10), __dmul_rn(i11, j11));
+    ux = __dadd_rn(ux, __dadd_rn(__dmul_rn(m00, ex), __dmul_rn(m01, ey)));
+    uy = __dadd_rn(uy, __dadd_rn(__dmul_rn(m10, ex), __dmul_rn(m11, ey)));
+    if (__dadd_rn(__dmul_rn(ex, ex), __dmul_rn(ey, ey)) < 2.220446049250313080847e-16) break;
+  }
+}
+
 }  // namespace b200ba

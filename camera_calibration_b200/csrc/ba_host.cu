@@ -3239,6 +3239,56 @@ int b200ba_render_voronoi(int device, int32_t width, int32_t height, int64_t n_s
   return cs.rc;
 }
 
+// Stand-alone VisualizeCameraModel of a libvis RadtanCamera8d (APP/tools/visualize_calibration.cc:39-96): the
+// orientation and the image on the device. The argument checks come first and touch no CUDA state.
+int b200ba_visualize_camera(int device, int32_t width, int32_t height, const double* params, uint8_t* image,
+                            double* rotation, double* directions, double* device_ms) {
+  if (!params || !image) {
+    g_create_error = "b200ba_visualize_camera: params and image are required";
+    return 2;
+  }
+  if (width < 1 || height < 1 || width > (1 << 24) || height > (1 << 24) ||
+      static_cast<int64_t>(width) * height > (int64_t(1) << 31)) {
+    g_create_error = "b200ba_visualize_camera: width and height must be >= 1 and the image at most 2^31 pixels";
+    return 2;
+  }
+  for (int k = 0; k < 8; ++k)
+    if (!std::isfinite(params[k])) {
+      g_create_error = "b200ba_visualize_camera: a parameter is not finite";
+      return 2;
+    }
+  if (params[4] == 0 || params[5] == 0) {
+    g_create_error = "b200ba_visualize_camera: fx and fy must not be 0";
+    return 2;
+  }
+  CallScope cs(&g_create_error);
+  if (int rc = cs.use_device(device)) return rc;
+  const int64_t pixels = static_cast<int64_t>(width) * height;
+  double* d_params = nullptr;
+  double2* d_win = nullptr;
+  double* d_rot = nullptr;
+  uint8_t* d_img = nullptr;
+  double* d_dirs = nullptr;
+  cs.alloc(&d_params, 8);
+  cs.alloc(&d_win, static_cast<size_t>(21) * width);  // the orientation window: at most 21 rows of at most width pixels
+  cs.alloc(&d_rot, 9);
+  cs.alloc(&d_img, 3 * pixels);
+  if (directions) cs.alloc(&d_dirs, 3 * pixels);
+  if (cs.rc == 0) cs.ok(cudaMemcpy(d_params, params, sizeof(double) * 8, cudaMemcpyHostToDevice));
+  if (cs.rc == 0) {
+    cs.record(0, 0);
+    launch_visualize_orientation(d_params, width, height, d_win, d_rot, 0);
+    launch_visualize_camera(d_params, width, height, d_rot, d_img, d_dirs, 0);
+    cs.record(1, 0);
+    cs.ok(cudaGetLastError());
+    cs.ok(cudaMemcpy(image, d_img, 3 * pixels, cudaMemcpyDeviceToHost));
+    if (rotation) cs.ok(cudaMemcpy(rotation, d_rot, sizeof(double) * 9, cudaMemcpyDeviceToHost));
+    if (directions) cs.ok(cudaMemcpy(directions, d_dirs, sizeof(double) * 3 * pixels, cudaMemcpyDeviceToHost));
+  }
+  if (cs.rc == 0 && device_ms) *device_ms = cs.elapsed_ms(0, 1);
+  return cs.rc;
+}
+
 // Eigen::LDLT<MatrixXd, Lower>(A.selfadjointView<Upper>()).solve(b) for n = 3 (SolveDensely, LV/lm_optimizer.h:1022-1023):
 // symmetric pivoting on the largest remaining |diagonal| entry as Eigen's left-looking factorisation sees it (the
 // ORIGINAL values of the trailing diagonal), then x = P^T L^-T D^-1 L^-1 P b with 1 / d_i taken as 0 where

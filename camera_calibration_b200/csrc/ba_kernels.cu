@@ -3349,10 +3349,19 @@ void launch_report_sites(const ProblemDev& pb, const ReportDev& r, int64_t n_gro
                                                                                      group_obs, sites, colors);
 }
 
-// VisualizeModelDirections (:1165-1190) with CreateObservationDirectionsImage (util.cc:190-229): the direction of
-// (x + 0.5f, y + 0.5f) (the line direction for non-central models), black where the un-projection fails; the colour
+// The observation-direction colour of a direction d (util.cc:190-229, tools/visualize_calibration.cc:84-93):
 // ((70 * 255.99f) / 2.f) * (d + 1) (x, y) and ((270 * 255.99f) / 2.f) * (d + 1) (z) is a double that the reference
 // converts to u8 as x86-64 does: truncation to int32, then the low byte (hence the stripes).
+__device__ __forceinline__ void direction_colour(d3 d, uint8_t out[3]) {
+  const double kxy = static_cast<double>((70 * 255.99f) / 2.f), kz = static_cast<double>((270 * 255.99f) / 2.f);
+  out[0] = static_cast<uint8_t>(report_trunc(__dmul_rn(kxy, __dadd_rn(d.x, 1.0))));
+  out[1] = static_cast<uint8_t>(report_trunc(__dmul_rn(kxy, __dadd_rn(d.y, 1.0))));
+  out[2] = static_cast<uint8_t>(report_trunc(__dmul_rn(kz, __dadd_rn(d.z, 1.0))));
+}
+
+// VisualizeModelDirections (:1165-1190) with CreateObservationDirectionsImage (util.cc:190-229): the direction of
+// (x + 0.5f, y + 0.5f) (the line direction for non-central models) in direction_colour, black where the un-projection
+// fails.
 constexpr int kDirTileX = 16, kDirTileY = 8;
 __global__ void __launch_bounds__(kDirTileX * kDirTileY)
     observation_directions_kernel(CamDev c, const double* __restrict__ intr, uint8_t* __restrict__ img) {
@@ -3371,10 +3380,7 @@ __global__ void __launch_bounds__(kDirTileX * kDirTileY)
       noncentral_eval(c, intr, intr + 3 * static_cast<int64_t>(c.gw) * c.gh, px, py, e);
       d = e.u;
     }
-    const double kxy = static_cast<double>((70 * 255.99f) / 2.f), kz = static_cast<double>((270 * 255.99f) / 2.f);
-    out[0] = static_cast<uint8_t>(report_trunc(__dmul_rn(kxy, __dadd_rn(d.x, 1.0))));
-    out[1] = static_cast<uint8_t>(report_trunc(__dmul_rn(kxy, __dadd_rn(d.y, 1.0))));
-    out[2] = static_cast<uint8_t>(report_trunc(__dmul_rn(kz, __dadd_rn(d.z, 1.0))));
+    direction_colour(d, out);
   }
   const int64_t p = 3 * (static_cast<int64_t>(y) * c.width + x);
   img[p] = out[0];
@@ -3384,6 +3390,139 @@ __global__ void __launch_bounds__(kDirTileX * kDirTileY)
 void launch_observation_directions(const CamDev& c, const double* intr, uint8_t* img, cudaStream_t s) {
   const dim3 grid((c.width + kDirTileX - 1) / kDirTileX, (c.height + kDirTileY - 1) / kDirTileY);
   observation_directions_kernel<<<grid, dim3(kDirTileX, kDirTileY), 0, s>>>(c, intr, img);
+}
+
+// ---- VisualizeCameraModel (APP/tools/visualize_calibration.cc:39-96) for a libvis RadtanCamera8d -----------------------
+// The orientation needs the mean un-normalised direction of the window x in [x0, w - 1], y in [y0, y1] to the right of
+// the image centre, summed in row-major order as the reference sums it, so that the rotation does not depend on the launch
+// shape: radtan8_window_kernel un-projects the window's pixels in parallel, radtan8_orientation_kernel adds them up on
+// one thread (three independent accumulators) and forms the rotation, visualize_camera_kernel draws every pixel.
+__global__ void radtan8_window_kernel(const double* __restrict__ params, int x0, int nx, int y0, int64_t n,
+                                      double2* __restrict__ win) {
+  const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (i >= n) return;
+  const int x = x0 + static_cast<int>(i % nx), y = y0 + static_cast<int>(i / nx);
+  double ux, uy;
+  radtan8_unproject(params, static_cast<double>(x + 0.5f), static_cast<double>(y + 0.5f), ux, uy);
+  win[i] = make_double2(ux, uy);
+}
+
+// The rotation of VisualizeCameraModel (:48-82) from forward = Unproject(0.5f w, 0.5f h) and the window's directions,
+// summed on one thread in row-major order (the z components, all 1, summed like the others), every operation but
+// atan2 / sin / cos rounded on its own in Eigen's order: tiny images make the angle atan2 of two small numbers formed by
+// cancellation, where any other order of the same operations moves the rotation by far more than an ulp. The block
+// stages the directions through shared memory so that the summing thread waits on shared-memory rather than L2 latency.
+constexpr int kWinThreads = 256, kWinChunk = 2048;
+__global__ void __launch_bounds__(kWinThreads)
+    radtan8_orientation_kernel(const double* __restrict__ params, int w, int h, int64_t n,
+                               const double2* __restrict__ win, double* __restrict__ rot) {
+  __shared__ double2 chunk[kWinChunk];
+  double sx = 0, sy = 0, sz = 0;
+  for (int64_t base = 0; base < n; base += kWinChunk) {
+    const int m = static_cast<int>(min(static_cast<int64_t>(kWinChunk), n - base));
+    __syncthreads();
+    for (int i = threadIdx.x; i < m; i += kWinThreads) chunk[i] = win[base + i];
+    __syncthreads();
+    if (threadIdx.x == 0) {
+#pragma unroll 8
+      for (int i = 0; i < m; ++i) {
+        const double2 d = chunk[i];
+        sx = __dadd_rn(sx, d.x);
+        sy = __dadd_rn(sy, d.y);
+        sz = __dadd_rn(sz, 1.0);
+      }
+    }
+  }
+  if (threadIdx.x != 0) return;
+  double fx, fy;
+  radtan8_unproject(params, static_cast<double>(0.5f * static_cast<float>(w)),
+                    static_cast<double>(0.5f * static_cast<float>(h)), fx, fy);
+  // Quaterniond::FromTwoVectors(forward, e_z).toRotationMatrix() in Eigen's order: forward.normalized(); c = e_z . v0;
+  // axis = v0 x e_z; s = sqrt((1 + c) * 2); q = (s * 0.5, axis * (1 / s)). Eigen's branch for c < -1 + 1e-12 cannot
+  // be taken: the forward direction (u, 1) has c = 1 / |(u, 1)| > 0, or NaN.
+  const double sq = __dadd_rn(__dadd_rn(__dmul_rn(fx, fx), __dmul_rn(fy, fy)), 1.0);
+  double v0[3] = {fx, fy, 1.0};
+  if (sq > 0) {
+    const double n = sqrt(sq);
+    for (int k = 0; k < 3; ++k) v0[k] = __ddiv_rn(v0[k], n);
+  }
+  const double c = __dadd_rn(__dadd_rn(__dmul_rn(0.0, v0[0]), __dmul_rn(0.0, v0[1])), __dmul_rn(1.0, v0[2]));
+  const double axis[3] = {__dsub_rn(__dmul_rn(v0[1], 1.0), __dmul_rn(v0[2], 0.0)),
+                          __dsub_rn(__dmul_rn(v0[2], 0.0), __dmul_rn(v0[0], 1.0)),
+                          __dsub_rn(__dmul_rn(v0[0], 0.0), __dmul_rn(v0[1], 0.0))};
+  const double s = sqrt(__dmul_rn(__dadd_rn(1.0, c), 2.0)), invs = __ddiv_rn(1.0, s);
+  const double qw = __dmul_rn(s, 0.5), qx = __dmul_rn(axis[0], invs), qy = __dmul_rn(axis[1], invs),
+               qz = __dmul_rn(axis[2], invs);
+  const double tx = __dmul_rn(2.0, qx), ty = __dmul_rn(2.0, qy), tz = __dmul_rn(2.0, qz);
+  const double twx = __dmul_rn(tx, qw), twy = __dmul_rn(ty, qw), twz = __dmul_rn(tz, qw);
+  const double txx = __dmul_rn(tx, qx), txy = __dmul_rn(ty, qx), txz = __dmul_rn(tz, qx);
+  const double tyy = __dmul_rn(ty, qy), tyz = __dmul_rn(tz, qy), tzz = __dmul_rn(tz, qz);
+  const double F[9] = {__dsub_rn(1.0, __dadd_rn(tyy, tzz)), __dsub_rn(txy, twz), __dadd_rn(txz, twy),
+                       __dadd_rn(txy, twz), __dsub_rn(1.0, __dadd_rn(txx, tzz)), __dsub_rn(tyz, twx),
+                       __dsub_rn(txz, twy), __dadd_rn(tyz, twx), __dsub_rn(1.0, __dadd_rn(txx, tyy))};
+  // right_sum / right_count, rotated by F; angle = atan2(-y, x); AngleAxisd(angle, e_z).toRotationMatrix() in Eigen's
+  // order; rotation = right_rotation * forward_rotation, each entry's products added left to right
+  const double count = static_cast<double>(n);
+  const double m[3] = {__ddiv_rn(sx, count), __ddiv_rn(sy, count), __ddiv_rn(sz, count)};
+  double r[3];
+  for (int i = 0; i < 3; ++i)
+    r[i] = __dadd_rn(__dadd_rn(__dmul_rn(F[3 * i], m[0]), __dmul_rn(F[3 * i + 1], m[1])), __dmul_rn(F[3 * i + 2], m[2]));
+  const double angle = atan2(-r[1], r[0]);
+  const double ca = cos(angle), sa = sin(angle);
+  const double Rz[9] = {ca, -sa, 0.0, sa, ca, 0.0, 0.0, 0.0, __dadd_rn(__dsub_rn(1.0, ca), ca)};
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j)
+      rot[3 * i + j] = __dadd_rn(__dadd_rn(__dmul_rn(Rz[3 * i], F[j]), __dmul_rn(Rz[3 * i + 1], F[3 + j])),
+                                 __dmul_rn(Rz[3 * i + 2], F[6 + j]));
+}
+
+// Every pixel: d = Unproject(x + 0.5f, y + 0.5f), normalized() (d / sqrt(|d|^2), a zero vector unchanged), rotated
+// (row-major R, the products of each row added left to right) and coloured with direction_colour. dirs (nullable):
+// the rotated unit directions [h * w * 3].
+__global__ void __launch_bounds__(kDirTileX * kDirTileY)
+    visualize_camera_kernel(const double* __restrict__ params, int w, int h, const double* __restrict__ rot,
+                            uint8_t* __restrict__ img, double* __restrict__ dirs) {
+  const int x = blockIdx.x * kDirTileX + threadIdx.x, y = blockIdx.y * kDirTileY + threadIdx.y;
+  if (x >= w || y >= h) return;
+  double ux, uy;
+  radtan8_unproject(params, static_cast<double>(x + 0.5f), static_cast<double>(y + 0.5f), ux, uy);
+  double vx = ux, vy = uy, vz = 1.0;
+  const double sq = __dadd_rn(__dadd_rn(__dmul_rn(ux, ux), __dmul_rn(uy, uy)), 1.0);
+  if (sq > 0) {
+    const double n = sqrt(sq);
+    vx = __ddiv_rn(vx, n);
+    vy = __ddiv_rn(vy, n);
+    vz = __ddiv_rn(vz, n);
+  }
+  double r[3];
+#pragma unroll
+  for (int i = 0; i < 3; ++i)
+    r[i] = __dadd_rn(__dadd_rn(__dmul_rn(__ldg(rot + 3 * i), vx), __dmul_rn(__ldg(rot + 3 * i + 1), vy)),
+                     __dmul_rn(__ldg(rot + 3 * i + 2), vz));
+  uint8_t out[3];
+  direction_colour(mk3(r[0], r[1], r[2]), out);
+  const int64_t p = 3 * (static_cast<int64_t>(y) * w + x);
+  img[p] = out[0];
+  img[p + 1] = out[1];
+  img[p + 2] = out[2];
+  if (dirs) {
+    dirs[p] = r[0];
+    dirs[p + 1] = r[1];
+    dirs[p + 2] = r[2];
+  }
+}
+
+void launch_visualize_orientation(const double* params, int w, int h, double2* win, double* rot, cudaStream_t s) {
+  const int x0 = std::min(w - 1, w / 2 + 11), y0 = std::max(0, h / 2 - 10), y1 = std::min(h - 1, h / 2 + 10);
+  const int nx = w - x0;
+  const int64_t n = static_cast<int64_t>(nx) * (y1 - y0 + 1);
+  radtan8_window_kernel<<<static_cast<unsigned>((n + 127) / 128), 128, 0, s>>>(params, x0, nx, y0, n, win);
+  radtan8_orientation_kernel<<<1, kWinThreads, 0, s>>>(params, w, h, n, win, rot);
+}
+void launch_visualize_camera(const double* params, int w, int h, const double* rot, uint8_t* img, double* dirs,
+                             cudaStream_t s) {
+  const dim3 grid((w + kDirTileX - 1) / kDirTileX, (h + kDirTileY - 1) / kDirTileY);
+  visualize_camera_kernel<<<grid, dim3(kDirTileX, kDirTileY), 0, s>>>(params, w, h, rot, img, dirs);
 }
 
 // Generic small-block Schur preparation for b200ba_schur_solve (block size <= 6, arbitrary

@@ -98,6 +98,12 @@ void launch_report_sites(const ProblemDev& pb, const ReportDev& r, int64_t n_gro
                          const uint32_t* group_obs, int2* sites, float* colors, cudaStream_t s);
 // observation-direction image of one camera (VisualizeModelDirections): central- or non-central-generic
 void launch_observation_directions(const CamDev& c, const double* intr, uint8_t* img, cudaStream_t s);
+// VisualizeCameraModel of a libvis RadtanCamera8d (params [8] k1 k2 r1 r2 fx fy cx cy, on the device): the orientation
+// rot [9] (window directions win: at most 21 * w), then the image [h * w * 3] and, dirs non-null, the rotated unit
+// directions [h * w * 3]
+void launch_visualize_orientation(const double* params, int w, int h, double2* win, double* rot, cudaStream_t s);
+void launch_visualize_camera(const double* params, int w, int h, const double* rot, uint8_t* img, double* dirs,
+                             cudaStream_t s);
 void launch_generic_block_inverse(int bs, int nb, int nd, const double* D, const double* B, const double* b1,
                                   double* DinvB, double* Dinvb, cudaStream_t s);
 void launch_symmetrize(int n, double* M, cudaStream_t s);

@@ -19,6 +19,7 @@ Formats follow applications/camera_calibration/src/camera_calibration/io/calibra
 from __future__ import annotations
 
 import os
+import re
 import struct
 from typing import Dict, List, Optional, Tuple
 
@@ -682,3 +683,150 @@ def MeshLabProjectPaths(reconstruction_path_1, reconstruction_path_2, cwd=None):
         absolute = p if p.startswith(b"/") else _path_join(cwd, p)
         files += [_path_join(absolute, b"points.yaml.obj"), _path_join(absolute, b"rig_tr_global.yaml.obj")]
     return prefix + b"reconstructions_aligned_at_start.mlp", rest1, rest2, files
+
+
+# ---------------------------------------------------------------------------------------
+# calibration visualisation (the --visualize_kalibr_calibration, --visualize_colmap_calibration and
+# --create_legends tools)
+# ---------------------------------------------------------------------------------------
+# Numbers are converted from their text as strtod / strtol read a whole token (decimal only, no hex, no '_'),
+# so that the C++ readers (b200ba_io.hpp) accept exactly the same texts.
+_DECIMAL = re.compile(r"[+-]?((\d+\.?\d*|\.\d+)([eE][+-]?\d+)?|[iI][nN][fF]([iI][nN][iI][tT][yY])?|[nN][aA][nN])",
+                      re.ASCII)
+_INTEGER = re.compile(r"[+-]?\d+", re.ASCII)
+_COLMAP_TOKEN = re.compile(r"[^ \t\v\f\r]+")
+KALIBR_CAMERA_FIELDS = ("camera_model", "distortion_model", "resolution", "distortion_coeffs", "intrinsics")
+
+
+def ParseDecimal(text: str) -> Optional[float]:
+    """The double that strtod reads from the whole of ``text``; None if it is not a decimal number, inf or nan."""
+    return float(text) if _DECIMAL.fullmatch(text) else None
+
+
+def ParseInt32(text: str) -> Optional[int]:
+    """The int that strtol reads from the whole of ``text``; None if it is not a decimal int32."""
+    if not _INTEGER.fullmatch(text):
+        return None
+    v = int(text)
+    return v if -2 ** 31 <= v < 2 ** 31 else None
+
+
+def ReadKalibrCamchain(camchain_path: str):
+    """The cameras of a Kalibr camchain YAML file as VisualizeKalibrCalibration reads them
+    (APP/tools/visualize_calibration.cc:98-165): ``cam0``, ``cam1``, ... up to the first missing key. Returns a list of
+    dicts with ``name`` and the texts of ``camera_model`` and ``distortion_model`` ("" when absent or not a scalar) and
+    of ``resolution``, ``distortion_coeffs`` and ``intrinsics`` (lists of strings; None when absent or not a flat list).
+    Other keys (``T_cn_cnm1``, ``cam_overlaps``, ``rostopic``, ...) are skipped. Returns None if the file cannot be read
+    or is not a YAML map. The YAML structure is parsed with every scalar kept as text (numbers are converted later by
+    ``KalibrRadtanParameters``: YAML 1.1 would read ``1e-5`` as a string)."""
+    try:
+        with open(camchain_path, encoding="utf-8") as f:
+            doc = yaml.load(f, Loader=yaml.BaseLoader)
+    except (OSError, UnicodeDecodeError, yaml.YAMLError):
+        return None
+    if not isinstance(doc, dict):
+        return None
+    cameras = []
+    while f"cam{len(cameras)}" in doc:
+        name = f"cam{len(cameras)}"
+        node = doc[name] if isinstance(doc[name], dict) else {}
+        cam = {"name": name}
+        for key in KALIBR_CAMERA_FIELDS[:2]:
+            cam[key] = node[key] if isinstance(node.get(key), str) else ""
+        for key in KALIBR_CAMERA_FIELDS[2:]:
+            v = node.get(key)
+            cam[key] = list(v) if isinstance(v, list) and all(isinstance(e, str) for e in v) else None
+        cameras.append(cam)
+    return cameras
+
+
+def KalibrRadtanParameters(camera) -> Optional[Tuple[int, int, List[float]]]:
+    """(width, height, [k1 k2 r1 r2 fx fy cx cy]) of a pinhole-radtan camera of ReadKalibrCamchain: the
+    ``distortion_coeffs`` followed by the ``intrinsics`` (fu fv pu pv), as the reference concatenates them. None unless
+    the resolution holds 2 ints and there are exactly 4 distortion coefficients and 4 intrinsics, all numbers (the
+    reference reads out of bounds with fewer)."""
+    res, dist, intr = camera["resolution"], camera["distortion_coeffs"], camera["intrinsics"]
+    if res is None or dist is None or intr is None or len(res) != 2 or len(dist) != 4 or len(intr) != 4:
+        return None
+    size = [ParseInt32(t) for t in res]
+    params = [ParseDecimal(t) for t in dist + intr]
+    if None in size or None in params:
+        return None
+    return size[0], size[1], params
+
+
+def ReadColmapCameras(cameras_txt_path: str):
+    """libvis/src/libvis/external_io/colmap_model.cc:47-72: one camera per line, ``CAMERA_ID MODEL WIDTH HEIGHT
+    PARAMS[]``; lines that are empty or start with '#' are skipped. Returns a list of dicts (``camera_id``,
+    ``model_name``, ``width``, ``height``, ``parameters``) in file order, keeping the first camera of an id that appears
+    twice (the reference's unordered_map::insert), or None if the file cannot be read. The parameters are what
+    libstdc++'s ``while (!eof) { push_back(0); stream >> back(); }`` reads: a line that ends in whitespace (a blank,
+    a tab, a carriage return) gets one more parameter, 0. Where the reference never ends (a token that is not a number)
+    the parameters stop before that token; a line whose first four fields are not an int, a name and two ints is
+    skipped."""
+    try:
+        with open(cameras_txt_path, encoding="utf-8", errors="surrogateescape", newline="") as f:
+            lines = f.read().split("\n")
+    except OSError:
+        return None
+    cameras, seen = [], set()
+    for line in lines:
+        if len(line) == 0 or line[0] == "#":
+            continue
+        tokens = _COLMAP_TOKEN.findall(line)
+        if len(tokens) < 4:
+            continue
+        camera_id, width, height = ParseInt32(tokens[0]), ParseInt32(tokens[2]), ParseInt32(tokens[3])
+        if camera_id is None or width is None or height is None:
+            continue
+        parameters = []
+        for t in tokens[4:]:
+            v = ParseDecimal(t)
+            if v is None:
+                break
+            parameters.append(v)
+        else:
+            if line[-1] in " \t\v\f\r":
+                parameters.append(0.0)
+        if camera_id in seen:
+            continue
+        seen.add(camera_id)
+        cameras.append(dict(camera_id=camera_id, model_name=tokens[1], width=width, height=height,
+                            parameters=parameters))
+    return cameras
+
+
+def ColmapRadtanParameters(camera) -> Optional[List[float]]:
+    """[k1 k2 r1 r2 fx fy cx cy] of an OPENCV camera of ReadColmapCameras (COLMAP's fx fy cx cy k1 k2 p1 p2 with the
+    halves swapped, visualize_calibration.cc:181-198); None with fewer than 8 parameters."""
+    p = camera["parameters"]
+    return None if len(p) < 8 else list(p[4:8]) + list(p[0:4])
+
+
+_LIBM = None
+
+
+def _atan2f(y: float, x: float) -> float:
+    """(double)atan2f(y, x) of the C library, as the C++ legend computes it."""
+    global _LIBM
+    if _LIBM is None:
+        import ctypes
+        import ctypes.util
+        _LIBM = ctypes.CDLL(ctypes.util.find_library("m"))
+        _LIBM.atan2f.restype = ctypes.c_float
+        _LIBM.atan2f.argtypes = [ctypes.c_float, ctypes.c_float]
+    return float(_LIBM.atan2f(y, x))
+
+
+def LegendErrorDirectionsImage() -> np.ndarray:
+    """``legend_error_directions.png`` of CreateLegends (APP/tools/create_legends.cc:35-54): 200 x 200 pixels, the offset
+    e = (x + 0.5f, y + 0.5f) - (100, 100) in float, dir = (double)atan2f(e.y, e.x), colour (127 + 127 sin(dir) + 0.5,
+    127 + 127 cos(dir) + 0.5, 127) in double, truncated. 40 000 pixels: computed on the host, as the C++ LegendErrorDirections
+    (b200ba_io.hpp) does, with the same C library."""
+    import math
+    image = np.empty((200, 200, 3), np.uint8)
+    for y in range(200):
+        for x in range(200):
+            d = _atan2f(y + 0.5 - 100.0, x + 0.5 - 100.0)
+            image[y, x] = (int(127 + 127 * math.sin(d) + 0.5), int(127 + 127 * math.cos(d) + 0.5), 127)
+    return image

@@ -312,6 +312,36 @@ B200BA_API int b200ba_unproject(int device, const b200ba_camera* cam, const doub
 B200BA_API int b200ba_render_voronoi(int device, int32_t width, int32_t height, int64_t n_sites, const int32_t* sites_q,
                                      const float* colors, uint8_t* image, double* device_ms);
 
+/* ---- calibration visualisation: VisualizeCameraModel (APP/tools/visualize_calibration.cc:39-96, the
+ * --visualize_kalibr_calibration / --visualize_colmap_calibration tools) for a libvis RadtanCamera8d,
+ * params = k1 k2 r1 r2 fx fy cx cy (libvis/camera.h: RadtanDistortion4 :500-591, PixelMapping4 :1011-1121).
+ *   Unproject(x, y): n = (fx_inv x + cx_inv, fy_inv y + cy_inv), fx_inv = 1 / fx, cx_inv = -cx / fx (pixel-corner
+ *     convention); then at most 5 Gauss-Newton steps from u = n: e = n - D(u), u += (J^T J)^-1 J^T e, Eigen's closed-form
+ *     2 x 2 inverse (1 / det times the adjugate) and the products taken left to right; the iteration stops after the
+ *     step whose e has |e|^2 < DBL_EPSILON. The direction is (u.x, u.y, 1). Where 5 steps do not converge it is the
+ *     fifth iterate; where the iteration diverges it holds whatever IEEE arithmetic gives (NaN, inf).
+ *   Orientation: F = FromTwoVectors(Unproject(0.5f w, 0.5f h), e_z); the directions of the window x in
+ *     [min(w - 1, w/2 + 11), w - 1], y in [max(0, h/2 - 10), min(h - 1, h/2 + 10)] at (x + 0.5f, y + 0.5f), not
+ *     normalised, are summed in row-major order (independent of the launch shape) and divided by their count, giving
+ *     m; angle = atan2(-(F m).y, (F m).x); rotation = AngleAxisd(angle, e_z) F. Every operation but atan2, sin and cos
+ *     is rounded on its own in Eigen's order (FromTwoVectors, toRotationMatrix, the products), because for tiny images
+ *     the angle is atan2 of two small numbers formed by cancellation.
+ *   Every pixel: d = rotation * Unproject(x + 0.5f, y + 0.5f).normalized() (division by sqrt of the squared norm; a
+ *     zero or NaN vector is left as it is), coloured ((70 * 255.99f) / 2.f) * (d + 1) (x, y) and
+ *     ((270 * 255.99f) / 2.f) * (d + 1) (z) in double and converted to u8 as b200ba_report_images' observation
+ *     directions are: truncation to int32 with INT_MIN for NaN and out-of-range values, then the low byte (so a NaN
+ *     direction is black). A forward direction or window sum that is not finite makes every pixel NaN, as in the
+ *     reference.
+ * Every value-path operation is rounded on its own (no fused multiply-add) in the reference's order, so that a
+ * restatement in double reproduces each direction bit for bit given the rotation.
+ * image [h*w*3] RGB row-major. rotation (nullable): [9] row-major. directions (nullable): [h*w*3] the rotated unit
+ * directions. device_ms (nullable): device time. Stand-alone (allocates, computes, frees); returns 2 before any CUDA
+ * call for a NULL params or image, width or height < 1 or > 2^24 or more than 2^31 pixels, a parameter that is not
+ * finite, or fx == 0 or fy == 0 (the reference divides by zero there); 3 without a device. Repeated calls give
+ * identical bytes. */
+B200BA_API int b200ba_visualize_camera(int device, int32_t width, int32_t height, const double* params, uint8_t* image,
+                                       double* rotation, double* directions, double* device_ms);
+
 /* ---- model resampling (row f-4): CentralGenericModel::FitToPixelDirectionsImpl --------
  * (APP/models/central_generic.cc:551-568 with the cost function of :152-228 and the state of
  * :40-83). Levenberg-Marquardt over the direction grid -- 2 local DoF per control point in its

@@ -23,7 +23,9 @@
 #pragma once
 
 #include <algorithm>
+#include <cctype>
 #include <cerrno>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -861,6 +863,310 @@ inline std::string EncodeMeshLabProject(const std::vector<MeshLabMesh>& meshes) 
 }
 inline bool WriteMeshLabProject(const std::string& path, const std::vector<MeshLabMesh>& meshes) {
   return io_detail::write_file(path, EncodeMeshLabProject(meshes));
+}
+
+// ---- calibration visualisation inputs (the --visualize_kalibr_calibration / --visualize_colmap_calibration tools) ----
+// Numbers are read from whole tokens as strtod / strtol read them, restricted to decimal texts (no hex, no '_'): io.py's
+// ParseDecimal / ParseInt32 accept exactly the same texts.
+namespace io_detail {
+inline bool is_decimal_text(const std::string& t) {
+  size_t i = 0;
+  const size_t n = t.size();
+  if (i < n && (t[i] == '+' || t[i] == '-')) ++i;
+  std::string rest = t.substr(i);
+  for (char& ch : rest) ch = static_cast<char>(std::tolower(static_cast<unsigned char>(ch)));
+  if (rest == "inf" || rest == "infinity" || rest == "nan") return true;
+  auto digit = [&](size_t k) { return k < n && t[k] >= '0' && t[k] <= '9'; };
+  size_t digits = 0;
+  while (digit(i)) ++i, ++digits;
+  if (i < n && t[i] == '.') {
+    ++i;
+    while (digit(i)) ++i, ++digits;
+  }
+  if (digits == 0) return false;
+  if (i < n && (t[i] == 'e' || t[i] == 'E')) {
+    ++i;
+    if (i < n && (t[i] == '+' || t[i] == '-')) ++i;
+    size_t exponent_digits = 0;
+    while (digit(i)) ++i, ++exponent_digits;
+    if (exponent_digits == 0) return false;
+  }
+  return i == n;
+}
+}  // namespace io_detail
+inline bool ParseDecimal(const std::string& text, double* v) {
+  if (!io_detail::is_decimal_text(text)) return false;
+  *v = std::strtod(text.c_str(), nullptr);
+  return true;
+}
+inline bool ParseInt32(const std::string& text, int* v) {
+  size_t i = (!text.empty() && (text[0] == '+' || text[0] == '-')) ? 1 : 0;
+  if (i == text.size()) return false;
+  for (size_t k = i; k < text.size(); ++k)
+    if (text[k] < '0' || text[k] > '9') return false;
+  errno = 0;
+  const long long x = std::strtoll(text.c_str(), nullptr, 10);
+  if (errno != 0 || x < -2147483648LL || x > 2147483647LL) return false;
+  *v = static_cast<int>(x);
+  return true;
+}
+
+// One camera of a Kalibr camchain: the texts of its fields (io.py's ReadKalibrCamchain returns the same). A model that is
+// absent or not a scalar reads as ""; has_* is false for a number list that is absent or not a flat list.
+struct KalibrCamera {
+  std::string name, camera_model, distortion_model;
+  bool has_resolution = false, has_distortion_coeffs = false, has_intrinsics = false;
+  std::vector<std::string> resolution, distortion_coeffs, intrinsics;
+};
+namespace io_detail {
+// a YAML value of the subset of Kalibr's camchain files: a scalar, a flat list of scalars (flow or block), or anything
+// else (nested lists such as T_cn_cnm1, nested maps), which is skipped
+struct KalibrValue {
+  enum Kind { kScalar, kList, kOther } kind = kOther;
+  std::string scalar;
+  std::vector<std::string> items;
+};
+inline std::string unquote(const std::string& s) {
+  if (s.size() >= 2 && (s[0] == '"' || s[0] == '\'') && s.back() == s[0]) return s.substr(1, s.size() - 2);
+  return s;
+}
+inline size_t indent_of(const std::string& line) {
+  size_t k = 0;
+  while (k < line.size() && line[k] == ' ') ++k;
+  return k;
+}
+// value text behind "key:"; a flow list may continue on the following lines (*i is advanced past them)
+inline bool kalibr_value(const std::string& value, const std::vector<std::string>& lines, size_t* i, KalibrValue* out) {
+  if (value.empty() || value[0] != '[') {
+    out->kind = KalibrValue::kScalar;
+    out->scalar = unquote(value);
+    return true;
+  }
+  std::string body = value.substr(1);
+  while (body.find(']') == std::string::npos) {
+    if (*i >= lines.size()) return false;
+    body += " " + lines[(*i)++];
+  }
+  if (!trim(body.substr(body.find(']') + 1)).empty()) return false;
+  body.resize(body.find(']'));
+  out->kind = KalibrValue::kList;
+  if (body.find('[') != std::string::npos) out->kind = KalibrValue::kOther;
+  const std::string t = trim(body);
+  for (size_t a = 0; !t.empty() && a <= t.size();) {
+    size_t b = t.find(',', a);
+    if (b == std::string::npos) b = t.size();
+    out->items.push_back(unquote(trim(t.substr(a, b - a))));
+    a = b + 1;
+  }
+  return true;
+}
+}  // namespace io_detail
+
+// The cameras of a Kalibr camchain YAML file as VisualizeKalibrCalibration reads them (APP/tools/visualize_calibration.cc
+// :98-165): cam0, cam1, ... up to the first missing key, every field kept as text. The reference parses the file with
+// yaml-cpp; the reader below understands what Kalibr writes: top-level `camN:` maps whose entries are `key: scalar`,
+// `key: [flow, list]` (possibly spanning lines) or `key:` followed by a block list (`- 752`, or `- [...]` rows as in
+// T_cn_cnm1, which are skipped), and `#` comments. Returns false if the file cannot be read or is not such a map.
+inline bool ReadKalibrCamchain(const std::string& camchain_path, std::vector<KalibrCamera>* cameras) {
+  using namespace io_detail;
+  std::string text;
+  if (!read_file(camchain_path, &text)) return false;
+  std::vector<std::string> lines;
+  for (std::string l : split_lines(text)) {
+    for (size_t k = 0; k < l.size(); ++k)
+      if (l[k] == '#' && (k == 0 || l[k - 1] == ' ' || l[k - 1] == '\t')) {
+        l.resize(k);
+        break;
+      }
+    while (!l.empty() && (l.back() == ' ' || l.back() == '\t' || l.back() == '\r')) l.pop_back();
+    lines.push_back(l);
+  }
+  std::map<std::string, std::map<std::string, KalibrValue>> doc;
+  size_t i = 0;
+  while (i < lines.size()) {
+    if (lines[i].empty()) { ++i; continue; }
+    if (indent_of(lines[i]) != 0 || lines[i][0] == '-' || lines[i].find('\t') == 0) return false;
+    std::string key, value;
+    if (!split_key(lines[i++], &key, &value)) return false;
+    std::map<std::string, KalibrValue>& node = doc[key];
+    node.clear();
+    if (!value.empty()) {  // a top-level scalar or list: not a camera map
+      KalibrValue ignored;
+      if (!kalibr_value(value, lines, &i, &ignored)) return false;
+      continue;
+    }
+    size_t map_indent = 0;
+    while (i < lines.size()) {
+      const std::string& line = lines[i];
+      if (line.empty()) { ++i; continue; }
+      const size_t ind = indent_of(line);
+      if (ind == 0 && line[0] != '-') break;  // the next top-level key
+      if (map_indent == 0) {
+        if (line[ind] == '-') {  // a top-level key holding a list: not a camera map
+          while (i < lines.size() && (lines[i].empty() || indent_of(lines[i]) > 0 || lines[i][0] == '-')) ++i;
+          break;
+        }
+        map_indent = ind;
+      }
+      if (ind != map_indent || line[ind] == '-') return false;
+      std::string k, v;
+      if (!split_key(line.substr(ind), &k, &v)) return false;
+      ++i;
+      KalibrValue& field = node[k];
+      field = KalibrValue();
+      if (!v.empty()) {
+        if (!kalibr_value(v, lines, &i, &field)) return false;
+        continue;
+      }
+      // a block below the key: list items at the key's indentation or deeper, or a nested map
+      field.kind = KalibrValue::kList;
+      while (i < lines.size()) {
+        const std::string& item = lines[i];
+        if (item.empty()) { ++i; continue; }
+        const size_t item_ind = indent_of(item);
+        if (item_ind < map_indent || (item_ind == map_indent && item[item_ind] != '-')) break;
+        ++i;
+        const std::string t = trim(item.substr(item_ind));
+        if (t[0] != '-') {
+          field.kind = KalibrValue::kOther;
+          continue;
+        }
+        const std::string entry = trim(t.substr(1));
+        std::string ek, ev;
+        if (entry.empty() || entry[0] == '[' || entry[0] == '-' || split_key(entry, &ek, &ev)) {
+          field.kind = KalibrValue::kOther;
+          if (!entry.empty() && entry[0] == '[') {
+            KalibrValue row;
+            if (!kalibr_value(entry, lines, &i, &row)) return false;
+          }
+          continue;
+        }
+        field.items.push_back(unquote(entry));
+      }
+      if (field.kind != KalibrValue::kList) field.items.clear();
+    }
+  }
+  if (doc.empty()) return false;  // no map at all
+  cameras->clear();
+  for (int c = 0;; ++c) {
+    const std::string name = "cam" + std::to_string(c);
+    auto it = doc.find(name);
+    if (it == doc.end()) break;
+    KalibrCamera cam;
+    cam.name = name;
+    const std::map<std::string, KalibrValue>& node = it->second;
+    auto scalar = [&](const char* key) {
+      auto f = node.find(key);
+      return (f != node.end() && f->second.kind == KalibrValue::kScalar) ? f->second.scalar : std::string();
+    };
+    auto list = [&](const char* key, std::vector<std::string>* out) {
+      auto f = node.find(key);
+      if (f == node.end() || f->second.kind != KalibrValue::kList) return false;
+      *out = f->second.items;
+      return true;
+    };
+    cam.camera_model = scalar("camera_model");
+    cam.distortion_model = scalar("distortion_model");
+    cam.has_resolution = list("resolution", &cam.resolution);
+    cam.has_distortion_coeffs = list("distortion_coeffs", &cam.distortion_coeffs);
+    cam.has_intrinsics = list("intrinsics", &cam.intrinsics);
+    cameras->push_back(cam);
+  }
+  return true;
+}
+
+// width, height and k1 k2 r1 r2 fx fy cx cy (distortion_coeffs followed by intrinsics, as the reference concatenates
+// them) of a pinhole-radtan camera; false unless the resolution holds 2 ints and there are exactly 4 distortion
+// coefficients and 4 intrinsics, all numbers (the reference reads out of bounds with fewer).
+inline bool KalibrRadtanParameters(const KalibrCamera& camera, int* width, int* height, double params[8]) {
+  if (!camera.has_resolution || !camera.has_distortion_coeffs || !camera.has_intrinsics || camera.resolution.size() != 2 ||
+      camera.distortion_coeffs.size() != 4 || camera.intrinsics.size() != 4)
+    return false;
+  if (!ParseInt32(camera.resolution[0], width) || !ParseInt32(camera.resolution[1], height)) return false;
+  for (int k = 0; k < 8; ++k)
+    if (!ParseDecimal(k < 4 ? camera.distortion_coeffs[k] : camera.intrinsics[k - 4], &params[k])) return false;
+  return true;
+}
+
+// libvis/src/libvis/external_io/colmap_model.cc:47-72: one camera per line, "CAMERA_ID MODEL WIDTH HEIGHT PARAMS[]";
+// lines that are empty or start with '#' are skipped. The cameras come in file order; of an id that appears twice the
+// first is kept (the reference's unordered_map::insert). The parameters are what libstdc++'s
+// `while (!eof) { push_back(0); stream >> back(); }` reads: a line that ends in whitespace (a blank, a tab, a carriage
+// return) gets one more parameter, 0. Where the reference never ends (a token that is not a number) the parameters stop
+// before that token; a line whose first four fields are not an int, a name and two ints is skipped. Returns false if
+// the file cannot be read. io.py's ReadColmapCameras returns the same.
+struct ColmapCamera {
+  int camera_id = 0;
+  std::string model_name;
+  int width = 0, height = 0;
+  std::vector<double> parameters;
+};
+inline bool ReadColmapCameras(const std::string& cameras_txt_path, std::vector<ColmapCamera>* cameras) {
+  using namespace io_detail;
+  std::string text;
+  if (!read_file(cameras_txt_path, &text)) return false;
+  cameras->clear();
+  std::vector<int> seen;
+  auto space = [](char ch) { return ch == ' ' || ch == '\t' || ch == '\v' || ch == '\f' || ch == '\r'; };
+  for (const std::string& line : split_lines(text)) {
+    if (line.empty() || line[0] == '#') continue;
+    std::vector<std::string> tokens;
+    for (size_t a = 0; a < line.size();) {
+      while (a < line.size() && space(line[a])) ++a;
+      size_t b = a;
+      while (b < line.size() && !space(line[b])) ++b;
+      if (b > a) tokens.push_back(line.substr(a, b - a));
+      a = b;
+    }
+    ColmapCamera cam;
+    if (tokens.size() < 4 || !ParseInt32(tokens[0], &cam.camera_id) || !ParseInt32(tokens[2], &cam.width) ||
+        !ParseInt32(tokens[3], &cam.height))
+      continue;
+    cam.model_name = tokens[1];
+    bool stopped = false;
+    for (size_t k = 4; k < tokens.size(); ++k) {
+      double v;
+      if (!ParseDecimal(tokens[k], &v)) {
+        stopped = true;
+        break;
+      }
+      cam.parameters.push_back(v);
+    }
+    if (!stopped && space(line.back())) cam.parameters.push_back(0.0);
+    if (std::find(seen.begin(), seen.end(), cam.camera_id) != seen.end()) continue;
+    seen.push_back(cam.camera_id);
+    cameras->push_back(cam);
+  }
+  return true;
+}
+
+// k1 k2 r1 r2 fx fy cx cy of an OPENCV camera (COLMAP's fx fy cx cy k1 k2 p1 p2 with the halves swapped,
+// visualize_calibration.cc:181-198); false with fewer than 8 parameters.
+inline bool ColmapRadtanParameters(const ColmapCamera& camera, double params[8]) {
+  if (camera.parameters.size() < 8) return false;
+  for (int k = 0; k < 4; ++k) {
+    params[k] = camera.parameters[4 + k];
+    params[4 + k] = camera.parameters[k];
+  }
+  return true;
+}
+
+// legend_error_directions.png of CreateLegends (APP/tools/create_legends.cc:35-54): 200 x 200 RGB pixels, the offset
+// e = (x + 0.5f, y + 0.5f) - (100, 100) in float, dir = (double)atan2f(e.y, e.x), colour (127 + 127 sin(dir) + 0.5,
+// 127 + 127 cos(dir) + 0.5, 127) in double, truncated. io.py's LegendErrorDirectionsImage computes the same bytes with
+// the same C library.
+inline std::vector<uint8_t> LegendErrorDirections() {
+  std::vector<uint8_t> image(200 * 200 * 3);
+  for (int y = 0; y < 200; ++y)
+    for (int x = 0; x < 200; ++x) {
+      const float ex = (static_cast<float>(x) + 0.5f) - 100.f, ey = (static_cast<float>(y) + 0.5f) - 100.f;
+      const double dir = static_cast<double>(atan2f(ey, ex));
+      uint8_t* p = &image[3 * (200 * y + x)];
+      p[0] = static_cast<uint8_t>(127 + 127 * std::sin(dir) + 0.5);
+      p[1] = static_cast<uint8_t>(127 + 127 * std::cos(dir) + 0.5);
+      p[2] = 127;
+    }
+  return image;
 }
 
 }  // namespace b200ba_shim

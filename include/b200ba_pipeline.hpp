@@ -1,7 +1,7 @@
 // b200ba_pipeline.hpp -- C++ host logic of the callers either side of the hot path (SURVEY.md 8f-3 / 8f-4):
 // the outlier deletion between bundle-adjustment rounds, the metric rescaling, the pyramid resampling of the generic
 // models, the calibration report's info files, the comparison of two calibrations, the localization accuracy test and
-// the --bundle_adjustment / --compare_reconstructions tools, over the containers of
+// the --bundle_adjustment / --compare_reconstructions tools and the calibration visualisation tools, over the containers of
 // b200ba_shim.hpp. (RunBundleAdjustment itself -- 8f-2 -- is in b200ba_shim.hpp and runs device-resident in the
 // library.) The Python mirror is camera_calibration_b200/pipeline.py.
 //
@@ -893,6 +893,101 @@ inline int CompareReconstructions(const std::string& reconstruction_path_1, cons
   }
   if (!WriteMeshLabProject(p.project, meshes))
     std::cerr << "Failed to save MeshLab project to: " << p.project << "\n";
+  return EXIT_SUCCESS;
+}
+
+// ---- --visualize_kalibr_calibration, --visualize_colmap_calibration and --create_legends -----------------------------
+// VisualizeCameraModel(camera, path) (tools/visualize_calibration.cc:39-96): the image of b200ba_visualize_camera written
+// as PNG. A camera the library refuses (return code 2: a size below 1, fx or fy 0, a parameter that is not finite) is
+// skipped with a message; EXIT_FAILURE where the file cannot be written; throws on another library error.
+inline int VisualizeCameraToFile(const std::string& name, int width, int height, const double params[8],
+                                 const std::string& path) {
+  std::vector<uint8_t> image(width > 0 && height > 0 ? 3 * static_cast<size_t>(width) * height : 0);
+  const int rc = b200ba_visualize_camera(-1, width, height, params, image.data(), nullptr, nullptr, nullptr);
+  if (rc == 2) {
+    std::cerr << "Camera " << name << " skipped: " << b200ba_last_error(nullptr) << "\n";
+    return EXIT_SUCCESS;
+  }
+  if (rc != 0) throw std::runtime_error(std::string("b200ba_visualize_camera: ") + b200ba_last_error(nullptr));
+  if (!WritePNG(path, width, height, 3, image.data())) {
+    std::cerr << "Cannot write file: " << path << "\n";
+    return EXIT_FAILURE;
+  }
+  return EXIT_SUCCESS;
+}
+
+// tools/visualize_calibration.cc:98-165: for cam0, cam1, ... of the camchain up to the first missing key
+// (ReadKalibrCamchain), the observation directions of every pinhole-radtan camera in their canonical orientation
+// written to <camchain_path>.camN.png; other cameras are skipped with the reference's messages ("Camera model not
+// handled: ...", "Distortion model not handled: ..."), and so are cameras without a resolution, 4 distortion
+// coefficients and 4 intrinsics; messages go to stderr in file order. Kalibr's pixel-centre cu, cv are used as
+// pixel-corner values, as the reference uses them. Returns EXIT_SUCCESS, or EXIT_FAILURE with "Cannot read file: ..."
+// where the file cannot be read or parsed, or where a PNG cannot be written. pipeline.py's VisualizeKalibrCalibration
+// prints and writes the same bytes.
+inline int VisualizeKalibrCalibration(const std::string& camchain_path) {
+  std::vector<KalibrCamera> cameras;
+  if (!ReadKalibrCamchain(camchain_path, &cameras)) {
+    std::cerr << "Cannot read file: " << camchain_path << "\n";
+    return EXIT_FAILURE;
+  }
+  for (const KalibrCamera& cam : cameras) {
+    if (cam.camera_model != "pinhole") {
+      std::cerr << "Camera model not handled: " << cam.camera_model << "\n";
+      continue;
+    }
+    if (cam.distortion_model != "radtan") {
+      std::cerr << "Distortion model not handled: " << cam.distortion_model << "\n";
+      continue;
+    }
+    int width = 0, height = 0;
+    double params[8];
+    if (!KalibrRadtanParameters(cam, &width, &height, params)) {
+      std::cerr << "Camera " << cam.name << " skipped: it needs a resolution, 4 distortion coefficients and 4 intrinsics\n";
+      continue;
+    }
+    if (VisualizeCameraToFile(cam.name, width, height, params, camchain_path + "." + cam.name + ".png") != EXIT_SUCCESS)
+      return EXIT_FAILURE;
+  }
+  return EXIT_SUCCESS;
+}
+
+// tools/visualize_calibration.cc:167-207: for every camera of a COLMAP cameras.txt (ReadColmapCameras, file order), the
+// observation directions of every OPENCV camera in their canonical orientation written to <cameras_path>.cam<id>.png;
+// other models are skipped with "Camera model not handled: ...", and so are cameras with fewer than 8 parameters;
+// messages go to stderr in file order. Returns EXIT_SUCCESS, or EXIT_FAILURE with "Cannot read file: ..." or where a
+// PNG cannot be written. pipeline.py's VisualizeColmapCalibration prints and writes the same bytes.
+inline int VisualizeColmapCalibration(const std::string& cameras_path) {
+  std::vector<ColmapCamera> cameras;
+  if (!ReadColmapCameras(cameras_path, &cameras)) {
+    std::cerr << "Cannot read file: " << cameras_path << "\n";
+    return EXIT_FAILURE;
+  }
+  for (const ColmapCamera& cam : cameras) {
+    const std::string name = "cam" + std::to_string(cam.camera_id);
+    if (cam.model_name != "OPENCV") {
+      std::cerr << "Camera model not handled: " << cam.model_name << "\n";
+      continue;
+    }
+    double params[8];
+    if (!ColmapRadtanParameters(cam, params)) {
+      std::cerr << "Camera " << name << " skipped: OPENCV needs 8 parameters, the file gives " << cam.parameters.size()
+                << "\n";
+      continue;
+    }
+    if (VisualizeCameraToFile(name, cam.width, cam.height, params, cameras_path + "." + name + ".png") != EXIT_SUCCESS)
+      return EXIT_FAILURE;
+  }
+  return EXIT_SUCCESS;
+}
+
+// tools/create_legends.cc:35-54: <directory>/legend_error_directions.png (LegendErrorDirections). Returns EXIT_SUCCESS,
+// or EXIT_FAILURE with "Cannot write file: ...". pipeline.py's CreateLegends writes the same bytes.
+inline int CreateLegends(const std::string& directory = ".") {
+  const std::string path = io_detail::join(directory, "legend_error_directions.png");
+  if (!WritePNG(path, 200, 200, 3, LegendErrorDirections().data())) {
+    std::cerr << "Cannot write file: " << path << "\n";
+    return EXIT_FAILURE;
+  }
   return EXIT_SUCCESS;
 }
 

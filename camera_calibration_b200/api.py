@@ -266,6 +266,26 @@ def VisualizeCameraModel(width: int, height: int, params, device: int = -1, dire
     return img, rot, dirs, ms.value
 
 
+def IntersectFeatures(n_datasets: int, list_offsets, xy, threshold: float = 3.0, device: int = -1):
+    """The feature level of --intersect_datasets (APP/tools/intersect_datasets.cc:130-225) on the device
+    (``b200ba_intersect_features``; the rules are specified in include/b200ba.h): list_offsets [n_lists * n_datasets
+    + 1] int64 splits xy [N, 2] float32 into n_lists independent lists of n_datasets feature lists each. Returns
+    (keep [N] bool, cabi.IntersectionReport, device_ms)."""
+    lib = cabi.load_library()
+    off = np.ascontiguousarray(np.asarray(list_offsets, dtype=np.int64).reshape(-1))
+    pts = np.ascontiguousarray(np.asarray(xy, dtype=np.float32).reshape(-1, 2))
+    if off.size < 1 or (off.size - 1) % max(int(n_datasets), 1) or off[-1] != len(pts):
+        raise ValueError("IntersectFeatures: list_offsets must hold n_lists * n_datasets + 1 entries ending at len(xy)")
+    keep = np.zeros(len(pts), np.uint8)
+    rep = cabi.IntersectionReport()
+    ms = C.c_double(0)
+    _check(lib.b200ba_intersect_features(device, int(n_datasets), (off.size - 1) // max(int(n_datasets), 1),
+                                         off.ctypes.data_as(C.POINTER(C.c_int64)),
+                                         pts.ctypes.data_as(C.POINTER(C.c_float)), float(threshold), _u8p(keep),
+                                         C.byref(rep), C.byref(ms)))
+    return keep.astype(bool), rep, ms.value
+
+
 def nccl_unique_id() -> bytes:
     lib = cabi.load_library()
     buf = (C.c_uint8 * cabi.NCCL_UNIQUE_ID_BYTES)()

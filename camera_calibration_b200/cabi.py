@@ -273,6 +273,16 @@ class LineOffsetsReport(C.Structure):
     ]
 
 
+class IntersectionReport(C.Structure):
+    """b200ba_intersection_report: the counts of one feature intersection."""
+    _fields_ = [
+        ("intersections", C.c_int64),
+        ("kept", C.c_int64),
+        ("uncovered", C.c_int64),
+        ("capped", C.c_int64),
+    ]
+
+
 class FitReport(C.Structure):
     """b200ba_fit_report."""
     _fields_ = [
@@ -467,6 +477,8 @@ SYMBOLS = {
     "b200ba_render_voronoi": (C.c_int, [C.c_int, C.c_int32, C.c_int32, C.c_int64, _I32, C.POINTER(C.c_float),
                                         C.POINTER(C.c_uint8), _D]),
     "b200ba_visualize_camera": (C.c_int, [C.c_int, C.c_int32, C.c_int32, _D, C.POINTER(C.c_uint8), _D, _D, _D]),
+    "b200ba_intersect_features": (C.c_int, [C.c_int, C.c_int32, C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_float),
+                                            C.c_double, C.POINTER(C.c_uint8), C.POINTER(IntersectionReport), _D]),
     "b200ba_snapshot_state": (C.c_int, [C.c_void_p]),
     "b200ba_restore_state": (C.c_int, [C.c_void_p]),
     "b200ba_version": (C.c_char_p, []),

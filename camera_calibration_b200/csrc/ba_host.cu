@@ -3289,6 +3289,84 @@ int b200ba_visualize_camera(int device, int32_t width, int32_t height, const dou
   return cs.rc;
 }
 
+// Stand-alone feature intersection of --intersect_datasets (APP/tools/intersect_datasets.cc:130-225): the walk and
+// the final pass of every list on the device. The argument checks come first and touch no CUDA state.
+int b200ba_intersect_features(int device, int32_t n_datasets, int64_t n_lists, const int64_t* list_offsets,
+                              const float* xy, double threshold, uint8_t* keep, b200ba_intersection_report* report,
+                              double* device_ms) {
+  if (n_datasets < 1 || n_datasets > 32 || n_lists < 0 || n_lists >= (int64_t(1) << 31) || !list_offsets) {
+    g_create_error = "b200ba_intersect_features: needs 1 <= n_datasets <= 32, 0 <= n_lists < 2^31 and list_offsets";
+    return 2;
+  }
+  const int64_t n_off = n_lists * n_datasets;
+  if (list_offsets[0] != 0) {
+    g_create_error = "b200ba_intersect_features: list_offsets must start at 0";
+    return 2;
+  }
+  int64_t max_list = 0;
+  for (int64_t k = 0; k < n_off; ++k)
+    if (list_offsets[k + 1] < list_offsets[k]) {
+      g_create_error = "b200ba_intersect_features: list_offsets must not decrease";
+      return 2;
+    }
+  for (int64_t l = 0; l < n_lists; ++l)
+    max_list = std::max(max_list, list_offsets[(l + 1) * n_datasets] - list_offsets[l * n_datasets]);
+  if (max_list >= (int64_t(1) << 31)) {
+    g_create_error = "b200ba_intersect_features: a list holds 2^31 features or more";
+    return 2;
+  }
+  const int64_t n = list_offsets[n_off];
+  if (n > 0 && (!xy || !keep)) {
+    g_create_error = "b200ba_intersect_features: xy and keep are required";
+    return 2;
+  }
+  const double thr2 = threshold * threshold;
+  float bound = static_cast<float>(thr2);  // the largest float <= thr2, so that float d <= bound iff (double)d <= thr2
+  if (static_cast<double>(bound) > thr2) bound = std::nextafter(bound, -std::numeric_limits<float>::infinity());
+  CallScope cs(&g_create_error);
+  if (int rc = cs.use_device(device)) return rc;
+  unsigned long long counts[2] = {0, 0};
+  int64_t intersections = 0, kept = 0;
+  if (n > 0) {
+    int64_t* d_off = nullptr;
+    float2* d_xy = nullptr;
+    uint8_t* d_keep = nullptr;
+    float2* d_cent = nullptr;
+    int* d_nc = nullptr;
+    unsigned long long* d_counts = nullptr;
+    cs.alloc(&d_off, n_off + 1);
+    cs.alloc(&d_xy, n);
+    cs.alloc(&d_keep, n);
+    cs.alloc(&d_cent, n);
+    cs.alloc(&d_nc, n_lists);
+    cs.alloc(&d_counts, 2);
+    if (cs.rc == 0) cs.ok(cudaMemcpy(d_off, list_offsets, sizeof(int64_t) * (n_off + 1), cudaMemcpyHostToDevice));
+    if (cs.rc == 0) cs.ok(cudaMemcpy(d_xy, xy, sizeof(float2) * n, cudaMemcpyHostToDevice));
+    if (cs.rc == 0) cs.ok(cudaMemset(d_keep, 1, n));
+    if (cs.rc == 0) cs.ok(cudaMemset(d_counts, 0, sizeof(counts)));
+    if (cs.rc == 0) {
+      cs.record(0, 0);
+      launch_intersect_features(n_datasets, n_lists, max_list, d_off, d_xy, bound, d_keep, d_cent, d_nc, d_counts, 0);
+      cs.record(1, 0);
+      cs.ok(cudaGetLastError());
+      cs.ok(cudaMemcpy(keep, d_keep, n, cudaMemcpyDeviceToHost));
+      cs.ok(cudaMemcpy(counts, d_counts, sizeof(counts), cudaMemcpyDeviceToHost));
+      std::vector<int> nc(n_lists);
+      cs.ok(cudaMemcpy(nc.data(), d_nc, sizeof(int) * n_lists, cudaMemcpyDeviceToHost));
+      for (int v : nc) intersections += v;
+      for (int64_t k = 0; k < n; ++k) kept += keep[k];
+    }
+  }
+  if (cs.rc == 0 && report) {
+    report->intersections = intersections;
+    report->kept = kept;
+    report->uncovered = static_cast<int64_t>(counts[0]);
+    report->capped = static_cast<int64_t>(counts[1]);
+  }
+  if (cs.rc == 0 && device_ms) *device_ms = n > 0 ? cs.elapsed_ms(0, 1) : 0.0;
+  return cs.rc;
+}
+
 // Eigen::LDLT<MatrixXd, Lower>(A.selfadjointView<Upper>()).solve(b) for n = 3 (SolveDensely, LV/lm_optimizer.h:1022-1023):
 // symmetric pivoting on the largest remaining |diagonal| entry as Eigen's left-looking factorisation sees it (the
 // ORIGINAL values of the trailing diagonal), then x = P^T L^-T D^-1 L^-1 P b with 1 / d_i taken as 0 where

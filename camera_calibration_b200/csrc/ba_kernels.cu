@@ -3982,4 +3982,174 @@ void launch_mask_fixed(const Layout& L, const SystemDev& sys, const FixedRanges&
   }
 }
 
+// ---- feature intersection (b200ba_intersect_features; APP/tools/intersect_datasets.cc:130-225) -------------------
+// The reference erases features from std::vectors while it walks dataset 0 by index. Erasing keeps the order of the
+// remaining elements, so every position in a current vector is the rank of an original index among the alive ones,
+// and the same walk runs on the original arrays with one alive flag per feature:
+//   - "the last index o with d <= best" is the last ALIVE original index with the smallest d <= thr2: an erased
+//     feature's x is overwritten with NaN, so its d is NaN and never accepted;
+//   - covered-index vectors of two passes of one fixed-point loop compare equal as positions exactly when they do as
+//     original indices (nothing is erased inside the loop);
+//   - after a rejection the reference erases the covered features and steps f back by one where covered[0] <= f,
+//     then advances it by one. With covered[0] < f the element at f moved to f - 1, so the new f is the element after
+//     the old f; with covered[0] == f it is the element after the erased one; with covered[0] > f, f + 1 is the next
+//     element that is still there. In each case: the next alive original index after f. With covered[0] == -1 the
+//     same f runs again, and after an acceptance the next alive index follows.
+// Comparisons d <= thr2 (float d, double thr2) are d <= bound in float, bound = the largest float <= thr2.
+constexpr int kIntersectMaxPasses = 100;
+constexpr int kIntersectSmemBytes = 200 * 1024;  // lists up to 25600 features are staged in shared memory
+
+// (float)(p.x - cx)^2 + (float)(p.y - cy)^2, each operation rounded on its own
+__device__ __forceinline__ float intersect_d2(float2 p, float cx, float cy) {
+  const float dx = __fsub_rn(p.x, cx), dy = __fsub_rn(p.y, cy);
+  return __fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy));
+}
+
+// The closest feature of pts [b, e) to (cx, cy) with d <= bound, ties to the later index; -1 if none. One warp; every
+// lane returns the same index ((d, index) is reduced under one total order: smaller d first, then larger index).
+__device__ int intersect_closest(const float2* pts, int b, int e, float cx, float cy, float bound, int lane) {
+  float best = bound;
+  int idx = -1;
+#pragma unroll 4
+  for (int k = b + lane; k < e; k += 32) {
+    const float d = intersect_d2(pts[k], cx, cy);
+    if (d <= best) {  // a lane sees its indices in increasing order, so a tie goes to the later one
+      best = d;
+      idx = k;
+    }
+  }
+#pragma unroll
+  for (int s = 16; s; s >>= 1) {
+    const float ob = __shfl_xor_sync(0xffffffffu, best, s);
+    const int oi = __shfl_xor_sync(0xffffffffu, idx, s);
+    if (ob < best || (ob == best && oi > idx)) {
+      best = ob;
+      idx = oi;
+    }
+  }
+  return idx;
+}
+
+// One CTA per list, one warp per dataset: warp w answers the closest-feature query of dataset w in every pass, and
+// every thread then forms the same centre from the covered features in dataset order. The walk, the fixed-point loop
+// and the acceptance are uniform over the CTA. Both loops are bounded: a pass loop by kIntersectMaxPasses, the walk by
+// n0 advances plus one re-run per erased feature (a re-run without an erasure is the pinned "uncovered" case, which
+// advances).
+__global__ void __launch_bounds__(1024) intersect_walk_kernel(int D, const int64_t* __restrict__ off, float2* xy,
+                                                              int use_smem, float bound, uint8_t* keep, float2* centres,
+                                                              int* n_centres, unsigned long long* counts) {
+  extern __shared__ float2 s_pts[];
+  __shared__ int s_cov[32], s_old[32], s_b[33];
+  const int64_t l = blockIdx.x;
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t* o = off + l * D;
+  const int64_t base = o[0];
+  const int total = static_cast<int>(o[D] - base);
+  float2* pts = xy + base;
+  if (use_smem) {
+    for (int k = threadIdx.x; k < total; k += blockDim.x) s_pts[k] = pts[k];
+    pts = s_pts;
+  }
+  if (threadIdx.x <= D) s_b[threadIdx.x] = static_cast<int>(o[threadIdx.x] - base);
+  __syncthreads();
+  const int n0 = s_b[1], bw = s_b[w], ew = s_b[w + 1];
+  uint8_t* alive = keep + base;
+  float2* cent = centres + base;
+  int nc = 0;
+  unsigned long long uncovered = 0, capped = 0;
+  int f = 0;
+  while (f < n0) {
+    float cx = pts[f].x, cy = pts[f].y;
+    int k = -1;
+    for (int pass = 1;; ++pass) {
+      k = intersect_closest(pts, bw, ew, cx, cy, bound, lane);
+      if (lane == 0) s_cov[w] = k;
+      __syncthreads();
+      float sx = 0.f, sy = 0.f;
+      int count = 0;
+      bool same = pass > 1;  // the first pass compares against an empty vector
+      for (int i = 0; i < D; ++i) {
+        const int ki = s_cov[i];
+        if (ki >= 0) {
+          const float2 p = pts[ki];
+          sx = __fadd_rn(sx, p.x);
+          sy = __fadd_rn(sy, p.y);
+          ++count;
+        }
+        same = same && ki == s_old[i];
+      }
+      cx = __fdiv_rn(sx, static_cast<float>(count));
+      cy = __fdiv_rn(sy, static_cast<float>(count));
+      __syncthreads();  // s_cov and s_old are read by every thread before they change
+      if (same) break;
+      if (lane == 0) s_old[w] = k;
+      if (pass == kIntersectMaxPasses) {
+        ++capped;
+        break;
+      }
+    }
+    bool accept = true, any = false;
+    for (int i = 0; i < D; ++i) {
+      accept = accept && s_cov[i] >= 0;
+      any = any || s_cov[i] >= 0;
+    }
+    const int c0 = s_cov[0];
+    if (accept) {
+      if (threadIdx.x == 0) cent[nc] = make_float2(cx, cy);
+      ++nc;
+    } else if (!any) {
+      ++uncovered;
+    } else if (lane == 0 && k >= 0) {
+      pts[k].x = __int_as_float(0x7fc00000);
+      alive[k] = 0;
+    }
+    __syncthreads();  // erasures are visible, and s_cov is read, before the next walk step
+    if (accept || !any || c0 != -1) {
+      ++f;
+      while (f < n0 && !alive[f]) ++f;
+    }
+  }
+  if (threadIdx.x == 0) {
+    n_centres[l] = nc;
+    if (uncovered) atomicAdd(counts, uncovered);
+    if (capped) atomicAdd(counts + 1, capped);
+  }
+}
+
+// The final pass: every alive feature of list l is kept where some accepted centre lies within thr2 of it.
+__global__ void intersect_keep_kernel(int D, const int64_t* __restrict__ off, const float2* __restrict__ xy, float bound,
+                                      const float2* __restrict__ centres, const int* __restrict__ n_centres,
+                                      uint8_t* keep) {
+  const int64_t l = blockIdx.x;
+  const int64_t base = off[l * D], end = off[l * D + D];
+  const int nc = n_centres[l];
+  const float2* cent = centres + base;
+  for (int64_t k = base + threadIdx.x; k < end; k += blockDim.x) {
+    if (!keep[k]) continue;
+    const float2 p = xy[k];
+    uint8_t near = 0;
+    for (int c = 0; c < nc; ++c) {
+      const float2 q = __ldg(cent + c);
+      if (intersect_d2(p, q.x, q.y) <= bound) {  // (c - p)^2 == (p - c)^2 bit for bit
+        near = 1;
+        break;
+      }
+    }
+    keep[k] = near;
+  }
+}
+
+void launch_intersect_features(int d, int64_t n_lists, int64_t max_list, const int64_t* off, float2* xy, float bound,
+                               uint8_t* keep, float2* centres, int* n_centres, unsigned long long* counts,
+                               cudaStream_t s) {
+  if (n_lists == 0 || max_list == 0) return;
+  const size_t bytes = sizeof(float2) * static_cast<size_t>(max_list);
+  const bool use_smem = bytes <= static_cast<size_t>(kIntersectSmemBytes);
+  if (use_smem && bytes > 48 * 1024)
+    cudaFuncSetAttribute(intersect_walk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
+  intersect_walk_kernel<<<static_cast<unsigned>(n_lists), 32 * d, use_smem ? bytes : 0, s>>>(
+      d, off, xy, use_smem ? 1 : 0, bound, keep, centres, n_centres, counts);
+  intersect_keep_kernel<<<static_cast<unsigned>(n_lists), 256, 0, s>>>(d, off, xy, bound, centres, n_centres, keep);
+}
+
 }  // namespace b200ba

@@ -104,6 +104,13 @@ void launch_observation_directions(const CamDev& c, const double* intr, uint8_t*
 void launch_visualize_orientation(const double* params, int w, int h, double2* win, double* rot, cudaStream_t s);
 void launch_visualize_camera(const double* params, int w, int h, const double* rot, uint8_t* img, double* dirs,
                              cudaStream_t s);
+// feature intersection of b200ba_intersect_features: n_lists independent lists of d datasets (off [n_lists * d + 1],
+// xy [off[n_lists * d]] -- its erased features are overwritten with NaN), bound = the largest float <= thr2 (NaN for a
+// NaN thr2), max_list = the largest list. keep [N] must hold 1 on entry; centres [N] and n_centres [n_lists] are
+// scratch; counts [2] (uncovered walks, capped loops) are added to.
+void launch_intersect_features(int d, int64_t n_lists, int64_t max_list, const int64_t* off, float2* xy, float bound,
+                               uint8_t* keep, float2* centres, int* n_centres, unsigned long long* counts,
+                               cudaStream_t s);
 void launch_generic_block_inverse(int bs, int nb, int nd, const double* D, const double* B, const double* b1,
                                   double* DinvB, double* Dinvb, cudaStream_t s);
 void launch_symmetrize(int n, double* M, cudaStream_t s);

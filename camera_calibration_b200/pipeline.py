@@ -660,3 +660,134 @@ def CreateLegends(directory: str = ".") -> int:
         print(f"Cannot write file: {path}", file=sys.stderr)
         return 1
     return 0
+
+
+def _feature_count(dataset) -> int:
+    return sum(len(dataset.GetImageset(k).FeaturesOfCamera(c)["id"])
+               for k in range(dataset.ImagesetCount()) for c in range(dataset.num_cameras()))
+
+
+def IntersectDatasets(dataset_paths, intersection_threshold: float = 3.0, intersect=None) -> int:
+    """The ``--intersect_datasets`` tool (tools/intersect_datasets.cc:41-261): of several ``dataset.bin`` files of one
+    image sequence (e.g. one per feature detector), keep only the features that all of them detected, and write each
+    to ``<path>.intersected.bin``. Imagesets are matched by filename:
+      - dataset 0's imagesets are walked by index; a filename missing from another dataset is deleted from every
+        dataset that has it (the first imageset of a repeated filename, as ``unordered_map::insert`` keeps it) and the
+        walk steps back by one. A later duplicate in dataset 0 of a filename already deleted is itself deleted (the
+        reference walks it forever);
+      - otherwise dataset 0's imageset and dataset i's first imageset of that filename form a task; at the end every
+        imageset of datasets 1.. whose filename dataset 0 no longer holds is deleted.
+    The features of every (task, camera) are intersected by ``intersect`` (default ``api.IntersectFeatures``, on the
+    device; the rules are in include/b200ba.h). Tasks that share an imageset run in separate calls in task order, so a
+    later task reads the features an earlier one thinned, as in the reference. Messages go to stderr; the two pinned
+    counts are printed where they are not zero. Returns EXIT_SUCCESS, or EXIT_FAILURE for an empty path list or more than
+    32 paths (the device walk runs one warp per dataset in one CTA; the reference has no such limit), a file
+    that cannot be read or written, or datasets with different camera counts. The C++ IntersectDatasets
+    (b200ba_pipeline.hpp) prints and writes the same bytes."""
+    import sys
+    from . import io
+    intersect = intersect or api.IntersectFeatures
+    paths = list(dataset_paths)
+    if not paths:
+        print("IntersectDatasets needs at least one dataset", file=sys.stderr)
+        return 1
+    if len(paths) > 32:
+        print(f"IntersectDatasets takes at most 32 datasets, not {len(paths)}", file=sys.stderr)
+        return 1
+    datasets = []
+    for i, path in enumerate(paths):
+        print(f"Dataset {i}: {path}", file=sys.stderr)
+        ds = io.LoadDataset(path)
+        if ds is None:
+            print(f"Cannot read file: {path}", file=sys.stderr)
+            return 1
+        if i > 0 and ds.num_cameras() != datasets[0].num_cameras():
+            print(f"Number of cameras in dataset {path} does not match the number of cameras in dataset {paths[0]}",
+                  file=sys.stderr)
+            return 1
+        datasets.append(ds)
+    for i, ds in enumerate(datasets):
+        print(f"Input features in dataset {i}: {_feature_count(ds)} (#imagesets: {ds.ImagesetCount()})", file=sys.stderr)
+
+    n = len(datasets)
+    maps = []
+    for ds in datasets:
+        m = {}
+        for k in range(ds.ImagesetCount()):
+            m.setdefault(ds.GetImageset(k).GetFilename(), k)
+        maps.append(m)
+    tasks = []
+    index = 0
+    while index < datasets[0].ImagesetCount():
+        walked = datasets[0].GetImageset(index)
+        name = walked.GetFilename()
+        if all(name in maps[i] for i in range(1, n)):
+            tasks.append([walked] + [datasets[i].GetImageset(maps[i][name]) for i in range(1, n)])
+            index += 1
+            continue
+        for i in range(n):
+            if name in maps[i]:
+                doomed = maps[i].pop(name)
+            elif i == 0:
+                print(f"Imageset {name} of dataset 0 deleted: its filename was deleted before", file=sys.stderr)
+                doomed = index
+            else:
+                continue
+            datasets[i].DeleteImageset(doomed)
+            for key, k in maps[i].items():
+                if k > doomed:
+                    maps[i][key] = k - 1
+
+    # waves: a task runs after every earlier task that shares one of its imagesets
+    waves, last_wave = [], {}
+    for task in tasks:
+        w = max((last_wave.get(id(s), -1) for s in task), default=-1) + 1
+        for s in task:
+            last_wave[id(s)] = w
+        if w == len(waves):
+            waves.append([])
+        waves[w].append(task)
+    ncam = datasets[0].num_cameras()
+    uncovered = capped = 0
+    for wave in waves:
+        groups = [[s.FeaturesOfCamera(c) for s in task] for task in wave for c in range(ncam)]
+        sizes = [len(ft["id"]) for group in groups for ft in group]
+        if sum(sizes) == 0:
+            continue
+        offsets = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
+        xy = np.concatenate([ft["xy"] for group in groups for ft in group]).astype(np.float32)
+        keep, report, _ = intersect(n, offsets, xy, intersection_threshold)
+        uncovered += report.uncovered
+        capped += report.capped
+        k = 0
+        for task in wave:
+            for c in range(ncam):
+                for s in task:
+                    ft = s.FeaturesOfCamera(c)
+                    m = keep[offsets[k]:offsets[k + 1]]
+                    s.SetFeaturesOfCamera(c, ft["xy"][m], ft["id"][m], ft["index"][m])
+                    k += 1
+    if uncovered:
+        print(f"Features rejected with nothing covered, left in place: {uncovered}", file=sys.stderr)
+    if capped:
+        print(f"Fixed-point loops stopped after 100 passes: {capped}", file=sys.stderr)
+
+    for i in range(1, n):
+        k = 0
+        while k < datasets[i].ImagesetCount():
+            if datasets[i].GetImageset(k).GetFilename() not in maps[0]:
+                datasets[i].DeleteImageset(k)
+            else:
+                k += 1
+    for path, ds in zip(paths, datasets):
+        out = path + ".intersected.bin"
+        try:
+            ok = io.SaveDataset(out, ds)
+        except OSError:
+            ok = False
+        if not ok:
+            print(f"Cannot write file: {out}", file=sys.stderr)
+            return 1
+    for i, ds in enumerate(datasets):
+        print(f"Remaining features in dataset {i}: {_feature_count(ds)}", file=sys.stderr)
+    return 0

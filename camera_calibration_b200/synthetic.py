@@ -499,3 +499,36 @@ def make_problem(config: int = 2, *, seed: Optional[int] = None, n_imagesets: Op
                 image=(W, H), grid=(cams[0].grid_width, cams[0].grid_height), noise_px=noise_px,
                 pose_redraws=n_redraw, f=f)
     return SyntheticProblem(f"config{config}", problem, init, gt, seed, info)
+
+
+def flatten_lists(lists):
+    """Feature lists for ``api.IntersectFeatures``: [[xy of dataset 0, xy of dataset 1, ...] per list] ->
+    (list_offsets [n_lists * D + 1] int64, xy [N, 2] float32)."""
+    arrays = [np.asarray(a, np.float32).reshape(-1, 2) for group in lists for a in group]
+    offsets = np.concatenate([[0], np.cumsum([len(a) for a in arrays])]).astype(np.int64)
+    return offsets, np.concatenate(arrays) if arrays else np.zeros((0, 2), np.float32)
+
+
+def intersection_lists(seed: int = 0, d: int = 2, config: int = 2):
+    """D feature lists per (imageset, camera) of a config-sized problem, as ``--intersect_datasets`` sees them: dataset 0
+    is the observations of make_problem(config); every other dataset jitters each feature by up to 0.5 px, drops 5 %,
+    adds 5 % spurious features (uniform over the image's feature box) and shuffles each image. Returns
+    [[xy of dataset 0, ..., xy of dataset d - 1] per (imageset, camera)]."""
+    pb = make_problem(config=config).problem
+    rng = np.random.default_rng(seed)
+    key = pb.obs_imageset.astype(np.int64) * (int(pb.obs_camera.max()) + 1) + pb.obs_camera
+    order = np.argsort(key, kind="stable")
+    bounds = np.flatnonzero(np.diff(key[order])) + 1
+    lists = []
+    for idx in np.split(order, bounds):
+        base = pb.obs_xy[idx].astype(np.float32)
+        group = [base]
+        for _ in range(d - 1):
+            keep = rng.random(len(base)) >= 0.05
+            pts = base[keep] + rng.uniform(-0.5, 0.5, (keep.sum(), 2)).astype(np.float32)
+            lo, hi = base.min(0), base.max(0)
+            spur = rng.uniform(lo, hi, (int(round(0.05 * len(base))), 2)).astype(np.float32)
+            pts = np.concatenate([pts, spur])
+            group.append(pts[rng.permutation(len(pts))].astype(np.float32))
+        lists.append(group)
+    return lists

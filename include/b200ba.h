@@ -562,6 +562,51 @@ B200BA_API int b200ba_line_offsets(int device, const b200ba_camera* cam, const d
                                    b200ba_line_offsets_report* report, uint8_t* image, double* offsets, int32_t obj_step,
                                    double* obj_lines, int64_t* n_obj, double* device_ms);
 
+/* ---- feature intersection (APP/tools/intersect_datasets.cc:130-225, the feature level of --intersect_datasets):
+ * of D feature lists of one (imageset, camera) -- one list per dataset, e.g. one per feature detector -- keep only the
+ * features that every list detected. A "list" below is one such group of D lists (one per dataset); n_lists of them
+ * are processed independently. thr2 = threshold * threshold in double (so a negative threshold acts as its absolute
+ * value and a NaN threshold covers nothing). All coordinates are the given float xy.
+ *   distance: d = (float)(x_o - c_x)^2 + (float)(y_o - c_y)^2 in float, each operation rounded on its own, compared
+ *     with thr2 as a double.
+ *   closest feature of dataset i to a centre c: the LAST index o, in list order among the features not yet erased,
+ *     with d <= best, best starting at thr2 and taking every accepted d; so ties go to the later index, d == thr2 is
+ *     covered and a NaN d never is. None (-1) where no d <= thr2.
+ *   fixed-point loop of a centre: each pass finds the closest feature of every dataset, then sets the centre to the
+ *     float sum of the covered features in dataset order divided by (float)count (0 / 0 = NaN when nothing is
+ *     covered). It stops after the first pass whose covered-index vector equals the previous pass's (the first pass
+ *     compares against an empty vector, so there are at least two passes), or after 100 passes, taking the 100th
+ *     pass's result (the reference never ends on a loop that cycles without repeating its previous pass).
+ *   walk: for f over dataset 0's features, from the feature's own xy: if every dataset covered a feature, the centre
+ *     is accepted; otherwise every covered feature is erased and, where dataset 0 covered nothing (covered[0] == -1),
+ *     the same f is walked again, else the next feature after f that is not erased. Accepted features stay and may be
+ *     covered again by a later f.
+ *   end: every feature whose distance to every accepted centre is > thr2 (or NaN) is erased.
+ * Erasing only removes elements and keeps the order of the rest, so the walk is computed with one "alive" flag per
+ * feature of the original order: the last index in list order is the last alive original index, and the next f is the
+ * next alive feature after the current one. One rule of the reference never ends and is pinned here:
+ *   - a rejected pass that covered nothing in any dataset (a feature with a NaN or infinite coordinate, a NaN
+ *     threshold, or a centre that moved out of reach of everything) would re-run the same f forever; that f is
+ *     rejected, left in place, and the walk moves on to the next feature. A rejection with covered[0] == -1 that
+ *     erased features elsewhere is re-run as in the reference (it ends: every re-run erases at least one feature).
+ * list_offsets [n_lists * D + 1]: list l, dataset i holds the features [list_offsets[l D + i], list_offsets[l D + i
+ * + 1]) of xy [2 N] (x, y), N = list_offsets[n_lists D]; the offsets start at 0 and do not decrease, and one list
+ * holds fewer than 2^31 features. The lists of one call must be independent (no feature in two lists); a caller with
+ * tasks that share features runs them in order, one call after the other. keep [N]: 1 for a feature that survives,
+ * else 0. report (nullable): the counts below. device_ms (nullable): device time of the intersection.
+ * Stand-alone (allocates, computes, frees). Returns 2 for a bad argument before any CUDA call (n_datasets < 1 or
+ * > 32, n_lists < 0 or >= 2^31, a NULL list_offsets, a NULL xy or keep with N > 0, offsets that do not start at 0 or
+ * decrease, a list of 2^31 features or more), 3 without a device. Repeated calls give identical bytes. */
+typedef struct b200ba_intersection_report {
+  int64_t intersections;  /* accepted centres over all lists */
+  int64_t kept;           /* features with keep == 1 */
+  int64_t uncovered;      /* walks of a dataset-0 feature rejected with nothing covered, left in place (pinned above) */
+  int64_t capped;         /* fixed-point loops stopped after 100 passes */
+} b200ba_intersection_report;
+B200BA_API int b200ba_intersect_features(int device, int32_t n_datasets, int64_t n_lists, const int64_t* list_offsets,
+                                         const float* xy, double threshold, uint8_t* keep,
+                                         b200ba_intersection_report* report, double* device_ms);
+
 /* ---- multi-GPU: imagesets sharded over ranks, one NCCL all-reduce per H/b build --- */
 #define B200BA_NCCL_UNIQUE_ID_BYTES 128
 B200BA_API int b200ba_nccl_unique_id(uint8_t id[B200BA_NCCL_UNIQUE_ID_BYTES]);

@@ -19,6 +19,7 @@
 #include <iostream>
 #include <map>
 #include <sstream>
+#include <unordered_map>
 
 #include "b200ba_io.hpp"
 #include "b200ba_shim.hpp"
@@ -988,6 +989,172 @@ inline int CreateLegends(const std::string& directory = ".") {
     std::cerr << "Cannot write file: " << path << "\n";
     return EXIT_FAILURE;
   }
+  return EXIT_SUCCESS;
+}
+
+// ---- --intersect_datasets ------------------------------------------------------------------------------------------
+// (n_datasets, list_offsets [n_lists * n_datasets + 1], xy [2 N], threshold) -> keep [N], report: the feature level of
+// b200ba_intersect_features. The default runs it on the device.
+using IntersectLists = std::function<void(int32_t, const std::vector<int64_t>&, const std::vector<float>&, double,
+                                          std::vector<uint8_t>*, b200ba_intersection_report*)>;
+
+inline void IntersectListsOnDevice(int32_t n_datasets, const std::vector<int64_t>& offsets, const std::vector<float>& xy,
+                                   double threshold, std::vector<uint8_t>* keep, b200ba_intersection_report* report) {
+  keep->assign(xy.size() / 2, 0);
+  const int64_t n_lists = static_cast<int64_t>(offsets.size() - 1) / n_datasets;
+  if (b200ba_intersect_features(-1, n_datasets, n_lists, offsets.data(), xy.data(), threshold, keep->data(), report,
+                                nullptr) != 0)
+    throw std::runtime_error(std::string("b200ba_intersect_features: ") + b200ba_last_error(nullptr));
+}
+
+inline int64_t IntersectFeatureCount(const Dataset& dataset) {
+  int64_t count = 0;
+  for (int k = 0; k < dataset.ImagesetCount(); ++k)
+    for (int c = 0; c < dataset.num_cameras(); ++c) count += dataset.GetImageset(k)->FeaturesOfCamera(c).size();
+  return count;
+}
+
+// tools/intersect_datasets.cc:41-261: of several dataset.bin files of one image sequence (e.g. one per feature
+// detector), keep only the features that all of them detected, and write each to <path>.intersected.bin. Imagesets are
+// matched by filename: dataset 0's imagesets are walked by index; a filename missing from another dataset is deleted
+// from every dataset that has it (the first imageset of a repeated filename, as unordered_map::insert keeps it) and the
+// walk steps back by one; a later duplicate in dataset 0 of a filename already deleted is itself deleted (the
+// reference walks it forever); otherwise dataset 0's imageset and dataset i's first imageset of that filename form a
+// task, and at the end every imageset of datasets 1.. whose filename dataset 0 no longer holds is deleted. The features
+// of every (task, camera) are intersected by `intersect` (the rules are in b200ba.h); tasks that share an imageset run
+// in separate calls in task order, so that a later task reads the features an earlier one thinned, as in the
+// reference. Messages go to stderr; the two pinned counts are printed where they are not zero. Returns EXIT_SUCCESS, or
+// EXIT_FAILURE for an empty path list or more than 32 paths (the device walk runs one warp per dataset in one CTA; the
+// reference has no such limit), a file that cannot be read or written, or datasets with different camera counts.
+// pipeline.py's IntersectDatasets prints and writes the same bytes.
+inline int IntersectDatasets(const std::vector<std::string>& dataset_paths, double intersection_threshold = 3.0,
+                             const IntersectLists& intersect = IntersectListsOnDevice) {
+  if (dataset_paths.empty()) {
+    std::cerr << "IntersectDatasets needs at least one dataset\n";
+    return EXIT_FAILURE;
+  }
+  if (dataset_paths.size() > 32) {
+    std::cerr << "IntersectDatasets takes at most 32 datasets, not " << dataset_paths.size() << "\n";
+    return EXIT_FAILURE;
+  }
+  const int n = static_cast<int>(dataset_paths.size());
+  std::vector<std::shared_ptr<Dataset>> datasets(n);
+  for (int i = 0; i < n; ++i) {
+    std::cerr << "Dataset " << i << ": " << dataset_paths[i] << "\n";
+    if (!LoadDataset(dataset_paths[i].c_str(), &datasets[i])) {
+      std::cerr << "Cannot read file: " << dataset_paths[i] << "\n";
+      return EXIT_FAILURE;
+    }
+    if (i > 0 && datasets[i]->num_cameras() != datasets[0]->num_cameras()) {
+      std::cerr << "Number of cameras in dataset " << dataset_paths[i]
+                << " does not match the number of cameras in dataset " << dataset_paths[0] << "\n";
+      return EXIT_FAILURE;
+    }
+  }
+  for (int i = 0; i < n; ++i)
+    std::cerr << "Input features in dataset " << i << ": " << IntersectFeatureCount(*datasets[i])
+              << " (#imagesets: " << datasets[i]->ImagesetCount() << ")\n";
+
+  std::vector<std::unordered_map<std::string, int>> maps(n);
+  for (int i = 0; i < n; ++i)
+    for (int k = 0; k < datasets[i]->ImagesetCount(); ++k)
+      maps[i].insert(std::make_pair(datasets[i]->GetImageset(k)->GetFilename(), k));
+  std::vector<std::vector<std::shared_ptr<Imageset>>> tasks;
+  for (int index = 0; index < datasets[0]->ImagesetCount();) {
+    std::vector<std::shared_ptr<Imageset>> task{datasets[0]->GetImageset(index)};
+    const std::string name = task[0]->GetFilename();
+    for (int i = 1; i < n; ++i) {
+      auto it = maps[i].find(name);
+      if (it == maps[i].end()) break;
+      task.push_back(datasets[i]->GetImageset(it->second));
+    }
+    if (static_cast<int>(task.size()) == n) {
+      tasks.push_back(task);
+      ++index;
+      continue;
+    }
+    for (int i = 0; i < n; ++i) {
+      auto it = maps[i].find(name);
+      int doomed;
+      if (it != maps[i].end()) {
+        doomed = it->second;
+        maps[i].erase(it);
+      } else if (i == 0) {
+        std::cerr << "Imageset " << name << " of dataset 0 deleted: its filename was deleted before\n";
+        doomed = index;
+      } else {
+        continue;
+      }
+      datasets[i]->DeleteImageset(doomed);
+      for (auto& item : maps[i])
+        if (item.second > doomed) --item.second;
+    }
+  }
+
+  // waves: a task runs after every earlier task that shares one of its imagesets
+  std::vector<std::vector<size_t>> waves;
+  std::unordered_map<const Imageset*, size_t> last_wave;
+  for (size_t t = 0; t < tasks.size(); ++t) {
+    size_t w = 0;
+    for (const auto& s : tasks[t]) {
+      auto it = last_wave.find(s.get());
+      if (it != last_wave.end()) w = std::max(w, it->second + 1);
+    }
+    for (const auto& s : tasks[t]) last_wave[s.get()] = w;
+    if (w == waves.size()) waves.emplace_back();
+    waves[w].push_back(t);
+  }
+  const int ncam = datasets[0]->num_cameras();
+  int64_t uncovered = 0, capped = 0;
+  for (const std::vector<size_t>& wave : waves) {
+    std::vector<int64_t> offsets{0};
+    std::vector<float> xy;
+    for (size_t t : wave)
+      for (int c = 0; c < ncam; ++c)
+        for (const auto& s : tasks[t]) {
+          for (const PointFeature& f : s->FeaturesOfCamera(c)) {
+            xy.push_back(f.xy.x);
+            xy.push_back(f.xy.y);
+          }
+          offsets.push_back(static_cast<int64_t>(xy.size() / 2));
+        }
+    if (xy.empty()) continue;
+    std::vector<uint8_t> keep;
+    b200ba_intersection_report report{};
+    intersect(n, offsets, xy, intersection_threshold, &keep, &report);
+    uncovered += report.uncovered;
+    capped += report.capped;
+    size_t k = 0;
+    for (size_t t : wave)
+      for (int c = 0; c < ncam; ++c)
+        for (const auto& s : tasks[t]) {
+          std::vector<PointFeature>& features = s->FeaturesOfCamera(c);
+          std::vector<PointFeature> kept;
+          for (size_t j = 0; j < features.size(); ++j)
+            if (keep[offsets[k] + j]) kept.push_back(features[j]);
+          features.swap(kept);
+          ++k;
+        }
+  }
+  if (uncovered) std::cerr << "Features rejected with nothing covered, left in place: " << uncovered << "\n";
+  if (capped) std::cerr << "Fixed-point loops stopped after 100 passes: " << capped << "\n";
+
+  for (int i = 1; i < n; ++i)
+    for (int k = 0; k < datasets[i]->ImagesetCount();) {
+      if (maps[0].count(datasets[i]->GetImageset(k)->GetFilename()) == 0)
+        datasets[i]->DeleteImageset(k);
+      else
+        ++k;
+    }
+  for (int i = 0; i < n; ++i) {
+    const std::string out = dataset_paths[i] + ".intersected.bin";
+    if (!SaveDataset(out.c_str(), *datasets[i])) {
+      std::cerr << "Cannot write file: " << out << "\n";
+      return EXIT_FAILURE;
+    }
+  }
+  for (int i = 0; i < n; ++i)
+    std::cerr << "Remaining features in dataset " << i << ": " << IntersectFeatureCount(*datasets[i]) << "\n";
   return EXIT_SUCCESS;
 }
 

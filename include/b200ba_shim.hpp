@@ -202,6 +202,7 @@ class Dataset {
     m_imagesets.emplace_back(new Imageset(m_num_cameras));
     return m_imagesets.back();
   }
+  void DeleteImageset(int i) { m_imagesets.erase(m_imagesets.begin() + i); }
   std::shared_ptr<Imageset> GetImageset(int i) { return m_imagesets[i]; }
   std::shared_ptr<const Imageset> GetImageset(int i) const { return m_imagesets[i]; }
   int ImagesetCount() const { return static_cast<int>(m_imagesets.size()); }

@@ -286,6 +286,69 @@ def IntersectFeatures(n_datasets: int, list_offsets, xy, threshold: float = 3.0,
     return keep.astype(bool), rep, ms.value
 
 
+def _pattern_struct(pattern) -> "cabi.Pattern":
+    if isinstance(pattern, cabi.Pattern):
+        return pattern
+    p = cabi.Pattern()
+    for key in ("squares_x", "squares_y", "num_star_segments"):
+        setattr(p, key, int(pattern[key]))
+    for key in ("page_width_mm", "page_height_mm", "pattern_start_x_mm", "pattern_start_y_mm", "pattern_end_x_mm",
+                "pattern_end_y_mm"):
+        setattr(p, key, float(np.float32(pattern[key])))
+    tags = list(pattern.get("tags", []))
+    if len(tags) > cabi.PATTERN_MAX_TAGS:
+        raise ValueError(f"a pattern holds at most {cabi.PATTERN_MAX_TAGS} AprilTags")
+    p.num_tags = len(tags)
+    for k, t in enumerate(tags):
+        p.tags[k] = cabi.PatternTag(int(t["x"]), int(t["y"]), int(t["width"]), int(t["height"]), int(t["index"]))
+    return p
+
+
+def _camera_floats(fx_fy_cx_cy):
+    k = np.ascontiguousarray(np.asarray(fx_fy_cx_cy, dtype=np.float32).reshape(-1))
+    if k.size != 4:
+        raise ValueError("fx_fy_cx_cy must hold fx fy cx cy")
+    return k
+
+
+def SyntheticPoses(pattern, pattern_size, image_size, fx_fy_cx_cy, n: int, seed: int = 0):
+    """The random poses of --render_synthetic_dataset (render_synthetic_dataset.cc:156-196) from the seeded stream
+    of ``b200ba_synthetic_poses`` (specified in include/b200ba.h): pattern is a dict of io.LoadPatternYAML (or a
+    cabi.Pattern), pattern_size = (w, h) of the pattern image, image_size = (w, h) of the pinhole camera. Returns
+    (camera_tr_global [n, 12] float64: R row-major, t; attempts [n] int64)."""
+    lib = cabi.load_library()
+    p = _pattern_struct(pattern)
+    k = _camera_floats(fx_fy_cx_cy)
+    poses = np.zeros((max(int(n), 0), 12))
+    attempts = np.zeros(max(int(n), 0), np.int64)
+    _check(lib.b200ba_synthetic_poses(C.byref(p), int(pattern_size[0]), int(pattern_size[1]), int(image_size[0]),
+                                      int(image_size[1]), k.ctypes.data_as(C.POINTER(C.c_float)), int(n),
+                                      int(seed) & 0xFFFFFFFFFFFFFFFF, _dp(poses),
+                                      attempts.ctypes.data_as(C.POINTER(C.c_int64))))
+    return poses, attempts
+
+
+def RenderPatternImages(pattern, pattern_image, image_size, fx_fy_cx_cy, camera_tr_global, device: int = -1):
+    """The images of --render_synthetic_dataset (render_synthetic_dataset.cc:198-291) on the device
+    (``b200ba_render_pattern_images``; the arithmetic is specified in include/b200ba.h): the star pattern with exact
+    per-pixel coverage, the pattern image (grey [h, w] uint8) outside the repeating area. camera_tr_global [n, 12]
+    as SyntheticPoses returns it. Returns (images [n, height, width] uint8, device_ms)."""
+    lib = cabi.load_library()
+    p = _pattern_struct(pattern)
+    k = _camera_floats(fx_fy_cx_cy)
+    pat = np.ascontiguousarray(pattern_image, dtype=np.uint8)
+    if pat.ndim != 2:
+        raise ValueError("RenderPatternImages: pattern_image must be a grey [h, w] uint8 image")
+    poses = np.ascontiguousarray(np.asarray(camera_tr_global, dtype=np.float64).reshape(-1, 12))
+    w, h = int(image_size[0]), int(image_size[1])
+    images = np.zeros((len(poses), max(h, 0), max(w, 0)), np.uint8)
+    ms = C.c_double(0)
+    _check(lib.b200ba_render_pattern_images(device, C.byref(p), _u8p(pat), pat.shape[1], pat.shape[0], w, h,
+                                            k.ctypes.data_as(C.POINTER(C.c_float)), len(poses), _dp(poses),
+                                            _u8p(images), C.byref(ms)))
+    return images, ms.value
+
+
 def nccl_unique_id() -> bytes:
     lib = cabi.load_library()
     buf = (C.c_uint8 * cabi.NCCL_UNIQUE_ID_BYTES)()

@@ -283,6 +283,32 @@ class IntersectionReport(C.Structure):
     ]
 
 
+PATTERN_MAX_TAGS = 16
+
+
+class PatternTag(C.Structure):
+    """b200ba_pattern_tag: tag_x, tag_y, width, height (squares) and index of one AprilTag."""
+    _fields_ = [("x", C.c_int32), ("y", C.c_int32), ("width", C.c_int32), ("height", C.c_int32),
+                ("index", C.c_int32)]
+
+
+class Pattern(C.Structure):
+    """b200ba_pattern: the numbers of a pattern YAML file (PatternData), at most PATTERN_MAX_TAGS tags."""
+    _fields_ = [
+        ("squares_x", C.c_int32),
+        ("squares_y", C.c_int32),
+        ("num_star_segments", C.c_int32),
+        ("num_tags", C.c_int32),
+        ("page_width_mm", C.c_float),
+        ("page_height_mm", C.c_float),
+        ("pattern_start_x_mm", C.c_float),
+        ("pattern_start_y_mm", C.c_float),
+        ("pattern_end_x_mm", C.c_float),
+        ("pattern_end_y_mm", C.c_float),
+        ("tags", PatternTag * PATTERN_MAX_TAGS),
+    ]
+
+
 class FitReport(C.Structure):
     """b200ba_fit_report."""
     _fields_ = [
@@ -479,6 +505,11 @@ SYMBOLS = {
     "b200ba_visualize_camera": (C.c_int, [C.c_int, C.c_int32, C.c_int32, _D, C.POINTER(C.c_uint8), _D, _D, _D]),
     "b200ba_intersect_features": (C.c_int, [C.c_int, C.c_int32, C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_float),
                                             C.c_double, C.POINTER(C.c_uint8), C.POINTER(IntersectionReport), _D]),
+    "b200ba_synthetic_poses": (C.c_int, [C.POINTER(Pattern), C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                         C.POINTER(C.c_float), C.c_int64, C.c_uint64, _D, C.POINTER(C.c_int64)]),
+    "b200ba_render_pattern_images": (C.c_int, [C.c_int, C.POINTER(Pattern), C.POINTER(C.c_uint8), C.c_int32,
+                                               C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_float), C.c_int64, _D,
+                                               C.POINTER(C.c_uint8), _D]),
     "b200ba_snapshot_state": (C.c_int, [C.c_void_p]),
     "b200ba_restore_state": (C.c_int, [C.c_void_p]),
     "b200ba_version": (C.c_char_p, []),

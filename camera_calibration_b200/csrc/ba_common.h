@@ -219,4 +219,13 @@ struct FixedRanges {
   }
 };
 
+// SplitMix64, the mixing function of the counter-based random streams of b200ba_localization_accuracy and
+// b200ba_synthetic_poses (include/b200ba.h)
+__host__ __device__ __forceinline__ uint64_t loc_splitmix64(uint64_t z) {
+  z += 0x9E3779B97F4A7C15ull;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+
 }  // namespace b200ba

@@ -3367,6 +3367,312 @@ int b200ba_intersect_features(int device, int32_t n_datasets, int64_t n_lists, c
   return cs.rc;
 }
 
+// ---- synthetic pattern images (--render_synthetic_dataset; the arithmetic is specified in include/b200ba.h) ----
+namespace {
+bool synth_valid_pattern_coord(const b200ba_pattern& p, float x, float y) {  // PatternData::IsValidPatternCoord
+  if (!(x >= -1.f && y >= -1.f && x <= p.squares_x - 1.f && y <= p.squares_y - 1.f)) return false;
+  for (int k = 0; k < p.num_tags; ++k) {
+    const b200ba_pattern_tag& t = p.tags[k];
+    if (x >= t.x - 1 && y >= t.y - 1 && x <= t.x - 1 + t.width && y <= t.y - 1 + t.height) return false;
+  }
+  return true;
+}
+
+// PatternData::GetStarCoord with square_length 1: float angle and float sin / cos, the offset in double
+float2 synth_star_coord(int num_star_segments, float i, float center_x, float center_y) {
+  const float angle = ((2 * M_PI) * i) / num_star_segments;
+  float x = std::sin(angle), y = std::cos(angle);
+  const float max_abs_x = std::max(std::fabs(x), std::fabs(y));
+  x /= max_abs_x;
+  y /= max_abs_x;
+  return make_float2(static_cast<float>(center_x - 0.5 * x), static_cast<float>(center_y - 0.5 * y));
+}
+
+// pattern_to_pattern_image_coord of render_synthetic_dataset.cc:79-87, in float
+float2 synth_pattern_to_image(const b200ba_pattern& p, int32_t pattern_w, int32_t pattern_h, float cx, float cy) {
+  const float mx = p.pattern_start_x_mm + ((cx + 1.f) / static_cast<float>(p.squares_x)) *
+                                              (p.pattern_end_x_mm - p.pattern_start_x_mm);
+  const float my = p.pattern_start_y_mm + ((cy + 1.f) / static_cast<float>(p.squares_y)) *
+                                              (p.pattern_end_y_mm - p.pattern_start_y_mm);
+  return make_float2((static_cast<float>(pattern_w) / p.page_width_mm) * mx,
+                     (static_cast<float>(pattern_h) / p.page_height_mm) * my);
+}
+
+// PatternData::ComputePatternGeometry (without AprilTags) in generation order, mapped to pattern-image pixels
+void synth_geometry(const b200ba_pattern& p, int32_t pattern_w, int32_t pattern_h, std::vector<float2>* verts,
+                    std::vector<int8_t>* nv) {
+  const int n = p.num_star_segments;
+  for (int y = -1; y < p.squares_y; ++y) {
+    for (int x = -1; x < p.squares_x; ++x) {
+      bool in_tag = false;
+      for (int k = 0; k < p.num_tags && !in_tag; ++k) {
+        const b200ba_pattern_tag& t = p.tags[k];
+        in_tag = x >= t.x && y >= t.y && x <= t.x - 2 + t.width && y <= t.y - 2 + t.height;
+      }
+      if (in_tag) continue;
+      for (int segment = 0; segment < n; segment += 2) {
+        const float2 middle = synth_star_coord(n, segment + 0.5f, x, y);
+        if (!synth_valid_pattern_coord(p, middle.x, middle.y)) continue;
+        float2 poly[kSynthMaxVerts];
+        int c = 0;
+        poly[c++] = make_float2(x, y);
+        poly[c++] = synth_star_coord(n, segment, x, y);
+        const float angle1 = (2 * M_PI) * (segment) / n;
+        const float angle2 = (2 * M_PI) * (segment + 1) / n;
+        if (std::floor((angle1 - M_PI / 4) / (M_PI / 2)) != std::floor((angle2 - M_PI / 4) / (M_PI / 2))) {
+          const float corner_angle = (M_PI / 4) + (M_PI / 2) * std::floor((angle2 - M_PI / 4) / (M_PI / 2));
+          float corner_x = std::sin(corner_angle), corner_y = std::cos(corner_angle);
+          const float normalizer = std::fabs(corner_x);
+          corner_x /= normalizer;
+          corner_y /= normalizer;
+          poly[c++] = make_float2(static_cast<float>(x - 0.5 * corner_x), static_cast<float>(y - 0.5 * corner_y));
+        }
+        poly[c++] = synth_star_coord(n, segment + 1, x, y);
+        for (int v = 0; v < kSynthMaxVerts; ++v)
+          verts->push_back(v < c ? synth_pattern_to_image(p, pattern_w, pattern_h, poly[v].x, poly[v].y)
+                                 : make_float2(0.f, 0.f));
+        nv->push_back(static_cast<int8_t>(c));
+      }
+    }
+  }
+}
+
+// Eigen's Quaternion::toRotationMatrix, row-major
+void synth_rotation(double w, double x, double y, double z, double* R) {
+  const double tx = 2 * x, ty = 2 * y, tz = 2 * z;
+  const double twx = tx * w, twy = ty * w, twz = tz * w;
+  const double txx = tx * x, txy = ty * x, txz = tz * x;
+  const double tyy = ty * y, tyz = tz * y, tzz = tz * z;
+  R[0] = 1 - (tyy + tzz), R[1] = txy - twz, R[2] = txz + twy;
+  R[3] = txy + twz, R[4] = 1 - (txx + tzz), R[5] = tyz - twx;
+  R[6] = txz - twy, R[7] = tyz + twx, R[8] = 1 - (txx + tyy);
+}
+
+void synth_cross(const double* a, const double* b, double* r) {
+  r[0] = a[1] * b[2] - a[2] * b[1];
+  r[1] = a[2] * b[0] - a[0] * b[2];
+  r[2] = a[0] * b[1] - a[1] * b[0];
+}
+
+// attempt a of image i: exp(tangent) * (I, t0) as Sophus composes it; pose = [R row-major, t]
+void synth_pose_attempt(uint64_t seed_hash, int64_t i, int a, int32_t pattern_w, int32_t pattern_h, double* pose) {
+  uint64_t h[9];
+  for (int c = 0; c < 9; ++c)
+    h[c] = loc_splitmix64(seed_hash ^ ((static_cast<uint64_t>(i) << 24) | (static_cast<uint64_t>(a) << 4) | c));
+  float f[3];
+  for (int c = 0; c < 3; ++c) f[c] = static_cast<float>(h[c] % 10000) / 10000.f;
+  const double t0[3] = {0.0 - static_cast<double>((-1.f + 2.f * f[0]) * static_cast<float>(pattern_w)),
+                        0.0 - static_cast<double>((-1.f + 2.f * f[1]) * static_cast<float>(pattern_h)),
+                        0.0 + static_cast<double>(500.f + 800.f * f[2])};
+  double tan[6];
+  for (int c = 0; c < 6; ++c) tan[c] = 0.5 * (-1.0 + 2.0 * (static_cast<double>(h[3 + c] >> 11) * 0x1p-53));
+  const double* u = tan;
+  const double* w = tan + 3;
+  const double th2 = (w[0] * w[0] + w[1] * w[1]) + w[2] * w[2];
+  const double th = std::sqrt(th2);
+  const double half = 0.5 * th;
+  double im, re;
+  if (th < 1e-10) {
+    const double th4 = th2 * th2;
+    im = (0.5 - (1.0 / 48.0) * th2) + (1.0 / 3840.0) * th4;
+    re = (1.0 - 0.5 * th2) + (1.0 / 384.0) * th4;
+  } else {
+    im = std::sin(half) / th;
+    re = std::cos(half);
+  }
+  const double qv[3] = {im * w[0], im * w[1], im * w[2]};
+  const double qw = re;
+  double V[9];
+  if (th < 1e-10) {
+    synth_rotation(qw, qv[0], qv[1], qv[2], V);
+  } else {
+    const double W[9] = {0, -w[2], w[1], w[2], 0, -w[0], -w[1], w[0], 0};
+    double W2[9];
+    for (int r = 0; r < 3; ++r)
+      for (int c = 0; c < 3; ++c) W2[r * 3 + c] = (W[r * 3] * W[c] + W[r * 3 + 1] * W[3 + c]) + W[r * 3 + 2] * W[6 + c];
+    const double c1 = (1.0 - std::cos(th)) / th2, c2 = (th - std::sin(th)) / (th2 * th);
+    for (int k = 0; k < 9; ++k) V[k] = ((k % 4 == 0 ? 1.0 : 0.0) + c1 * W[k]) + c2 * W2[k];
+  }
+  double t[3];
+  for (int r = 0; r < 3; ++r) t[r] = (V[r * 3] * u[0] + V[r * 3 + 1] * u[1]) + V[r * 3 + 2] * u[2];
+  double uv[3], uv2[3];
+  synth_cross(qv, t0, uv);
+  for (double& e : uv) e = e + e;
+  synth_cross(qv, uv, uv2);
+  for (int r = 0; r < 3; ++r) t[r] = t[r] + ((t0[r] + qw * uv[r]) + uv2[r]);
+  double q[4] = {qv[0], qv[1], qv[2], qw};  // Eigen's coefficient order x, y, z, w
+  const double s = (q[0] * q[0] + q[2] * q[2]) + (q[1] * q[1] + q[3] * q[3]);
+  if (s != 1.0)
+    for (double& e : q) e *= 2.0 / (1.0 + s);
+  synth_rotation(q[3], q[0], q[1], q[2], pose);
+  for (int r = 0; r < 3; ++r) pose[9 + r] = t[r];
+}
+
+// PinholeCamera4f::ProjectToPixelCornerConvIfVisible(p, 0) of the float pose
+bool synth_visible(const float* Rf, const float* tf, const float* k, int32_t width, int32_t height, float x, float y) {
+  float p[3];
+  for (int r = 0; r < 3; ++r) p[r] = (((Rf[r * 3] * x) + (Rf[r * 3 + 1] * y)) + (Rf[r * 3 + 2] * 0.f)) + tf[r];
+  if (p[2] <= 0.f) return false;
+  const float u = k[0] * (p[0] / p[2]) + k[2], v = k[1] * (p[1] / p[2]) + k[3];
+  return u >= 0.f && v >= 0.f && u < static_cast<float>(width) - 0.f && v < static_cast<float>(height) - 0.f;
+}
+
+// the float pose (Rf, tf) and the float inverse (Rc, tc) of one double pose
+void synth_float_pose(const double* pose, float* out) {
+  const double* R = pose;
+  const double* t = pose + 9;
+  for (int k = 0; k < 12; ++k) out[k] = static_cast<float>(pose[k]);
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c) out[12 + r * 3 + c] = static_cast<float>(R[c * 3 + r]);
+  for (int r = 0; r < 3; ++r) out[21 + r] = static_cast<float>((R[r] * -t[0] + R[3 + r] * -t[1]) + R[6 + r] * -t[2]);
+}
+
+const char* synth_check_pattern(const b200ba_pattern* p, int32_t pattern_w, int32_t pattern_h, int32_t width,
+                                int32_t height, const float* k) {
+  if (!p || !k) return "pattern and fx_fy_cx_cy are required";
+  if (pattern_w < 1 || pattern_h < 1 || width < 1 || height < 1 || pattern_w > 32768 || pattern_h > 32768 ||
+      width > 32768 || height > 32768)
+    return "sizes must lie in [1, 32768]";
+  if (p->num_tags < 0 || p->num_tags > B200BA_PATTERN_MAX_TAGS) return "num_tags must lie in [0, B200BA_PATTERN_MAX_TAGS]";
+  if (p->squares_x < 1 || p->squares_y < 1) return "squares_x and squares_y must be at least 1";
+  if (p->num_star_segments < 2 || p->num_star_segments % 2 || p->num_star_segments > 1024)
+    return "num_star_segments must be even and in [2, 1024]";
+  if (int64_t(p->squares_x + 1) * (p->squares_y + 1) * (p->num_star_segments / 2) > (int64_t(1) << 24))
+    return "the pattern has more than 2^24 star segments";
+  if (!std::isfinite(k[0]) || !std::isfinite(k[1]) || k[0] == 0.f || k[1] == 0.f || !std::isfinite(k[2]) ||
+      !std::isfinite(k[3]))
+    return "fx and fy must be finite and non-zero, cx and cy finite";
+  return nullptr;
+}
+}  // namespace
+
+int b200ba_synthetic_poses(const b200ba_pattern* pattern, int32_t pattern_w, int32_t pattern_h, int32_t width,
+                           int32_t height, const float* fx_fy_cx_cy, int64_t n, uint64_t seed,
+                           double* camera_tr_global, int64_t* attempts) {
+  if (const char* e = synth_check_pattern(pattern, pattern_w, pattern_h, width, height, fx_fy_cx_cy)) {
+    g_create_error = std::string("b200ba_synthetic_poses: ") + e;
+    return 2;
+  }
+  if (n < 1 || n >= (int64_t(1) << 40) || !camera_tr_global) {
+    g_create_error = "b200ba_synthetic_poses: needs 1 <= n < 2^40 and camera_tr_global";
+    return 2;
+  }
+  const b200ba_pattern& p = *pattern;
+  std::vector<float2> lo(p.num_tags), hi(p.num_tags);
+  for (int k = 0; k < p.num_tags; ++k) {
+    const b200ba_pattern_tag& t = p.tags[k];
+    lo[k] = synth_pattern_to_image(p, pattern_w, pattern_h, t.x - 1, t.y - 1);
+    hi[k] = synth_pattern_to_image(p, pattern_w, pattern_h, t.x - 1 + t.width, t.y - 1 + t.height);
+  }
+  const uint64_t seed_hash = loc_splitmix64(seed);
+  for (int64_t i = 0; i < n; ++i) {
+    double* pose = camera_tr_global + 12 * i;
+    bool visible = false;
+    int a = 0;
+    for (; a < 4096 && !visible; ++a) {
+      synth_pose_attempt(seed_hash, i, a, pattern_w, pattern_h, pose);
+      float f[24];
+      synth_float_pose(pose, f);
+      for (int k = 0; k < p.num_tags && !visible; ++k)
+        visible = synth_visible(f, f + 9, fx_fy_cx_cy, width, height, lo[k].x, lo[k].y) &&
+                  synth_visible(f, f + 9, fx_fy_cx_cy, width, height, hi[k].x, lo[k].y) &&
+                  synth_visible(f, f + 9, fx_fy_cx_cy, width, height, lo[k].x, hi[k].y) &&
+                  synth_visible(f, f + 9, fx_fy_cx_cy, width, height, hi[k].x, hi[k].y);
+    }
+    if (attempts) attempts[i] = a;
+    if (!visible) {
+      g_create_error = "b200ba_synthetic_poses: no tag is visible after 4096 attempts";
+      return 4;
+    }
+  }
+  return 0;
+}
+
+int b200ba_render_pattern_images(int device, const b200ba_pattern* pattern, const uint8_t* pattern_image,
+                                 int32_t pattern_w, int32_t pattern_h, int32_t width, int32_t height,
+                                 const float* fx_fy_cx_cy, int64_t n, const double* camera_tr_global, uint8_t* images,
+                                 double* device_ms) {
+  if (const char* e = synth_check_pattern(pattern, pattern_w, pattern_h, width, height, fx_fy_cx_cy)) {
+    g_create_error = std::string("b200ba_render_pattern_images: ") + e;
+    return 2;
+  }
+  if (n < 0 || !pattern_image || (n > 0 && (!camera_tr_global || !images))) {
+    g_create_error = "b200ba_render_pattern_images: needs n >= 0, pattern_image, camera_tr_global and images";
+    return 2;
+  }
+  const b200ba_pattern& pat = *pattern;
+  std::vector<float2> verts;
+  std::vector<int8_t> nv;
+  synth_geometry(pat, pattern_w, pattern_h, &verts, &nv);
+  SynthParams sp{};
+  sp.w = width;
+  sp.h = height;
+  sp.tiles_x = (width + kSynthTile - 1) / kSynthTile;
+  sp.tiles_y = (height + kSynthTile - 1) / kSynthTile;
+  sp.n_poly = static_cast<int>(nv.size());
+  sp.words = std::max(1, (sp.n_poly + 31) / 32);
+  sp.fx = fx_fy_cx_cy[0], sp.fy = fx_fy_cx_cy[1], sp.cx = fx_fy_cx_cy[2], sp.cy = fx_fy_cx_cy[3];
+  sp.pattern_w = pattern_w, sp.pattern_h = pattern_h, sp.squares_x = pat.squares_x, sp.squares_y = pat.squares_y;
+  sp.num_tags = pat.num_tags;
+  sp.page_w = pat.page_width_mm, sp.page_h = pat.page_height_mm;
+  sp.start_x = pat.pattern_start_x_mm, sp.start_y = pat.pattern_start_y_mm;
+  sp.end_x = pat.pattern_end_x_mm, sp.end_y = pat.pattern_end_y_mm;
+  for (int k = 0; k < pat.num_tags; ++k)
+    sp.tags[k] = make_int4(pat.tags[k].x, pat.tags[k].y, pat.tags[k].width, pat.tags[k].height);
+  // images per chunk: device memory bounded by about 512 MiB (B200BA_SYNTH_CHUNK caps the count)
+  const int64_t pixels = static_cast<int64_t>(width) * height;
+  const int64_t per_image = static_cast<int64_t>(sp.tiles_x) * sp.tiles_y * sp.words * 4 +
+                            static_cast<int64_t>(sp.n_poly) * (kSynthMaxVerts * 16 + 16) + pixels + 96;
+  int64_t chunk = std::max<int64_t>(1, (int64_t(512) << 20) / per_image);
+  if (const char* e = getenv("B200BA_SYNTH_CHUNK")) chunk = std::max<int64_t>(1, std::min<int64_t>(chunk, atoll(e)));
+  chunk = std::min<int64_t>(chunk, std::max<int64_t>(n, 1));
+  chunk = std::min<int64_t>(chunk, 65535);
+  CallScope cs(&g_create_error);
+  if (int rc = cs.use_device(device)) return rc;
+  if (n == 0) {
+    if (device_ms) *device_ms = 0.0;
+    return 0;
+  }
+  std::vector<float> poses(24 * n);
+  for (int64_t i = 0; i < n; ++i) synth_float_pose(camera_tr_global + 12 * i, poses.data() + 24 * i);
+  float2* d_verts = nullptr;
+  int8_t* d_nv = nullptr;
+  float* d_poses = nullptr;
+  uint8_t* d_pattern = nullptr;
+  double2* d_proj = nullptr;
+  int4* d_range = nullptr;
+  uint32_t* d_bits = nullptr;
+  uint8_t* d_img = nullptr;
+  const size_t bits_per_image = static_cast<size_t>(sp.tiles_x) * sp.tiles_y * sp.words;
+  cs.alloc(&d_verts, std::max<size_t>(1, verts.size()));
+  cs.alloc(&d_nv, std::max<size_t>(1, nv.size()));
+  cs.alloc(&d_poses, poses.size());
+  cs.alloc(&d_pattern, static_cast<size_t>(pattern_w) * pattern_h);
+  cs.alloc(&d_proj, std::max<size_t>(1, static_cast<size_t>(chunk) * sp.n_poly * kSynthMaxVerts));
+  cs.alloc(&d_range, std::max<size_t>(1, static_cast<size_t>(chunk) * sp.n_poly));
+  cs.alloc(&d_bits, static_cast<size_t>(chunk) * bits_per_image);
+  cs.alloc(&d_img, static_cast<size_t>(chunk) * pixels);
+  if (cs.rc == 0 && !verts.empty())
+    cs.ok(cudaMemcpy(d_verts, verts.data(), sizeof(float2) * verts.size(), cudaMemcpyHostToDevice));
+  if (cs.rc == 0 && !nv.empty()) cs.ok(cudaMemcpy(d_nv, nv.data(), nv.size(), cudaMemcpyHostToDevice));
+  if (cs.rc == 0) cs.ok(cudaMemcpy(d_poses, poses.data(), sizeof(float) * poses.size(), cudaMemcpyHostToDevice));
+  if (cs.rc == 0)
+    cs.ok(cudaMemcpy(d_pattern, pattern_image, static_cast<size_t>(pattern_w) * pattern_h, cudaMemcpyHostToDevice));
+  double ms = 0.0;
+  for (int64_t i0 = 0; i0 < n && cs.rc == 0; i0 += chunk) {
+    const int m = static_cast<int>(std::min<int64_t>(chunk, n - i0));
+    cs.record(0, 0);
+    cs.ok(cudaMemsetAsync(d_bits, 0, sizeof(uint32_t) * bits_per_image * m, 0));
+    launch_render_pattern(sp, m, d_verts, d_nv, d_poses + 24 * i0, d_pattern, d_proj, d_range, d_bits, d_img, 0);
+    cs.record(1, 0);
+    cs.ok(cudaGetLastError());
+    cs.ok(cudaMemcpy(images + i0 * pixels, d_img, static_cast<size_t>(m) * pixels, cudaMemcpyDeviceToHost));
+    if (cs.rc == 0) ms += cs.elapsed_ms(0, 1);
+  }
+  if (cs.rc == 0 && device_ms) *device_ms = ms;
+  return cs.rc;
+}
+
 // Eigen::LDLT<MatrixXd, Lower>(A.selfadjointView<Upper>()).solve(b) for n = 3 (SolveDensely, LV/lm_optimizer.h:1022-1023):
 // symmetric pivoting on the largest remaining |diagonal| entry as Eigen's left-looking factorisation sees it (the
 // ORIGINAL values of the trailing diagonal), then x = P^T L^-T D^-1 L^-1 P b with 1 / d_i taken as 0 where

@@ -2271,12 +2271,6 @@ void launch_compare_models(const CamDev& a, const double* ga, const CamDev& b, c
 // trial, then one pose fit per trial (opengv's absolute_pose::optimize_nonlinear cost; the iteration and the random
 // stream are specified in include/b200ba.h)
 // ------------------------------------------------------------------------------------------
-__host__ __device__ __forceinline__ uint64_t loc_splitmix64(uint64_t z) {
-  z += 0x9E3779B97F4A7C15ull;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  return z ^ (z >> 31);
-}
 // (float)(h >> 40) * 2^-24f * extent: the first product is exact, the second rounds once
 __device__ __forceinline__ float loc_coordinate(uint64_t h, float extent) {
   return __fmul_rn(static_cast<float>(h >> 40) * 0x1p-24f, extent);
@@ -4150,6 +4144,229 @@ void launch_intersect_features(int d, int64_t n_lists, int64_t max_list, const i
   intersect_walk_kernel<<<static_cast<unsigned>(n_lists), 32 * d, use_smem ? bytes : 0, s>>>(
       d, off, xy, use_smem ? 1 : 0, bound, keep, centres, n_centres, counts);
   intersect_keep_kernel<<<static_cast<unsigned>(n_lists), 256, 0, s>>>(d, off, xy, bound, centres, n_centres, keep);
+}
+
+// ------------------------------------------------------------------------------------------
+// synthetic pattern images (tools/render_synthetic_dataset.cc:202-291; the arithmetic is specified in
+// include/b200ba.h). Every float and double operation that feeds a pixel is an explicit _rn intrinsic, so nvcc
+// cannot contract it into a fused multiply-add; the library's global flags stay as they are.
+// ------------------------------------------------------------------------------------------
+// the float pose of one image: Rf (9, row-major), tf (3), then the inverse Rc (9), tc (3)
+constexpr int kSynthPoseFloats = 24;
+constexpr int kSynthClipCap = 20;  // Sutherland-Hodgman output of a 4-gon against 4 edges: at most 6, 9, 13, 19
+
+// p_cam_i = ((R_i0 x + R_i1 y) + R_i2 z) + t_i (Eigen's 3 x 3 lazy product, then the translation)
+__device__ __forceinline__ float synth_row(const float* r, float x, float y, float z) {
+  return __fadd_rn(__fadd_rn(__fmul_rn(r[0], x), __fmul_rn(r[1], y)), __fmul_rn(r[2], z));
+}
+
+// the pixel range of one polygon, converted to int as x86-64 does (report_trunc) and clamped to the image
+__device__ __forceinline__ int synth_lo(double v) { return max(0, report_trunc(v)); }
+__device__ __forceinline__ int synth_hi(double v, int extent) { return min(extent - 1, report_trunc(v)); }
+
+// One thread per (image, polygon): projects the vertices, stores the reference's clamped integer pixel range
+// (x0, x1, y0, y1; empty when x0 > x1 or y0 > y1) and marks the polygon in the bitmap of every tile the range
+// touches. Bit k of a tile's bitmap is polygon k, so a tile's polygons come out in generation order.
+__global__ void synth_project_kernel(SynthParams p, int n_img, const float2* __restrict__ verts,
+                                     const int8_t* __restrict__ nv, const float* __restrict__ poses,
+                                     double2* __restrict__ proj, int4* __restrict__ range, uint32_t* bits) {
+  const int64_t k = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (k >= static_cast<int64_t>(n_img) * p.n_poly) return;
+  const int img = static_cast<int>(k / p.n_poly), poly = static_cast<int>(k % p.n_poly);
+  const float* R = poses + static_cast<int64_t>(img) * kSynthPoseFloats;
+  const float* t = R + 9;
+  const int n = nv[poly];
+  double min_x = 1.7976931348623157e308, min_y = 1.7976931348623157e308;
+  double max_x = -1.7976931348623157e308, max_y = -1.7976931348623157e308;
+  bool nan = false;
+  for (int v = 0; v < n; ++v) {
+    const float2 q = verts[poly * kSynthMaxVerts + v];
+    const float X = __fadd_rn(synth_row(R, q.x, q.y, 0.f), t[0]);
+    const float Y = __fadd_rn(synth_row(R + 3, q.x, q.y, 0.f), t[1]);
+    const float Z = __fadd_rn(synth_row(R + 6, q.x, q.y, 0.f), t[2]);
+    const double u = __fadd_rn(__fmul_rn(p.fx, __fdiv_rn(X, Z)), p.cx);
+    const double w = __fadd_rn(__fmul_rn(p.fy, __fdiv_rn(Y, Z)), p.cy);
+    proj[k * kSynthMaxVerts + v] = make_double2(u, w);
+    nan |= u != u || w != w;
+    min_x = u < min_x ? u : min_x;
+    max_x = u > max_x ? u : max_x;
+    min_y = w < min_y ? w : min_y;
+    max_y = w > max_y ? w : max_y;
+  }
+  int4 r = make_int4(1, 0, 1, 0);  // empty
+  if (!nan) r = make_int4(synth_lo(min_x), synth_hi(max_x, p.w), synth_lo(min_y), synth_hi(max_y, p.h));
+  range[k] = r;
+  if (r.x > r.y || r.z > r.w) return;
+  uint32_t* b = bits + static_cast<int64_t>(img) * p.tiles_y * p.tiles_x * p.words + (poly >> 5);
+  const uint32_t bit = 1u << (poly & 31);
+  for (int ty = r.z / kSynthTile; ty <= r.w / kSynthTile; ++ty)
+    for (int tx = r.x / kSynthTile; tx <= r.y / kSynthTile; ++tx)
+      atomicOr(b + (static_cast<int64_t>(ty) * p.tiles_x + tx) * p.words, bit);
+}
+
+// libvis' LineLineIntersection (geometry.h:49-79) of the lines a0-a1 and b0-b1; *r is left alone only when the
+// denominator is 0 (a non-finite quotient is stored before it is rejected)
+__device__ __forceinline__ void synth_intersect(double2 a0, double2 a1, double2 b0, double2 b1, double2* r) {
+  const double detL1 = __dsub_rn(__dmul_rn(a0.x, a1.y), __dmul_rn(a0.y, a1.x));
+  const double detL2 = __dsub_rn(__dmul_rn(b0.x, b1.y), __dmul_rn(b0.y, b1.x));
+  const double x1mx2 = __dsub_rn(a0.x, a1.x), x3mx4 = __dsub_rn(b0.x, b1.x);
+  const double y1my2 = __dsub_rn(a0.y, a1.y), y3my4 = __dsub_rn(b0.y, b1.y);
+  const double xnom = __dsub_rn(__dmul_rn(detL1, x3mx4), __dmul_rn(x1mx2, detL2));
+  const double ynom = __dsub_rn(__dmul_rn(detL1, y3my4), __dmul_rn(y1my2, detL2));
+  const double denom = __dsub_rn(__dmul_rn(x1mx2, y3my4), __dmul_rn(y1my2, x3mx4));
+  if (denom == 0) return;
+  r->x = __ddiv_rn(xnom, denom);
+  r->y = __ddiv_rn(ynom, denom);
+}
+
+__device__ __forceinline__ double synth_dot(double2 a, double2 b) {
+  return __dadd_rn(__dmul_rn(a.x, b.x), __dmul_rn(a.y, b.y));
+}
+
+// PolygonArea(ConvexClipPolygon(polygon, pixel square (x, y))) (geometry.h:147-207), in double with the float edge
+// offset and the float orientation determinant of the reference
+__device__ double synth_clip_area(const double2* __restrict__ poly, int n, int px, int py) {
+  const double x = px, y = py;
+  const double2 clip[4] = {make_double2(x, y), make_double2(__dadd_rn(x, 1.0), y),
+                           make_double2(__dadd_rn(x, 1.0), __dadd_rn(y, 1.0)), make_double2(x, __dadd_rn(y, 1.0))};
+  const float det = static_cast<float>(
+      __dsub_rn(__dmul_rn(__dsub_rn(clip[1].x, clip[0].x), __dsub_rn(clip[2].y, clip[0].y)),
+                __dmul_rn(__dsub_rn(clip[2].x, clip[0].x), __dsub_rn(clip[1].y, clip[0].y))));
+  const int orientation = det > 0 ? 1 : -1;
+  double2 buf[2][kSynthClipCap];
+  const double2* in = poly;
+  int n_in = n;
+  for (int e = 0; e < 4; ++e) {
+    const double2 s = clip[e], t = clip[(e + 1) & 3];
+    const double2 right = make_double2(__dsub_rn(t.y, s.y), -__dsub_rn(t.x, s.x));
+    const float edge_right = static_cast<float>(synth_dot(right, t));
+    double2* out = buf[e & 1];
+    int n_out = 0;
+    for (int i = 0; i < n_in; ++i) {
+      const double2 cur = in[i], prev = in[(i + n_in - 1) % n_in];
+      const bool cur_in = orientation * (synth_dot(right, cur) > edge_right ? 1 : -1) < 0;
+      if (cur_in) {
+        if (orientation * (synth_dot(right, prev) > edge_right ? 1 : -1) > 0) {
+          double2 r = prev;
+          synth_intersect(prev, cur, t, s, &r);
+          out[n_out++] = r;
+        }
+        out[n_out++] = cur;
+      } else if (orientation * (synth_dot(right, prev) > edge_right ? 1 : -1) < 0) {
+        double2 r = prev;
+        synth_intersect(prev, cur, t, s, &r);
+        out[n_out++] = r;
+      }
+    }
+    in = out;
+    n_in = n_out;
+  }
+  double sum = 0;
+  for (int i = 0, j = n_in - 1; i < n_in; j = i++)
+    sum = __dadd_rn(sum, __dmul_rn(__dsub_rn(in[i].x, in[j].x), __dadd_rn(in[i].y, in[j].y)));
+  return fabs(__dmul_rn(0.5, sum));
+}
+
+// float -> u8 as x86-64 executes it: cvttss2si (truncation, INT_MIN outside the int range and for NaN), low byte
+__device__ __forceinline__ uint8_t synth_u8(float v) {
+  return static_cast<uint8_t>((v > -2147483649.f && v < 2147483648.f) ? static_cast<int>(v) : INT_MIN);
+}
+
+// One thread per pixel of a kSynthTile x kSynthTile tile: walks the tile's bitmap in polygon order, subtracts the
+// clipped area of every polygon whose range holds the pixel, then composes the byte from the pixel's ray.
+__global__ void __launch_bounds__(kSynthTile * kSynthTile, 3)
+synth_render_kernel(SynthParams p, const float* __restrict__ poses, const int8_t* __restrict__ nv,
+                    const double2* __restrict__ proj, const int4* __restrict__ range,
+                    const uint32_t* __restrict__ bits, const uint8_t* __restrict__ pattern, uint8_t* images) {
+  const int img = blockIdx.z;
+  const int x = blockIdx.x * kSynthTile + threadIdx.x, y = blockIdx.y * kSynthTile + threadIdx.y;
+  if (x >= p.w || y >= p.h) return;
+  const uint32_t* b =
+      bits + ((static_cast<int64_t>(img) * p.tiles_y + blockIdx.y) * p.tiles_x + blockIdx.x) * p.words;
+  const int64_t pbase = static_cast<int64_t>(img) * p.n_poly;
+  float rendering = 1.f;
+  for (int wi = 0; wi < p.words; ++wi) {
+    uint32_t m = b[wi];
+    while (m) {
+      const int poly = wi * 32 + __ffs(m) - 1;
+      m &= m - 1;
+      const int4 r = range[pbase + poly];
+      if (x < r.x || x > r.y || y < r.z || y > r.w) continue;
+      const double a = synth_clip_area(proj + (pbase + poly) * kSynthMaxVerts, nv[poly], x, y);
+      rendering = __double2float_rn(__dsub_rn(static_cast<double>(rendering), a));
+    }
+  }
+  // the ray of the pixel centre (UnprojectFromPixelCornerConv, then the inverse pose) meets the plane z = 0
+  const float* Rc = poses + static_cast<int64_t>(img) * kSynthPoseFloats + 12;
+  const float* tc = Rc + 9;
+  const float lx = __fadd_rn(__fmul_rn(__fdiv_rn(1.f, p.fx), __fadd_rn(static_cast<float>(x), 0.5f)),
+                             __fdiv_rn(-p.cx, p.fx));
+  const float ly = __fadd_rn(__fmul_rn(__fdiv_rn(1.f, p.fy), __fadd_rn(static_cast<float>(y), 0.5f)),
+                             __fdiv_rn(-p.cy, p.fy));
+  float dx = synth_row(Rc, lx, ly, 1.f), dy = synth_row(Rc + 3, lx, ly, 1.f), dz = synth_row(Rc + 6, lx, ly, 1.f);
+  const float n2 = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
+  if (n2 > 0.f) {
+    const float s = __fsqrt_rn(n2);
+    dx = __fdiv_rn(dx, s);
+    dy = __fdiv_rn(dy, s);
+    dz = __fdiv_rn(dz, s);
+  }
+  const float offset = -0.f;
+  const float num = __fadd_rn(offset, __fadd_rn(__fadd_rn(__fmul_rn(0.f, tc[0]), __fmul_rn(0.f, tc[1])),
+                                                __fmul_rn(-1.f, tc[2])));
+  const float den = __fadd_rn(__fadd_rn(__fmul_rn(0.f, dx), __fmul_rn(0.f, dy)), __fmul_rn(-1.f, dz));
+  const float tt = __fdiv_rn(-num, den);
+  const float X = __fadd_rn(tc[0], __fmul_rn(dx, tt)), Y = __fadd_rn(tc[1], __fmul_rn(dy, tt));
+  const float lx2 = __fsub_rn(X, 0.f), ly2 = __fsub_rn(Y, -0.f);
+  const float ix = __fadd_rn(__fmul_rn(1.f, lx2), __fmul_rn(0.f, ly2));
+  const float iy = __fadd_rn(__fmul_rn(0.f, lx2), __fmul_rn(1.f, ly2));
+  const float mx = __fmul_rn(__fdiv_rn(p.page_w, static_cast<float>(p.pattern_w)), ix);
+  const float my = __fmul_rn(__fdiv_rn(p.page_h, static_cast<float>(p.pattern_h)), iy);
+  const float cx = __fsub_rn(__fmul_rn(__fdiv_rn(__fsub_rn(mx, p.start_x), __fsub_rn(p.end_x, p.start_x)),
+                                       static_cast<float>(p.squares_x)), 1.f);
+  const float cy = __fsub_rn(__fmul_rn(__fdiv_rn(__fsub_rn(my, p.start_y), __fsub_rn(p.end_y, p.start_y)),
+                                       static_cast<float>(p.squares_y)), 1.f);
+  bool valid = cx >= -1.f && cy >= -1.f && cx <= static_cast<float>(p.squares_x) - 1.f &&
+               cy <= static_cast<float>(p.squares_y) - 1.f;
+  for (int k = 0; valid && k < p.num_tags; ++k) {
+    const int4 tg = p.tags[k];
+    if (cx >= static_cast<float>(tg.x - 1) && cy >= static_cast<float>(tg.y - 1) &&
+        cx <= static_cast<float>(tg.x - 1 + tg.z) && cy <= static_cast<float>(tg.y - 1 + tg.w))
+      valid = false;
+  }
+  uint8_t out = 0;
+  if (valid) {
+    const float v = __fmul_rn(255.99f, rendering);
+    out = synth_u8(0.f < v ? v : 0.f);  // std::max<float>(0.f, v): NaN gives 0.f
+  } else {
+    const float qx = __fsub_rn(ix, 0.5f), qy = __fsub_rn(iy, 0.5f);
+    if (qx >= 0.f && qy >= 0.f && qx < static_cast<float>(p.pattern_w - 1) &&
+        qy < static_cast<float>(p.pattern_h - 1)) {
+      const int jx = static_cast<int>(qx), jy = static_cast<int>(qy);
+      const float fx = __fsub_rn(qx, static_cast<float>(jx)), fy = __fsub_rn(qy, static_cast<float>(jy));
+      const float gx = __fsub_rn(1.f, fx), gy = __fsub_rn(1.f, fy);
+      const uint8_t* row = pattern + static_cast<int64_t>(jy) * p.pattern_w + jx;
+      const float v = __fadd_rn(
+          __fadd_rn(__fadd_rn(__fmul_rn(__fmul_rn(gx, gy), static_cast<float>(row[0])),
+                              __fmul_rn(__fmul_rn(fx, gy), static_cast<float>(row[1]))),
+                    __fmul_rn(__fmul_rn(gx, fy), static_cast<float>(row[p.pattern_w]))),
+          __fmul_rn(__fmul_rn(fx, fy), static_cast<float>(row[p.pattern_w + 1])));
+      out = synth_u8(v);
+    }
+  }
+  images[(static_cast<int64_t>(img) * p.h + y) * p.w + x] = out;
+}
+
+void launch_render_pattern(const SynthParams& p, int n_img, const float2* verts, const int8_t* nv, const float* poses,
+                           const uint8_t* pattern, double2* proj, int4* range, uint32_t* bits, uint8_t* images,
+                           cudaStream_t s) {
+  if (n_img == 0) return;
+  const int64_t n = static_cast<int64_t>(n_img) * p.n_poly;
+  if (n > 0)
+    synth_project_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(p, n_img, verts, nv, poses, proj,
+                                                                               range, bits);
+  synth_render_kernel<<<dim3(p.tiles_x, p.tiles_y, n_img), dim3(kSynthTile, kSynthTile), 0, s>>>(
+      p, poses, nv, proj, range, bits, pattern, images);
 }
 
 }  // namespace b200ba

@@ -111,6 +111,22 @@ void launch_visualize_camera(const double* params, int w, int h, const double* r
 void launch_intersect_features(int d, int64_t n_lists, int64_t max_list, const int64_t* off, float2* xy, float bound,
                                uint8_t* keep, float2* centres, int* n_centres, unsigned long long* counts,
                                cudaStream_t s);
+// synthetic pattern images of b200ba_render_pattern_images (the arithmetic is specified in include/b200ba.h)
+constexpr int kSynthTile = 16;     // screen tiles of kSynthTile x kSynthTile pixels
+constexpr int kSynthMaxVerts = 4;  // vertices of one pattern polygon
+struct SynthParams {
+  int w, h, tiles_x, tiles_y, words, n_poly;  // words: 32-bit words of one tile's polygon bitmap
+  float fx, fy, cx, cy;
+  int pattern_w, pattern_h, squares_x, squares_y, num_tags;
+  float page_w, page_h, start_x, start_y, end_x, end_y;
+  int4 tags[B200BA_PATTERN_MAX_TAGS];  // x, y, width, height
+};
+// n_img images of one chunk: verts [n_poly][kSynthMaxVerts] (pattern-image pixels, z = 0), nv [n_poly], poses
+// [n_img][24] (Rf, tf, Rc, tc), pattern [pattern_h][pattern_w]; proj [n_img][n_poly][kSynthMaxVerts] and range
+// [n_img][n_poly] are scratch, bits [n_img][tiles_y][tiles_x][words] must be zero on entry; images [n_img][h][w].
+void launch_render_pattern(const SynthParams& p, int n_img, const float2* verts, const int8_t* nv, const float* poses,
+                           const uint8_t* pattern, double2* proj, int4* range, uint32_t* bits, uint8_t* images,
+                           cudaStream_t s);
 void launch_generic_block_inverse(int bs, int nb, int nd, const double* D, const double* B, const double* b1,
                                   double* DinvB, double* Dinvb, cudaStream_t s);
 void launch_symmetrize(int n, double* M, cudaStream_t s);

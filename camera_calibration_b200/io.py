@@ -830,3 +830,161 @@ def LegendErrorDirectionsImage() -> np.ndarray:
             d = _atan2f(y + 0.5 - 100.0, x + 0.5 - 100.0)
             image[y, x] = (int(127 + 127 * math.sin(d) + 0.5), int(127 + 127 * math.cos(d) + 0.5), 127)
     return image
+
+
+# ---------------------------------------------------------------------------------------
+# synthetic datasets: the pattern YAML file and PNG reading
+# ---------------------------------------------------------------------------------------
+def _float32_of_text(text: str) -> float:
+    """The float nearest to the decimal ``text`` (what yaml-cpp's ``as<float>()`` reads through strtof), ties to even;
+    rounding through the nearest double first could round twice."""
+    from fractions import Fraction
+    v = float(text)
+    f = np.float32(v)
+    if not np.isfinite(v) or not np.isfinite(f):
+        return float(f)
+    exact = Fraction(text.strip())
+    best = None
+    for c in (np.nextafter(f, np.float32(-np.inf)), f, np.nextafter(f, np.float32(np.inf))):
+        d = abs(Fraction(float(c)) - exact)
+        even = (int(np.array(c, np.float32).view(np.uint32)) & 1) == 0
+        if best is None or d < best[0] or (d == best[0] and even):
+            best = (d, c)
+    return float(best[1])
+
+
+def LoadPatternYAML(path: str):
+    """A pattern YAML file as FeatureDetectorTaggedPattern reads it (feature_detector_tagged_pattern.cc:175-196):
+    ``num_star_segments``, ``squares_x``, ``squares_y``, the ``page`` map (``width_mm``, ``height_mm``,
+    ``pattern_{start,end}_{x,y}_mm``, read as floats) and the ``apriltags`` list (``tag_x``, ``tag_y``, ``width``,
+    ``height``, ``index``). Returns a dict with the keys of cabi.Pattern (``page_width_mm``, ...) and ``tags`` (a list
+    of dicts ``x``, ``y``, ``width``, ``height``, ``index``), or None when the file cannot be read or a field is
+    missing or not a number. The C++ LoadPatternYAML (b200ba_io.hpp) reads the same values."""
+    try:
+        with open(path, encoding="utf-8") as f:
+            doc = yaml.load(f, Loader=yaml.BaseLoader)
+    except (OSError, UnicodeDecodeError, yaml.YAMLError):
+        return None
+    if not isinstance(doc, dict):
+        return None
+
+    def integer(node, key):
+        v = node.get(key) if isinstance(node, dict) else None
+        return ParseInt32(v.strip()) if isinstance(v, str) else None
+
+    def decimal(node, key):
+        v = node.get(key) if isinstance(node, dict) else None
+        return _float32_of_text(v) if isinstance(v, str) and ParseDecimal(v.strip()) is not None else None
+
+    out = {k: integer(doc, k) for k in ("num_star_segments", "squares_x", "squares_y")}
+    page = doc.get("page")
+    for key, name in (("page_width_mm", "width_mm"), ("page_height_mm", "height_mm"),
+                      ("pattern_start_x_mm", "pattern_start_x_mm"), ("pattern_start_y_mm", "pattern_start_y_mm"),
+                      ("pattern_end_x_mm", "pattern_end_x_mm"), ("pattern_end_y_mm", "pattern_end_y_mm")):
+        out[key] = decimal(page, name)
+    tags = doc.get("apriltags", [])
+    if tags in ("", None):
+        tags = []
+    if not isinstance(tags, list):
+        return None
+    out["tags"] = []
+    for t in tags:
+        tag = {k: integer(t, n) for k, n in (("x", "tag_x"), ("y", "tag_y"), ("width", "width"), ("height", "height"),
+                                           ("index", "index"))}
+        if None in tag.values():
+            return None
+        out["tags"].append(tag)
+    if any(v is None for v in out.values()):
+        return None
+    return out
+
+
+_PNG_CHANNELS = {0: 1, 2: 3, 4: 2, 6: 4}
+
+
+def DecodePNG(data: bytes) -> np.ndarray:
+    """An 8-bit, non-interlaced PNG of colour type 0, 2, 4 or 6 (any filter types, IDAT split over any number of
+    chunks) as a grey [h, w] uint8 image, converted as libvis' libpng reader converts it
+    (image_io_libpng.cc:219-226): alpha is dropped; a pixel with r == g == b is that value, any other RGB pixel is
+    (6968 r + 23434 g + 2366 b) >> 15 (libpng's default rgb_to_gray weights, truncated; gAMA, sRGB and other
+    ancillary chunks are ignored). Raises ValueError with a message for anything else (16-bit, palette, interlaced,
+    a broken stream). The C++ DecodePNG (b200ba_io.hpp) decodes to the same pixels."""
+    import zlib
+    if data[:8] != b"\x89PNG\r\n\x1a\n":
+        raise ValueError("DecodePNG: not a PNG file")
+    pos, ihdr, idat = 8, None, bytearray()
+    while pos + 8 <= len(data):
+        (length,) = struct.unpack(">I", data[pos:pos + 4])
+        kind = data[pos + 4:pos + 8]
+        body = data[pos + 8:pos + 8 + length]
+        if len(body) != length:
+            raise ValueError("DecodePNG: truncated chunk")
+        pos += 12 + length
+        if kind == b"IHDR":
+            ihdr = struct.unpack(">IIBBBBB", body)
+        elif kind == b"IDAT":
+            idat += body
+        elif kind == b"IEND":
+            break
+    if ihdr is None:
+        raise ValueError("DecodePNG: no IHDR chunk")
+    w, h, depth, color, compression, filt, interlace = ihdr
+    if depth != 8:
+        raise ValueError(f"DecodePNG: bit depth {depth} is not supported (only 8)")
+    if color not in _PNG_CHANNELS:
+        raise ValueError(f"DecodePNG: colour type {color} is not supported (only 0, 2, 4 and 6)")
+    if interlace != 0:
+        raise ValueError("DecodePNG: interlaced images are not supported")
+    if compression != 0 or filt != 0 or w < 1 or h < 1:
+        raise ValueError("DecodePNG: invalid IHDR")
+    ch = _PNG_CHANNELS[color]
+    try:
+        raw = zlib.decompress(bytes(idat))
+    except zlib.error as e:
+        raise ValueError(f"DecodePNG: broken zlib stream ({e})") from None
+    stride = w * ch
+    if len(raw) < h * (stride + 1):
+        raise ValueError("DecodePNG: image data too short")
+    rows = np.frombuffer(raw, np.uint8, h * (stride + 1)).reshape(h, stride + 1)
+    out = np.zeros((h, stride), np.int32)
+    prev = np.zeros(stride, np.int32)
+    for y in range(h):
+        ft, line = rows[y, 0], rows[y, 1:].astype(np.int32)
+        if ft == 0:
+            cur = line
+        elif ft == 2:
+            cur = (line + prev) & 0xFF
+        elif ft in (1, 3, 4):
+            cur = np.zeros(stride, np.int32)
+            for x in range(stride):
+                a = int(cur[x - ch]) if x >= ch else 0
+                b = int(prev[x])
+                if ft == 1:
+                    p = a
+                elif ft == 3:
+                    p = (a + b) >> 1
+                else:
+                    c = int(prev[x - ch]) if x >= ch else 0
+                    pa, pb, pc = abs(b - c), abs(a - c), abs(a + b - 2 * c)
+                    p = a if pa <= pb and pa <= pc else (b if pb <= pc else c)
+                cur[x] = (int(line[x]) + p) & 0xFF
+        else:
+            raise ValueError(f"DecodePNG: unknown filter type {ft}")
+        out[y] = cur
+        prev = cur
+    px = out.reshape(h, w, ch)
+    if ch <= 2:
+        return px[:, :, 0].astype(np.uint8)
+    r, g, b = px[:, :, 0], px[:, :, 1], px[:, :, 2]
+    mixed = (6968 * r + 23434 * g + 2366 * b) >> 15
+    return np.where((r == g) & (r == b), r, mixed).astype(np.uint8)
+
+
+def ReadPNG(path: str) -> Optional[np.ndarray]:
+    """DecodePNG of the file at ``path``; None if it cannot be read. Raises ValueError for an unsupported PNG."""
+    try:
+        with open(path, "rb") as f:
+            data = f.read()
+    except OSError:
+        return None
+    return DecodePNG(data)

@@ -9,7 +9,8 @@ the ``--compare_calibrations`` tool (``CompareCalibrations``, tools/compare_cali
 ``--localization_accuracy_test`` tool (``LocalizationAccuracyTest``, tools/localization_accuracy_test.cc:47-131), the
 ``--compare_reconstructions`` tool (``CompareReconstructions``, tools/bundle_adjustment.cc:223-392) and the calibration
 visualisation tools (``VisualizeKalibrCalibration``, ``VisualizeColmapCalibration``, tools/visualize_calibration.cc;
-``CreateLegends``, tools/create_legends.cc).
+``CreateLegends``, tools/create_legends.cc) and the ``--render_synthetic_dataset`` tool (``RenderSyntheticDataset``,
+tools/render_synthetic_dataset.cc).
 Host logic only; every numerical step (un-projection, the LM iteration, the report's statistics) runs in
 ``libb200ba.so``.
 """
@@ -791,3 +792,62 @@ def IntersectDatasets(dataset_paths, intersection_threshold: float = 3.0, inters
     for i, ds in enumerate(datasets):
         print(f"Remaining features in dataset {i}: {_feature_count(ds)}", file=sys.stderr)
     return 0
+
+
+SYNTHETIC_PATTERN_NAME = "pattern_resolution_17x24_segments_16_apriltag_0"
+
+
+def RenderSyntheticDataset(path: str, pattern_yaml: str = SYNTHETIC_PATTERN_NAME + ".yaml",
+                           pattern_png: str = SYNTHETIC_PATTERN_NAME + ".png", num_images: int = 500,
+                           seed: int = 0, device: int = -1) -> int:
+    """The ``--render_synthetic_dataset`` tool (tools/render_synthetic_dataset.cc:43-298): a 640 x 480 pinhole camera
+    (fx = fy = 480, cx = 320, cy = 240, pixel-corner convention) views the pattern of ``pattern_yaml`` /
+    ``pattern_png`` from ``num_images`` random poses (``api.SyntheticPoses``, seeded; the reference seeds with the
+    time and reads the pattern from beside its binary), and the images are rendered on the device
+    (``api.RenderPatternImages``). Writes ``<path>/dataset.yaml`` (the reference's text) and
+    ``<path>/images0/000000.png`` ... (io.WritePNG), printing ``Rendering image i ...`` to stderr. Returns
+    EXIT_SUCCESS / EXIT_FAILURE with the reference's messages; the C++ RenderSyntheticDataset (b200ba_pipeline.hpp)
+    writes the same bytes."""
+    import os
+    import sys
+    from . import cabi, io
+    width, height = 640, 480
+    k = np.array([height, height, 0.5 * width, 0.5 * height], np.float32)
+    pattern = io.LoadPatternYAML(pattern_yaml)
+    if pattern is None:
+        print(f"Failed to load: {pattern_yaml}", file=sys.stderr)
+        return 1
+    try:
+        pattern_image = io.ReadPNG(pattern_png)
+    except ValueError as e:
+        print(f"{e}", file=sys.stderr)
+        pattern_image = None
+    if pattern_image is None:
+        print(f"Cannot load the pattern image from: {pattern_png}", file=sys.stderr)
+        return 1
+    if len(pattern["tags"]) > cabi.PATTERN_MAX_TAGS:
+        print(f"The pattern has more than {cabi.PATTERN_MAX_TAGS} AprilTags, which is not supported.", file=sys.stderr)
+        return 1
+    os.makedirs(path, exist_ok=True)
+    yaml_path = os.path.abspath(os.path.join(path, "dataset.yaml"))
+    text = (f"- camera: \"Synthetic pinhole camera (fx: {k[0]:g}, fy: {k[1]:g}, cx: {k[2]:g}, cy: {k[3]:g}, "
+            f"'pixel corner' coordinate origin convention)\"\n  path: \"images0\"\n")
+    try:
+        with open(yaml_path, "w", newline="\n") as f:
+            f.write(text)
+    except OSError:
+        print(f"Failed to write dataset YAML file at: {yaml_path}", file=sys.stderr)
+        return 1
+    images_dir = os.path.join(path, "images0")
+    os.makedirs(images_dir, exist_ok=True)
+    if num_images < 1:
+        return 0
+    pattern_size = (pattern_image.shape[1], pattern_image.shape[0])
+    poses, _ = api.SyntheticPoses(pattern, pattern_size, (width, height), k, num_images, seed)
+    images, _ = api.RenderPatternImages(pattern, pattern_image, (width, height), k, poses, device=device)
+    for i in range(num_images):
+        print(f"Rendering image {i} ...", file=sys.stderr)
+        io.WritePNG(os.path.join(images_dir, f"{i:06d}.png"), images[i])
+    sys.stderr.flush()
+    return 0
+

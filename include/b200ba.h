@@ -607,6 +607,106 @@ B200BA_API int b200ba_intersect_features(int device, int32_t n_datasets, int64_t
                                          const float* xy, double threshold, uint8_t* keep,
                                          b200ba_intersection_report* report, double* device_ms);
 
+/* ---- synthetic calibration-pattern images (APP/tools/render_synthetic_dataset.cc, --render_synthetic_dataset): the
+ * star pattern of a pattern YAML file (feature_detector_tagged_pattern.{h,cc}: PatternData) seen through a pinhole
+ * camera from random poses, drawn with exact per-pixel area coverage so that the images carry no sampling bias.
+ * All float operations below are rounded one by one in the order written (no fused multiply-add).
+ *
+ * The pattern. Its numbers are the floats the reference reads (`as<float>()`); at most B200BA_PATTERN_MAX_TAGS tags
+ * are taken (more is refused with 2). pattern_w x pattern_h is the size of the pattern image (the PNG beside the
+ * YAML file). A pattern coordinate c (features at integers) maps to pattern-image pixels (pixel-corner convention) as
+ *   mm.x = start_x + ((c.x + 1) / (float)squares_x) * (end_x - start_x),  px.x = ((float)pattern_w / page_w) * mm.x
+ * (y alike). The polygons are PatternData::ComputePatternGeometry without AprilTags, in generation order (features
+ * y-major from (-1, -1), skipping features inside a tag, the black segments 0, 2, ... of each star whose middle
+ * direction lies in the repeating area), each vertex mapped as above and lifted to z = 0. The star corners are
+ * computed on the host with the C library's float sin / cos, as the reference computes them. Every polygon has 3 or 4
+ * vertices. */
+#define B200BA_PATTERN_MAX_TAGS 16
+typedef struct b200ba_pattern_tag {
+  int32_t x, y, width, height, index; /* tag_x, tag_y (squares), width, height (squares), index in its family */
+} b200ba_pattern_tag;
+typedef struct b200ba_pattern {
+  int32_t squares_x, squares_y, num_star_segments, num_tags;
+  float page_width_mm, page_height_mm, pattern_start_x_mm, pattern_start_y_mm, pattern_end_x_mm, pattern_end_y_mm;
+  b200ba_pattern_tag tags[B200BA_PATTERN_MAX_TAGS];
+} b200ba_pattern;
+/* Poses (host only; the Python and C++ tools both call this). camera_tr_global [n][12]: the row-major rotation R
+ * and the translation t of camera <- pattern, in double. Image i, attempt a (a = 0, 1, ...) draws from the stream of
+ * b200ba_localization_accuracy with key = (i << 24) | (a << 4) | component, h = SplitMix64(SplitMix64(seed) ^ key):
+ *   components 0-2: f_k = (float)(h_k % 10000) / 10000.f;
+ *     t0 = (0.0 - (double)((-1.f + 2.f * f_0) * (float)pattern_w), 0.0 - (double)((-1.f + 2.f * f_1) *
+ *          (float)pattern_h), 0.0 + (double)(500.f + 800.f * f_2));
+ *   components 3-8: r_k = -1.0 + 2.0 * ((double)(h_k >> 11) * 2^-53) in [-1, 1); the tangent is
+ *     (u, w) = 0.5 * (r_3 .. r_5, r_6 .. r_8) (Sophus order: translation part first).
+ *   Sophus' SE3d::exp, in double with the C library's sin / cos: th2 = (wx wx + wy wy) + wz wz, th = sqrt(th2);
+ *     th < 1e-10: im = (0.5 - (1/48) th2) + (1/3840) th2^2, re = (1 - 0.5 th2) + (1/384) th2^2, else
+ *     im = sin(th / 2) / th, re = cos(th / 2) (th / 2 as 0.5 * th); q = (re, im wx, im wy, im wz);
+ *     W = hat(w), W2 = W W (each entry a sum over k = 0, 1, 2 in order); V = rotation(q) when th < 1e-10, else
+ *     (I + ((1 - cos th) / th2) W) + ((th - sin th) / (th2 th)) W2; t_exp = V u (each row (a0 u0 + a1 u1) + a2 u2).
+ *   The pose is exp(tangent) * (I, t0) as Sophus composes it: t = t_exp + q.v where q.v = (v + re uv) + im_vec x uv,
+ *     uv = 2 (im_vec x v) (Eigen's _transformVector, with the un-normalised q); then q is renormalised as SO3's *=:
+ *     s = (x^2 + z^2) + (y^2 + w^2), q *= 2 / (1 + s) unless s == 1; R = rotation(q) with Eigen's toRotationMatrix
+ *     (tx = 2x, twx = tx w, txx = tx x, ..., R00 = 1 - (tyy + tzz), R01 = txy - twz, ...).
+ *   The pose is taken when, for some tag, the four corners of the tag's square (pattern coordinates (tag.x - 1,
+ *   tag.y - 1) and (tag.x - 1 + width, tag.y - 1 + height), mapped as above) are all visible with border 0 to the
+ *   float pose Rf = (float)R, tf = (float)t: p_cam_i = ((Rf_i0 x + Rf_i1 y) + Rf_i2 z) + tf_i, p_cam_z > 0 and the
+ *   pixel (fx (p_cam_x / p_cam_z) + cx, fy (p_cam_y / p_cam_z) + cy) inside [0, width) x [0, height). Otherwise the
+ *   attempt is drawn again. attempts (nullable): [n] the number of attempts of every image.
+ * Worked examples (the fixture pattern of tests/golden/pattern, 1124 x 1590, 640 x 480, fx = fy = 480, cx = 320,
+ * cy = 240):
+ *   seed 0, image 0: attempt 0 has h_0 = 0xa706dd2f4d197e6f (k = 7055); 11 attempts show no whole tag; attempt 11
+ *     (h_0 = 0x89c20cbbf41b13e7, k = 7431) is taken with t = (-88.31650879202545, -535.3216881191287,
+ *     1468.5512805064373), R_00 = 0.9036277796763321;
+ *   seed 7, image 3: attempt 0 (h_0 = 0x18080193089f89c2, k = 9218; h_3 = 0xfc9ef4a796148570) is taken with
+ *     t = (-928.6952246323646, -359.4073177209594, 1231.647888783845), R_00 = 0.9714992824303272.
+ * Returns 2 for a bad argument (NULL pointers, sizes below 1 or above 2^15, n < 1 or n >= 2^40, and the pattern and
+ * camera checks of b200ba_render_pattern_images below), 4 when an image has no visible tag
+ * after 4096 attempts (the reference would draw forever; camera_tr_global then holds the images before it).
+ * The reference seeds rand() with the time and draws Eigen / Sophus Random(); this stream is seeded and repeatable. */
+B200BA_API int b200ba_synthetic_poses(const b200ba_pattern* pattern, int32_t pattern_w, int32_t pattern_h,
+                                      int32_t width, int32_t height, const float* fx_fy_cx_cy, int64_t n,
+                                      uint64_t seed, double* camera_tr_global, int64_t* attempts);
+/* Images. images [n][height][width] u8, one per pose of camera_tr_global [n][12] (as above). The float pose is
+ * Rf = (float)R, tf = (float)t; the inverse is taken in double, R^T and ti = R^T (-t) (row i: (R_0i (-t0) +
+ * R_1i (-t1)) + R_2i (-t2)), and cast to float afterwards (Rc, tc).
+ *   Coverage (:202-243): a float image set to 1. For every polygon in generation order, every vertex p is projected
+ *     in float (p_cam_i = ((Rf_i0 p.x + Rf_i1 p.y) + Rf_i2 p.z) + tf_i, pixel = (fx (p_cam_x / p_cam_z) + cx,
+ *     fy (p_cam_y / p_cam_z) + cy)) and cast to double, without a visibility test: a vertex behind the camera is
+ *     projected through its negative depth, exactly as the reference does. The pixel range is the bounding box
+ *     of the vertices, converted to int as x86-64 does (truncation toward zero; INT_MIN for values outside the int
+ *     range and for +-inf, so that a box reaching beyond 2^31 in x or y draws nothing and one reaching below -2^31
+ *     starts at 0), clamped to [0, width - 1] x [0, height - 1]. A polygon with a NaN projected coordinate draws
+ *     nothing (the pinned case; it needs p_cam_z == 0 and p_cam_x == 0 or p_cam_y == 0). For every pixel (x, y) of
+ *     the range, rendering(x, y) = (float)((double)rendering(x, y) - A), A = libvis' PolygonArea of libvis'
+ *     ConvexClipPolygon of the projected polygon against the pixel square (x, y), (x + 1, y), (x + 1, y + 1),
+ *     (x, y + 1), in double, with its float edge offset and its IEEE comparisons (a NaN vertex counts as inside)
+ *     and LineLineIntersection's result (the previous vertex where its denominator is 0, else the quotients, even
+ *     non-finite ones); PolygonArea = |0.5 * sum_i (x_i - x_{i-1})
+ *     (y_i + y_{i-1})| summed from i = 0 with i - 1 = last.
+ *   Composition (:248-291): per pixel, the ray of (x + 0.5f, y + 0.5f) is d = Rc (x' , y', 1) with
+ *     x' = (1.f / fx) (x + 0.5f) + (-cx / fx) (y alike; rows (a0 x' + a1 y') + a2), normalised as Eigen does
+ *     (n2 = (dx dx + dy dy) + dz dz, d / sqrtf(n2) when n2 > 0), and meets the plane z = 0 (normal (0, 0, -1),
+ *     offset -0.f) at t = -(offset + ((0 tx + 0 ty) + -1 tz)) / ((0 dx + 0 dy) + -1 dz), point = tc + d t
+ *     (Eigen's ParametrizedLine::intersectionPoint). Its pattern-image coordinate is (1 (X - 0) + 0 (Y + 0), 0 (X - 0)
+ *     + 1 (Y + 0)) (the normalised image axes), mm = (page_w / (float)pattern_w) * that, pattern coordinate =
+ *     ((mm - start) / (end - start)) * (float)squares - 1. Inside IsValidPatternCoord (in [-1, squares - 1] and in
+ *     no tag's [tag - 1, tag - 1 + size] box) the byte is u8(max(0.f, 255.99f * rendering)); else, at c = coordinate
+ *     - 0.5f, if 0 <= c < (float)(pattern size - 1) it is libvis' InterpolateBilinear<float> of the pattern image
+ *     (i = (int)c, f = c - i, (((1 - fx)(1 - fy)) p00 + (fx (1 - fy)) p10) + ((1 - fx) fy) p01) + (fx fy) p11),
+ *     and 0 otherwise. u8(v) is static_cast<int>(v) as x86-64 executes it (truncation; INT_MIN for NaN, hence 0)
+ *     reduced to its low byte.
+ * pattern_image [pattern_h][pattern_w] grey u8. Images are rendered in chunks bounded in device memory (about
+ * 512 MiB; the environment variable B200BA_SYNTH_CHUNK lowers the images per chunk), so any n works; the bytes do not
+ * depend on the chunking. device_ms (nullable): device time of the rendering.
+ * Stand-alone (allocates, computes, frees). Returns 2 for a bad argument before any CUDA call (NULL pointers, a
+ * size below 1 or above 2^15, n < 0, num_tags outside [0, B200BA_PATTERN_MAX_TAGS], squares below 1,
+ * num_star_segments below 2, odd or above 1024, more than 2^24 star segments ((squares_x + 1) (squares_y + 1)
+ * num_star_segments / 2), a non-finite or zero focal length, a non-finite principal point), 3 without a device. Repeated calls give identical bytes. */
+B200BA_API int b200ba_render_pattern_images(int device, const b200ba_pattern* pattern, const uint8_t* pattern_image,
+                                            int32_t pattern_w, int32_t pattern_h, int32_t width, int32_t height,
+                                            const float* fx_fy_cx_cy, int64_t n, const double* camera_tr_global,
+                                            uint8_t* images, double* device_ms);
+
 /* ---- multi-GPU: imagesets sharded over ranks, one NCCL all-reduce per H/b build --- */
 #define B200BA_NCCL_UNIQUE_ID_BYTES 128
 B200BA_API int b200ba_nccl_unique_id(uint8_t id[B200BA_NCCL_UNIQUE_ID_BYTES]);

@@ -583,6 +583,14 @@ inline uint32_t png_crc32(const std::string& data, size_t begin) {
   for (size_t i = begin; i < data.size(); ++i) c = table[(c ^ static_cast<uint8_t>(data[i])) & 0xff] ^ (c >> 8);
   return c ^ 0xffffffffu;
 }
+inline uint32_t adler32(const std::string& data) {
+  uint32_t a = 1, b = 0;
+  for (char ch : data) {
+    a = (a + static_cast<uint8_t>(ch)) % 65521u;
+    b = (b + a) % 65521u;
+  }
+  return (b << 16) | a;
+}
 inline void put_be32(std::string* out, uint32_t v) {
   const char b[4] = {static_cast<char>(v >> 24), static_cast<char>(v >> 16), static_cast<char>(v >> 8), static_cast<char>(v)};
   out->append(b, 4);
@@ -619,12 +627,7 @@ inline bool WritePNG(const std::string& path, int width, int height, int channel
     z.append(raw, pos, len);
     pos += len;
   } while (pos < raw.size());
-  uint32_t a = 1, b = 0;  // Adler-32
-  for (char ch : raw) {
-    a = (a + static_cast<uint8_t>(ch)) % 65521u;
-    b = (b + a) % 65521u;
-  }
-  io_detail::put_be32(&z, (b << 16) | a);
+  io_detail::put_be32(&z, io_detail::adler32(raw));
   std::string ihdr;
   io_detail::put_be32(&ihdr, static_cast<uint32_t>(width));
   io_detail::put_be32(&ihdr, static_cast<uint32_t>(height));
@@ -1167,6 +1170,384 @@ inline std::vector<uint8_t> LegendErrorDirections() {
       p[2] = 127;
     }
   return image;
+}
+
+// ---- pattern YAML files (feature_detector_tagged_pattern.cc:175-196) ------------------------------------------------
+// The subset the pattern files use: top-level `key: scalar`, the `page:` map of scalars and the `apriltags:` block list
+// of flat maps (`- tag_x: 6` followed by the item's other keys, indented), `#` comments. Floats are read with strtof
+// (what yaml-cpp's as<float>() reads), integers as decimal int32. io.py's LoadPatternYAML reads the same values.
+struct PatternFile {
+  int num_star_segments = 0, squares_x = 0, squares_y = 0;
+  float page_width_mm = 0, page_height_mm = 0, pattern_start_x_mm = 0, pattern_start_y_mm = 0, pattern_end_x_mm = 0,
+        pattern_end_y_mm = 0;
+  struct Tag {
+    int x, y, width, height, index;
+  };
+  std::vector<Tag> tags;
+};
+
+namespace io_detail {
+inline std::string strip_comment(const std::string& line) {
+  char quote = 0;
+  for (size_t i = 0; i < line.size(); ++i) {
+    const char c = line[i];
+    if (quote) {
+      if (c == quote) quote = 0;
+    } else if (c == '"' || c == '\'') {
+      quote = c;
+    } else if (c == '#' && (i == 0 || line[i - 1] == ' ' || line[i - 1] == '\t')) {
+      return line.substr(0, i);
+    }
+  }
+  return line;
+}
+inline bool pattern_float(const std::map<std::string, std::string>& m, const char* key, float* out) {
+  auto it = m.find(key);
+  double unused;
+  if (it == m.end() || !ParseDecimal(it->second, &unused)) return false;
+  *out = std::strtof(it->second.c_str(), nullptr);
+  return true;
+}
+inline bool pattern_int(const std::map<std::string, std::string>& m, const char* key, int* out) {
+  auto it = m.find(key);
+  return it != m.end() && ParseInt32(it->second, out);
+}
+}  // namespace io_detail
+
+// Returns false when the file cannot be read or a field is missing or not a number.
+inline bool LoadPatternYAML(const std::string& path, PatternFile* pattern) {
+  std::string text;
+  if (!io_detail::read_file(path, &text)) return false;
+  std::map<std::string, std::string> top, page;
+  std::vector<std::map<std::string, std::string>> tags;
+  std::string section;  // "page" or "apriltags" while inside that block
+  for (std::string line : io_detail::split_lines(text)) {
+    if (!line.empty() && line.back() == '\r') line.pop_back();
+    line = io_detail::strip_comment(line);
+    if (io_detail::trim(line).empty()) continue;
+    const size_t indent = line.find_first_not_of(" \t");
+    std::string body = line.substr(indent);
+    if (indent == 0) {
+      section.clear();
+      const size_t colon = body.find(':');
+      if (colon == std::string::npos) return false;
+      const std::string key = io_detail::trim(body.substr(0, colon));
+      const std::string value = io_detail::trim(body.substr(colon + 1));
+      if (value.empty() && (key == "page" || key == "apriltags")) {
+        section = key;
+      } else if (!(key == "apriltags" && value == "[]")) {  // "apriltags: []" is a pattern without tags
+        top[key] = io_detail::unquote(value);
+      }
+      continue;
+    }
+    if (section.empty()) return false;
+    std::map<std::string, std::string>* target = &page;
+    if (section == "apriltags") {
+      if (body[0] == '-') {
+        tags.emplace_back();
+        body = io_detail::trim(body.substr(1));
+        if (body.empty()) continue;
+      } else if (tags.empty()) {
+        return false;
+      }
+      target = &tags.back();
+    }
+    const size_t colon = body.find(':');
+    if (colon == std::string::npos) return false;
+    (*target)[io_detail::trim(body.substr(0, colon))] = io_detail::unquote(io_detail::trim(body.substr(colon + 1)));
+  }
+  PatternFile p;
+  if (!io_detail::pattern_int(top, "num_star_segments", &p.num_star_segments) ||
+      !io_detail::pattern_int(top, "squares_x", &p.squares_x) || !io_detail::pattern_int(top, "squares_y", &p.squares_y) ||
+      !io_detail::pattern_float(page, "width_mm", &p.page_width_mm) ||
+      !io_detail::pattern_float(page, "height_mm", &p.page_height_mm) ||
+      !io_detail::pattern_float(page, "pattern_start_x_mm", &p.pattern_start_x_mm) ||
+      !io_detail::pattern_float(page, "pattern_start_y_mm", &p.pattern_start_y_mm) ||
+      !io_detail::pattern_float(page, "pattern_end_x_mm", &p.pattern_end_x_mm) ||
+      !io_detail::pattern_float(page, "pattern_end_y_mm", &p.pattern_end_y_mm))
+    return false;
+  for (const auto& t : tags) {
+    PatternFile::Tag tag;
+    if (!io_detail::pattern_int(t, "tag_x", &tag.x) || !io_detail::pattern_int(t, "tag_y", &tag.y) ||
+        !io_detail::pattern_int(t, "width", &tag.width) || !io_detail::pattern_int(t, "height", &tag.height) ||
+        !io_detail::pattern_int(t, "index", &tag.index))
+      return false;
+    p.tags.push_back(tag);
+  }
+  *pattern = p;
+  return true;
+}
+
+// ---- PNG reading ----------------------------------------------------------------------------------------------------
+// 8-bit, non-interlaced PNGs of colour type 0, 2, 4 or 6, any filter types, IDAT split over any number of chunks, as
+// a grey image converted as libvis' libpng reader converts it (image_io_libpng.cc:219-226): alpha is dropped; a pixel
+// with r == g == b is that value, any other RGB pixel is (6968 r + 23434 g + 2366 b) >> 15 (libpng's default
+// rgb_to_gray weights, truncated; gAMA, sRGB and other ancillary chunks are ignored). The zlib stream is inflated
+// here (stored, fixed- and dynamic-Huffman blocks), so no compression library is needed. io.py's DecodePNG decodes
+// to the same pixels.
+namespace io_detail {
+struct Inflate {
+  const uint8_t* in;
+  size_t n, pos = 0;
+  uint32_t bitbuf = 0;
+  int bitcnt = 0;
+  std::string* out;
+  bool error = false;
+
+  struct Huffman {
+    short count[16];
+    short symbol[288];
+  };
+  int bits(int need) {
+    uint32_t val = bitbuf;
+    while (bitcnt < need) {
+      if (pos >= n) {
+        error = true;
+        return 0;
+      }
+      val |= static_cast<uint32_t>(in[pos++]) << bitcnt;
+      bitcnt += 8;
+    }
+    bitbuf = val >> need;
+    bitcnt -= need;
+    return static_cast<int>(val & ((1u << need) - 1));
+  }
+  // canonical code from code lengths; false for an over-subscribed set
+  static bool construct(Huffman* h, const short* length, int n) {
+    for (int len = 0; len < 16; ++len) h->count[len] = 0;
+    for (int s = 0; s < n; ++s) h->count[length[s]]++;
+    int left = 1;
+    for (int len = 1; len < 16; ++len) {
+      left <<= 1;
+      left -= h->count[len];
+      if (left < 0) return false;
+    }
+    short offs[16];
+    offs[1] = 0;
+    for (int len = 1; len < 15; ++len) offs[len + 1] = offs[len] + h->count[len];
+    for (int s = 0; s < n; ++s)
+      if (length[s] != 0) h->symbol[offs[length[s]]++] = static_cast<short>(s);
+    return true;
+  }
+  int decode(const Huffman& h) {
+    int code = 0, first = 0, index = 0;
+    for (int len = 1; len < 16; ++len) {
+      code |= bits(1);
+      if (error) return -1;
+      const int count = h.count[len];
+      if (code - count < first) return h.symbol[index + (code - first)];
+      index += count;
+      first += count;
+      first <<= 1;
+      code <<= 1;
+    }
+    error = true;
+    return -1;
+  }
+  bool stored() {
+    bitbuf = 0;
+    bitcnt = 0;
+    if (pos + 4 > n) return false;
+    const unsigned len = in[pos] | (in[pos + 1] << 8);
+    const unsigned nlen = in[pos + 2] | (in[pos + 3] << 8);
+    pos += 4;
+    if (len != (~nlen & 0xffffu) || pos + len > n) return false;
+    out->append(reinterpret_cast<const char*>(in + pos), len);
+    pos += len;
+    return true;
+  }
+  bool codes(const Huffman& lencode, const Huffman& distcode) {
+    static const short lbase[29] = {3,  4,  5,  6,  7,  8,  9,  10, 11,  13,  15,  17,  19,  23, 27,
+                                    31, 35, 43, 51, 59, 67, 83, 99, 115, 131, 163, 195, 227, 258};
+    static const short lext[29] = {0, 0, 0, 0, 0, 0, 0, 0, 1, 1, 1, 1, 2, 2, 2, 2, 3, 3, 3, 3, 4, 4, 4, 4, 5, 5, 5, 5, 0};
+    static const short dbase[30] = {1,   2,   3,   4,   5,   7,    9,    13,   17,   25,   33,   49,   65,    97,    129,
+                                    193, 257, 385, 513, 769, 1025, 1537, 2049, 3073, 4097, 6145, 8193, 12289, 16385, 24577};
+    static const short dext[30] = {0, 0, 0, 0, 1, 1, 2, 2, 3, 3, 4, 4, 5, 5, 6, 6, 7, 7, 8, 8, 9, 9, 10, 10, 11, 11, 12, 12, 13, 13};
+    for (;;) {
+      int symbol = decode(lencode);
+      if (symbol < 0 || error) return false;
+      if (symbol < 256) {
+        out->push_back(static_cast<char>(symbol));
+      } else if (symbol == 256) {
+        return true;
+      } else {
+        symbol -= 257;
+        if (symbol >= 29) return false;
+        const int len = lbase[symbol] + bits(lext[symbol]);
+        const int dsym = decode(distcode);
+        if (dsym < 0 || dsym >= 30 || error) return false;
+        const size_t dist = static_cast<size_t>(dbase[dsym] + bits(dext[dsym]));
+        if (error || dist > out->size()) return false;
+        for (int k = 0; k < len; ++k) out->push_back((*out)[out->size() - dist]);
+      }
+    }
+  }
+  bool fixed() {
+    static Huffman lencode, distcode;
+    static bool init = false;
+    if (!init) {
+      short lengths[288];
+      int s = 0;
+      for (; s < 144; ++s) lengths[s] = 8;
+      for (; s < 256; ++s) lengths[s] = 9;
+      for (; s < 280; ++s) lengths[s] = 7;
+      for (; s < 288; ++s) lengths[s] = 8;
+      construct(&lencode, lengths, 288);
+      for (s = 0; s < 30; ++s) lengths[s] = 5;
+      construct(&distcode, lengths, 30);
+      init = true;
+    }
+    return codes(lencode, distcode);
+  }
+  bool dynamic() {
+    static const short order[19] = {16, 17, 18, 0, 8, 7, 9, 6, 10, 5, 11, 4, 12, 3, 13, 2, 14, 1, 15};
+    const int nlen = bits(5) + 257, ndist = bits(5) + 1, ncode = bits(4) + 4;
+    if (error || nlen > 286 || ndist > 30) return false;
+    short lengths[320];
+    int index = 0;
+    for (; index < ncode; ++index) lengths[order[index]] = static_cast<short>(bits(3));
+    for (; index < 19; ++index) lengths[order[index]] = 0;
+    if (error) return false;
+    Huffman lencode, distcode;
+    if (!construct(&lencode, lengths, 19)) return false;
+    index = 0;
+    while (index < nlen + ndist) {
+      int symbol = decode(lencode);
+      if (symbol < 0 || error) return false;
+      if (symbol < 16) {
+        lengths[index++] = static_cast<short>(symbol);
+      } else {
+        short len = 0;
+        int repeat;
+        if (symbol == 16) {
+          if (index == 0) return false;
+          len = lengths[index - 1];
+          repeat = 3 + bits(2);
+        } else if (symbol == 17) {
+          repeat = 3 + bits(3);
+        } else {
+          repeat = 11 + bits(7);
+        }
+        if (error || index + repeat > nlen + ndist) return false;
+        while (repeat--) lengths[index++] = len;
+      }
+    }
+    if (lengths[256] == 0) return false;
+    if (!construct(&lencode, lengths, nlen) || !construct(&distcode, lengths + nlen, ndist)) return false;
+    return codes(lencode, distcode);
+  }
+  // a zlib stream (RFC 1950) holding deflate blocks (RFC 1951); checks the header and the Adler-32
+  bool zlib() {
+    if (n < 6 || (in[0] & 0x0f) != 8 || ((in[0] << 8) | in[1]) % 31 != 0 || (in[1] & 0x20)) return false;
+    pos = 2;
+    int last;
+    do {
+      last = bits(1);
+      const int type = bits(2);
+      if (error) return false;
+      const bool ok = type == 0 ? stored() : type == 1 ? fixed() : type == 2 ? dynamic() : false;
+      if (!ok || error) return false;
+    } while (!last);
+    if (pos + 4 > n) return false;
+    const uint32_t want = (static_cast<uint32_t>(in[pos]) << 24) | (in[pos + 1] << 16) | (in[pos + 2] << 8) | in[pos + 3];
+    return want == adler32(*out);
+  }
+};
+inline uint32_t be32(const std::string& s, size_t at) {
+  return (static_cast<uint32_t>(static_cast<uint8_t>(s[at])) << 24) | (static_cast<uint8_t>(s[at + 1]) << 16) |
+         (static_cast<uint8_t>(s[at + 2]) << 8) | static_cast<uint8_t>(s[at + 3]);
+}
+}  // namespace io_detail
+
+// grey [height * width], row-major. Returns false with a message in *error for anything unsupported or broken.
+inline bool DecodePNG(const std::string& data, int* width, int* height, std::vector<uint8_t>* grey, std::string* error) {
+  auto fail = [&](const std::string& m) {
+    if (error) *error = "DecodePNG: " + m;
+    return false;
+  };
+  if (data.size() < 8 || data.compare(0, 8, std::string("\x89PNG\r\n\x1a\n", 8)) != 0) return fail("not a PNG file");
+  size_t pos = 8;
+  bool have_ihdr = false;
+  uint32_t w = 0, h = 0;
+  int depth = 0, color = 0, compression = 0, filter = 0, interlace = 0;
+  std::string idat;
+  while (pos + 8 <= data.size()) {
+    const uint32_t length = io_detail::be32(data, pos);
+    const std::string kind = data.substr(pos + 4, 4);
+    if (pos + 12 + static_cast<size_t>(length) > data.size() + 4 || pos + 8 + static_cast<size_t>(length) > data.size())
+      return fail("truncated chunk");
+    if (kind == "IHDR" && length >= 13) {
+      w = io_detail::be32(data, pos + 8);
+      h = io_detail::be32(data, pos + 12);
+      depth = static_cast<uint8_t>(data[pos + 16]);
+      color = static_cast<uint8_t>(data[pos + 17]);
+      compression = static_cast<uint8_t>(data[pos + 18]);
+      filter = static_cast<uint8_t>(data[pos + 19]);
+      interlace = static_cast<uint8_t>(data[pos + 20]);
+      have_ihdr = true;
+    } else if (kind == "IDAT") {
+      idat.append(data, pos + 8, length);
+    } else if (kind == "IEND") {
+      break;
+    }
+    pos += 12 + static_cast<size_t>(length);
+  }
+  if (!have_ihdr) return fail("no IHDR chunk");
+  if (depth != 8) return fail("bit depth " + std::to_string(depth) + " is not supported (only 8)");
+  const int ch = color == 0 ? 1 : color == 2 ? 3 : color == 4 ? 2 : color == 6 ? 4 : 0;
+  if (ch == 0) return fail("colour type " + std::to_string(color) + " is not supported (only 0, 2, 4 and 6)");
+  if (interlace != 0) return fail("interlaced images are not supported");
+  if (compression != 0 || filter != 0 || w < 1 || h < 1 || w > (1u << 24) || h > (1u << 24)) return fail("invalid IHDR");
+  std::string raw;
+  io_detail::Inflate inf{reinterpret_cast<const uint8_t*>(idat.data()), idat.size()};
+  inf.out = &raw;
+  if (!inf.zlib()) return fail("broken zlib stream");
+  const size_t stride = static_cast<size_t>(w) * ch;
+  if (raw.size() < (stride + 1) * h) return fail("image data too short");
+  std::vector<uint8_t> prev(stride, 0), cur(stride);
+  grey->assign(static_cast<size_t>(w) * h, 0);
+  for (uint32_t y = 0; y < h; ++y) {
+    const uint8_t* line = reinterpret_cast<const uint8_t*>(raw.data()) + y * (stride + 1);
+    const int ft = line[0];
+    if (ft > 4) return fail("unknown filter type " + std::to_string(ft));
+    for (size_t x = 0; x < stride; ++x) {
+      const int a = x >= static_cast<size_t>(ch) ? cur[x - ch] : 0, b = prev[x];
+      const int c = x >= static_cast<size_t>(ch) ? prev[x - ch] : 0;
+      int p = 0;
+      if (ft == 1) {
+        p = a;
+      } else if (ft == 2) {
+        p = b;
+      } else if (ft == 3) {
+        p = (a + b) >> 1;
+      } else if (ft == 4) {
+        const int pa = std::abs(b - c), pb = std::abs(a - c), pc = std::abs(a + b - 2 * c);
+        p = (pa <= pb && pa <= pc) ? a : (pb <= pc ? b : c);
+      }
+      cur[x] = static_cast<uint8_t>(line[1 + x] + p);
+    }
+    for (uint32_t x = 0; x < w; ++x) {
+      const uint8_t* px = &cur[static_cast<size_t>(x) * ch];
+      uint8_t g = px[0];
+      if (ch >= 3 && !(px[0] == px[1] && px[0] == px[2]))
+        g = static_cast<uint8_t>((6968u * px[0] + 23434u * px[1] + 2366u * px[2]) >> 15);
+      (*grey)[static_cast<size_t>(y) * w + x] = g;
+    }
+    prev.swap(cur);
+  }
+  *width = static_cast<int>(w);
+  *height = static_cast<int>(h);
+  return true;
+}
+
+// DecodePNG of the file at path; false with "Cannot read file: ..." when it cannot be read.
+inline bool ReadPNG(const std::string& path, int* width, int* height, std::vector<uint8_t>* grey, std::string* error) {
+  std::string data;
+  if (!io_detail::read_file(path, &data)) {
+    if (error) *error = "Cannot read file: " + path;
+    return false;
+  }
+  return DecodePNG(data, width, height, grey, error);
 }
 
 }  // namespace b200ba_shim

@@ -1,7 +1,8 @@
 // b200ba_pipeline.hpp -- C++ host logic of the callers either side of the hot path (SURVEY.md 8f-3 / 8f-4):
 // the outlier deletion between bundle-adjustment rounds, the metric rescaling, the pyramid resampling of the generic
 // models, the calibration report's info files, the comparison of two calibrations, the localization accuracy test and
-// the --bundle_adjustment / --compare_reconstructions tools and the calibration visualisation tools, over the containers of
+// the --bundle_adjustment / --compare_reconstructions tools, the calibration visualisation tools and the
+// --render_synthetic_dataset tool, over the containers of
 // b200ba_shim.hpp. (RunBundleAdjustment itself -- 8f-2 -- is in b200ba_shim.hpp and runs device-resident in the
 // library.) The Python mirror is camera_calibration_b200/pipeline.py.
 //
@@ -1155,6 +1156,97 @@ inline int IntersectDatasets(const std::vector<std::string>& dataset_paths, doub
   }
   for (int i = 0; i < n; ++i)
     std::cerr << "Remaining features in dataset " << i << ": " << IntersectFeatureCount(*datasets[i]) << "\n";
+  return EXIT_SUCCESS;
+}
+
+// ---- --render_synthetic_dataset -----------------------------------------------------------------------------------
+// The b200ba_pattern of a pattern file; false when it has more than B200BA_PATTERN_MAX_TAGS tags.
+inline bool PatternStruct(const PatternFile& file, b200ba_pattern* p) {
+  if (file.tags.size() > B200BA_PATTERN_MAX_TAGS) return false;
+  *p = b200ba_pattern{};
+  p->squares_x = file.squares_x;
+  p->squares_y = file.squares_y;
+  p->num_star_segments = file.num_star_segments;
+  p->num_tags = static_cast<int32_t>(file.tags.size());
+  p->page_width_mm = file.page_width_mm;
+  p->page_height_mm = file.page_height_mm;
+  p->pattern_start_x_mm = file.pattern_start_x_mm;
+  p->pattern_start_y_mm = file.pattern_start_y_mm;
+  p->pattern_end_x_mm = file.pattern_end_x_mm;
+  p->pattern_end_y_mm = file.pattern_end_y_mm;
+  for (size_t k = 0; k < file.tags.size(); ++k)
+    p->tags[k] = b200ba_pattern_tag{file.tags[k].x, file.tags[k].y, file.tags[k].width, file.tags[k].height,
+                                    file.tags[k].index};
+  return true;
+}
+
+// tools/render_synthetic_dataset.cc:43-298: a 640 x 480 pinhole camera (fx = fy = 480, cx = 320, cy = 240,
+// pixel-corner convention) views the pattern of pattern_yaml / pattern_png from num_images random poses
+// (b200ba_synthetic_poses, seeded; the reference seeds with the time and reads the pattern from beside its binary);
+// the images are rendered on the device (b200ba_render_pattern_images). Writes <path>/dataset.yaml (the reference's
+// text) and <path>/images0/000000.png ... (WritePNG), printing "Rendering image i ..." to stderr. Returns
+// EXIT_SUCCESS / EXIT_FAILURE with the reference's messages. pipeline.py's RenderSyntheticDataset writes the same
+// bytes.
+inline int RenderSyntheticDataset(const std::string& path,
+                                  const std::string& pattern_yaml = "pattern_resolution_17x24_segments_16_apriltag_0.yaml",
+                                  const std::string& pattern_png = "pattern_resolution_17x24_segments_16_apriltag_0.png",
+                                  int num_images = 500, uint64_t seed = 0, int device = -1) {
+  const int width = 640, height = 480;
+  const float fx = height, fy = height, cx = 0.5 * width, cy = 0.5 * height;
+  const float k[4] = {fx, fy, cx, cy};
+  PatternFile file;
+  if (!LoadPatternYAML(pattern_yaml, &file)) {
+    std::cerr << "Failed to load: " << pattern_yaml << "\n";
+    return EXIT_FAILURE;
+  }
+  int pattern_w = 0, pattern_h = 0;
+  std::vector<uint8_t> pattern_image;
+  std::string error;
+  if (!ReadPNG(pattern_png, &pattern_w, &pattern_h, &pattern_image, &error)) {
+    if (error.rfind("DecodePNG", 0) == 0) std::cerr << error << "\n";
+    std::cerr << "Cannot load the pattern image from: " << pattern_png << "\n";
+    return EXIT_FAILURE;
+  }
+  b200ba_pattern pattern;
+  if (!PatternStruct(file, &pattern)) {
+    std::cerr << "The pattern has more than " << B200BA_PATTERN_MAX_TAGS << " AprilTags, which is not supported.\n";
+    return EXIT_FAILURE;
+  }
+  std::error_code ec;
+  std::filesystem::create_directories(path, ec);
+  const std::string yaml_path = std::filesystem::absolute(std::filesystem::path(path) / "dataset.yaml").string();
+  {
+    std::ofstream yaml(yaml_path, std::ios::out | std::ios::binary);
+    if (!yaml) {
+      std::cerr << "Failed to write dataset YAML file at: " << yaml_path << "\n";
+      return EXIT_FAILURE;
+    }
+    yaml << "- camera: \"Synthetic pinhole camera (fx: " << fx << ", fy: " << fy << ", cx: " << cx << ", cy: " << cy
+         << ", 'pixel corner' coordinate origin convention)\"\n";
+    yaml << "  path: \"images0\"\n";
+  }
+  const std::string images_dir = io_detail::join(path, "images0");
+  std::filesystem::create_directories(images_dir, ec);
+  if (num_images < 1) return EXIT_SUCCESS;
+  std::vector<double> poses(12 * static_cast<size_t>(num_images));
+  if (int rc = b200ba_synthetic_poses(&pattern, pattern_w, pattern_h, width, height, k, num_images, seed, poses.data(),
+                                      nullptr)) {
+    std::cerr << "b200ba_synthetic_poses failed (" << rc << "): " << b200ba_last_error(nullptr) << "\n";
+    return EXIT_FAILURE;
+  }
+  std::vector<uint8_t> images(static_cast<size_t>(num_images) * width * height);
+  if (int rc = b200ba_render_pattern_images(device, &pattern, pattern_image.data(), pattern_w, pattern_h, width, height,
+                                            k, num_images, poses.data(), images.data(), nullptr)) {
+    std::cerr << "b200ba_render_pattern_images failed (" << rc << "): " << b200ba_last_error(nullptr) << "\n";
+    return EXIT_FAILURE;
+  }
+  for (int i = 0; i < num_images; ++i) {
+    std::cerr << "Rendering image " << i << " ...\n";
+    std::ostringstream name;
+    name << std::setw(6) << std::setfill('0') << i << ".png";
+    WritePNG(io_detail::join(images_dir, name.str()), width, height, 1,
+             images.data() + static_cast<size_t>(i) * width * height);
+  }
   return EXIT_SUCCESS;
 }
 

@@ -349,6 +349,73 @@ def RenderPatternImages(pattern, pattern_image, image_size, fx_fy_cx_cy, camera_
     return images, ms.value
 
 
+def _refine_sample_count(window_half_extent: int) -> int:
+    return int(8.0 * (2 * window_half_extent + 1) ** 2 + 0.5)
+
+
+def FeatureSamples(window_half_extent: int = 10):
+    """The reference's sample offsets of feature refinement (``b200ba_feature_samples``: srand(0), then Eigen's
+    Vec2f::Random() per sample from glibc's rand() stream, restated). Returns [n, 2] float32,
+    n = (int)(8 (2h + 1)^2 + 0.5)."""
+    lib = cabi.load_library()
+    n = _refine_sample_count(int(window_half_extent))
+    xy = np.zeros((n, 2), np.float32)
+    _check(lib.b200ba_feature_samples(int(window_half_extent), n, xy.ctypes.data_as(C.POINTER(C.c_float))))
+    return xy
+
+
+def _prediction_records(image, position, pattern_coordinate, local_pixel_tr_pattern):
+    """Packs prediction arrays (image [n], position [n, 2] pixel-centre, pattern_coordinate [n, 2] int,
+    local_pixel_tr_pattern [n, 3, 3]) into a b200ba_feature_prediction array."""
+    img = np.asarray(image, np.int64).reshape(-1)
+    n = len(img)
+    pos = np.asarray(position, np.float32).reshape(n, 2)
+    pc = np.asarray(pattern_coordinate, np.int32).reshape(n, 2)
+    hom = np.asarray(local_pixel_tr_pattern, np.float32).reshape(n, 9)
+    rec = np.zeros(n, dtype=np.dtype([("image", "<i8"), ("position", "<f4", 2), ("pattern_coordinate", "<i4", 2),
+                                      ("local_pixel_tr_pattern", "<f4", 9)], align=True))
+    assert rec.dtype.itemsize == C.sizeof(cabi.FeaturePrediction)
+    rec["image"], rec["position"], rec["pattern_coordinate"], rec["local_pixel_tr_pattern"] = img, pos, pc, hom
+    return rec
+
+
+def RefineFeatures(pattern, images, predictions, refinement_type="intensities", window_half_extent: int = 10,
+                   samples=None, device: int = -1):
+    """Sub-pixel refinement of predicted star-pattern features on the device (``b200ba_refine_features``; the
+    reference's RefineFeatureDetections with its CPU path's arithmetic, specified in include/b200ba.h).
+    pattern: a dict of io.LoadPatternYAML (or a cabi.Pattern); images: grey [n_images, h, w] uint8 (or one [h, w]);
+    predictions: (image [n], position [n, 2], pattern_coordinate [n, 2], local_pixel_tr_pattern [n, 3, 3]) or the
+    array FeaturePredictions returns; refinement_type: a name of cabi.REFINEMENT_TYPES or its number; samples:
+    [n, 2] float32 (default FeatureSamples(window_half_extent)). Returns (positions [n, 2] float32, NaN where
+    rejected; final_cost [n] float32, -1 where rejected; status [n] int32, indices of cabi.REFINE_STATUS;
+    device_ms)."""
+    lib = cabi.load_library()
+    p = _pattern_struct(pattern)
+    ims = np.ascontiguousarray(images, np.uint8)
+    if ims.ndim == 2:
+        ims = ims[None]
+    if ims.ndim != 3:
+        raise ValueError("RefineFeatures: images must be grey [n, h, w] uint8")
+    rec = predictions if isinstance(predictions, np.ndarray) and predictions.dtype.names else \
+        _prediction_records(*predictions)
+    rec = np.ascontiguousarray(rec)
+    t = cabi.REFINEMENT_TYPES[refinement_type] if isinstance(refinement_type, str) else int(refinement_type)
+    s = FeatureSamples(window_half_extent) if samples is None else np.ascontiguousarray(samples, np.float32)
+    n = len(rec)
+    xy = np.zeros((n, 2), np.float32)
+    cost = np.zeros(n, np.float32)
+    status = np.zeros(n, np.int32)
+    ms = C.c_double(0)
+    _check(lib.b200ba_refine_features(device, C.byref(p), _u8p(ims), ims.shape[2], ims.shape[1], ims.shape[0],
+                                      s.ctypes.data_as(C.POINTER(C.c_float)), len(s.reshape(-1, 2)),
+                                      int(window_half_extent), t, n,
+                                      rec.ctypes.data_as(C.POINTER(cabi.FeaturePrediction)),
+                                      xy.ctypes.data_as(C.POINTER(C.c_float)),
+                                      cost.ctypes.data_as(C.POINTER(C.c_float)),
+                                      status.ctypes.data_as(C.POINTER(C.c_int32)), C.byref(ms)))
+    return xy, cost, status, ms.value
+
+
 def nccl_unique_id() -> bytes:
     lib = cabi.load_library()
     buf = (C.c_uint8 * cabi.NCCL_UNIQUE_ID_BYTES)()

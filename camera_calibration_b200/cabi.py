@@ -309,6 +309,19 @@ class Pattern(C.Structure):
     ]
 
 
+class FeaturePrediction(C.Structure):
+    """b200ba_feature_prediction: image index, position (pixel-centre convention), integer pattern coordinate and the
+    row-major local_pixel_tr_pattern of one predicted feature."""
+    _fields_ = [("image", C.c_int64), ("position", C.c_float * 2), ("pattern_coordinate", C.c_int32 * 2),
+                ("local_pixel_tr_pattern", C.c_float * 9)]
+
+
+REFINEMENT_TYPES = {"gradients_xy": 0, "gradient_magnitude": 1, "intensities": 2, "no_refinement": 3}
+REFINE_STATUS = ("accepted", "image_border", "outside_pattern", "match_outside", "match_left_window",
+                 "match_not_converged", "match_bad_factor", "sym_outside", "sym_left_window", "sym_not_converged",
+                 "inconsistent")
+
+
 class FitReport(C.Structure):
     """b200ba_fit_report."""
     _fields_ = [
@@ -510,6 +523,11 @@ SYMBOLS = {
     "b200ba_render_pattern_images": (C.c_int, [C.c_int, C.POINTER(Pattern), C.POINTER(C.c_uint8), C.c_int32,
                                                C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_float), C.c_int64, _D,
                                                C.POINTER(C.c_uint8), _D]),
+    "b200ba_feature_samples": (C.c_int, [C.c_int32, C.c_int32, C.POINTER(C.c_float)]),
+    "b200ba_refine_features": (C.c_int, [C.c_int, C.POINTER(Pattern), C.POINTER(C.c_uint8), C.c_int32, C.c_int32,
+                                         C.c_int64, C.POINTER(C.c_float), C.c_int32, C.c_int32, C.c_int32, C.c_int64,
+                                         C.POINTER(FeaturePrediction), C.POINTER(C.c_float), C.POINTER(C.c_float),
+                                         C.POINTER(C.c_int32), _D]),
     "b200ba_snapshot_state": (C.c_int, [C.c_void_p]),
     "b200ba_restore_state": (C.c_int, [C.c_void_p]),
     "b200ba_version": (C.c_char_p, []),

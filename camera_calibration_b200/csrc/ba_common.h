@@ -4,6 +4,7 @@
 
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <string.h>
 
 #include "../../include/b200ba.h"
 
@@ -226,6 +227,192 @@ __host__ __device__ __forceinline__ uint64_t loc_splitmix64(uint64_t z) {
   z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
   z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
   return z ^ (z >> 31);
+}
+
+// ---- feature refinement (b200ba_refine_features): functions the kernel and tests/refine_features_oracle.cc both
+// compile, so that they agree bit for bit. On the device every operation is an explicit _rn intrinsic (nvcc cannot
+// contract it into a fused multiply-add); the host compiles them with -ffp-contract=off.
+__host__ __device__ __forceinline__ float rf_add(float a, float b) {
+#ifdef __CUDA_ARCH__
+  return __fadd_rn(a, b);
+#else
+  return a + b;
+#endif
+}
+__host__ __device__ __forceinline__ float rf_sub(float a, float b) {
+#ifdef __CUDA_ARCH__
+  return __fsub_rn(a, b);
+#else
+  return a - b;
+#endif
+}
+__host__ __device__ __forceinline__ float rf_mul(float a, float b) {
+#ifdef __CUDA_ARCH__
+  return __fmul_rn(a, b);
+#else
+  return a * b;
+#endif
+}
+__host__ __device__ __forceinline__ float rf_div(float a, float b) {
+#ifdef __CUDA_ARCH__
+  return __fdiv_rn(a, b);
+#else
+  return a / b;
+#endif
+}
+__host__ __device__ __forceinline__ double rd_add(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dadd_rn(a, b);
+#else
+  return a + b;
+#endif
+}
+__host__ __device__ __forceinline__ double rd_sub(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dsub_rn(a, b);
+#else
+  return a - b;
+#endif
+}
+__host__ __device__ __forceinline__ double rd_mul(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dmul_rn(a, b);
+#else
+  return a * b;
+#endif
+}
+__host__ __device__ __forceinline__ double rd_div(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __ddiv_rn(a, b);
+#else
+  return a / b;
+#endif
+}
+
+__host__ __device__ __forceinline__ bool rf_sign_bit(float v) {
+#ifdef __CUDA_ARCH__
+  return __float_as_uint(v) >> 31;
+#else
+  uint32_t u;
+  memcpy(&u, &v, sizeof u);
+  return u >> 31;
+#endif
+}
+
+// atan2 in float (the template's angle, PatternData::PatternIntensityAt). The device's atan2f and the C library's
+// are different functions; this one is the project's own, so the kernel and the restatement agree. With
+// a = min(|x|, |y|) / max(|x|, |y|) and s = a a, atan(a) = a + (a s) q(s) for a degree-7 polynomial q (Horner from
+// the highest coefficient, fitted to the relative error on [0, 1]); then r = pi/2 - r when |y| > |x|, r = pi - r
+// when x < 0, r = -r when y < 0 (sign bits, so -0 counts as negative). max(|x|, |y|) == 0 gives a = 0; NaN
+// propagates. Its error against glibc's atan2f is stated in DESIGN.md section 7.
+__host__ __device__ __forceinline__ float rf_atan2(float y, float x) {
+  const float ax = fabsf(x), ay = fabsf(y);
+  const float mx = ay > ax ? ay : ax, mn = ay > ax ? ax : ay;
+  const float a = mx == 0.f ? 0.f : rf_div(mn, mx);
+  const float s = rf_mul(a, a);
+  float q = 0.00291985273f;
+  q = rf_add(rf_mul(q, s), -0.0163645819f);
+  q = rf_add(rf_mul(q, s), 0.0432064496f);
+  q = rf_add(rf_mul(q, s), -0.0755176023f);
+  q = rf_add(rf_mul(q, s), 0.106657945f);
+  q = rf_add(rf_mul(q, s), -0.142110035f);
+  q = rf_add(rf_mul(q, s), 0.199937671f);
+  q = rf_add(rf_mul(q, s), -0.333331525f);
+  float r = rf_add(a, rf_mul(rf_mul(a, s), q));
+  if (ay > ax) r = rf_sub(1.57079637f, r);
+  if (rf_sign_bit(x)) r = rf_sub(3.14159274f, r);
+  if (rf_sign_bit(y)) r = -r;
+  return r;
+}
+
+// (int)v as x86-64 converts (cvttss2si / cvttsd2si): truncation, INT_MIN outside the int range and for NaN
+__host__ __device__ __forceinline__ int rf_trunc_int(float v) {
+  return (v > -2147483904.f && v < 2147483648.f) ? static_cast<int>(v) : static_cast<int>(0x80000000u);
+}
+__host__ __device__ __forceinline__ int rd_trunc_int(double v) {
+  return (v > -2147483649.0 && v < 2147483648.0) ? static_cast<int>(v) : static_cast<int>(0x80000000u);
+}
+
+// PatternData::PatternIntensityAt (feature_detector_tagged_pattern.h:115-130) with rf_atan2: 1 (white), 0 (black) or
+// 0.5 (on the feature). The integer products wrap as two's complement.
+__host__ __device__ __forceinline__ float rf_pattern_intensity(int num_star_segments, float x, float y) {
+  const int kx = static_cast<int>(static_cast<uint32_t>(x > 0.f ? 1 : -1) *
+                                  static_cast<uint32_t>(rf_trunc_int(rf_add(fabsf(x), 0.5f))));
+  const int ky = static_cast<int>(static_cast<uint32_t>(y > 0.f ? 1 : -1) *
+                                  static_cast<uint32_t>(rf_trunc_int(rf_add(fabsf(y), 0.5f))));
+  const float cx = rf_sub(x, static_cast<float>(kx)), cy = rf_sub(y, static_cast<float>(ky));
+  if (rf_add(rf_mul(cx, cx), rf_mul(cy, cy)) < 1e-8f) return 0.5f;
+  float angle = static_cast<float>(rd_sub(static_cast<double>(rf_atan2(cy, cx)), 0.5 * 3.14159265358979323846));
+  if (angle < 0.f) angle = static_cast<float>(rd_add(static_cast<double>(angle), 2 * 3.14159265358979323846));
+  const double v = rd_div(static_cast<double>(rf_mul(static_cast<float>(num_star_segments), angle)),
+                          2 * 3.14159265358979323846);
+  return rd_trunc_int(v) % 2 == 0 ? 1.f : 0.f;
+}
+
+// The inverse of a row-major 3 x 3 float matrix by the adjugate over the determinant: cofactor
+// c(i, j) = m(i1, j1) m(i2, j2) - m(i1, j2) m(i2, j1) with i1 = (i + 1) % 3, i2 = (i + 2) % 3 (j alike),
+// det = (c(0, 0) m(0, 0) + c(0, 1) m(0, 1)) + c(0, 2) m(0, 2), inv(j, i) = c(i, j) * (1 / det).
+__host__ __device__ __forceinline__ void rf_inverse3(const float* m, float* inv) {
+  float c[9];
+#pragma unroll
+  for (int i = 0; i < 3; ++i)
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+      const int i1 = (i + 1) % 3, i2 = (i + 2) % 3, j1 = (j + 1) % 3, j2 = (j + 2) % 3;
+      c[i * 3 + j] = rf_sub(rf_mul(m[i1 * 3 + j1], m[i2 * 3 + j2]), rf_mul(m[i1 * 3 + j2], m[i2 * 3 + j1]));
+    }
+  const float det = rf_add(rf_add(rf_mul(c[0], m[0]), rf_mul(c[1], m[1])), rf_mul(c[2], m[2]));
+  const float invdet = rf_div(1.f, det);
+#pragma unroll
+  for (int i = 0; i < 3; ++i)
+#pragma unroll
+    for (int j = 0; j < 3; ++j) inv[j * 3 + i] = rf_mul(c[i * 3 + j], invdet);
+}
+
+// Solves (A + lambda I) x = b for a symmetric N x N A given by its packed upper triangle in float (row-major:
+// (0,0), (0,1), ..., (0,N-1), (1,1), ...), all in double, by an LDL^T factorisation without pivoting:
+//   A'_ij = (double)A_ij, plus (double)lambda on the diagonal (the sum rounded to float first, as the float H_LM
+//   of the reference is: A'_ii = (double)(float)(A_ii + lambda));
+//   for j = 0..N-1: d_j = A'_jj - sum_{k<j} (L_jk L_jk) d_k, subtracting k = 0, 1, ... in order;
+//     for i > j: v = A'_ji - sum_{k<j} (L_ik L_jk) d_k, alike, and L_ij = v / d_j when |d_j| > 0, else L_ij = v;
+//   y_i = b_i - sum_{k<i} L_ik y_k (k ascending); z_i = y_i / d_i when |d_i| > DBL_MIN, else z_i = 0;
+//   x_i = z_i - sum_{k>i} L_ki x_k (i descending, k ascending); returned as (float)x_i.
+// A zero (or NaN) pivot is treated as Eigen 3.3's LDLT treats it: the column is not scaled, and the solution
+// component is set to 0 (the pseudo-inverse of D). So A = 0 with lambda = 0, the LM's system in a textureless
+// window, gives x = 0, a step that does not lower the cost.
+template <int N>
+__host__ __device__ __forceinline__ void rf_ldlt_solve(const float* A, float lambda, const float* b, float* x) {
+  double L[N][N], d[N], y[N];
+#pragma unroll
+  for (int j = 0; j < N; ++j) {
+    const int jj = j * N - j * (j - 1) / 2;  // packed index of (j, j)
+    double dj = static_cast<double>(rf_add(A[jj], lambda));
+#pragma unroll
+    for (int k = 0; k < j; ++k) dj = rd_sub(dj, rd_mul(rd_mul(L[j][k], L[j][k]), d[k]));
+    d[j] = dj;
+#pragma unroll
+    for (int i = j + 1; i < N; ++i) {
+      double v = static_cast<double>(A[jj + (i - j)]);
+#pragma unroll
+      for (int k = 0; k < j; ++k) v = rd_sub(v, rd_mul(rd_mul(L[i][k], L[j][k]), d[k]));
+      L[i][j] = fabs(dj) > 0.0 ? rd_div(v, dj) : v;
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < N; ++i) {
+    double v = static_cast<double>(b[i]);
+#pragma unroll
+    for (int k = 0; k < i; ++k) v = rd_sub(v, rd_mul(L[i][k], y[k]));
+    y[i] = v;
+  }
+#pragma unroll
+  for (int i = N - 1; i >= 0; --i) {
+    double v = fabs(d[i]) > 2.2250738585072014e-308 ? rd_div(y[i], d[i]) : 0.0;
+#pragma unroll
+    for (int k = i + 1; k < N; ++k) v = rd_sub(v, rd_mul(L[k][i], y[k]));
+    y[i] = v;
+    x[i] = static_cast<float>(v);
+  }
 }
 
 }  // namespace b200ba

@@ -3527,18 +3527,24 @@ void synth_float_pose(const double* pose, float* out) {
   for (int r = 0; r < 3; ++r) out[21 + r] = static_cast<float>((R[r] * -t[0] + R[3 + r] * -t[1]) + R[6 + r] * -t[2]);
 }
 
-const char* synth_check_pattern(const b200ba_pattern* p, int32_t pattern_w, int32_t pattern_h, int32_t width,
-                                int32_t height, const float* k) {
-  if (!p || !k) return "pattern and fx_fy_cx_cy are required";
-  if (pattern_w < 1 || pattern_h < 1 || width < 1 || height < 1 || pattern_w > 32768 || pattern_h > 32768 ||
-      width > 32768 || height > 32768)
-    return "sizes must lie in [1, 32768]";
+// the checks of a pattern struct that b200ba_render_pattern_images and b200ba_refine_features share
+const char* check_pattern_struct(const b200ba_pattern* p) {
   if (p->num_tags < 0 || p->num_tags > B200BA_PATTERN_MAX_TAGS) return "num_tags must lie in [0, B200BA_PATTERN_MAX_TAGS]";
   if (p->squares_x < 1 || p->squares_y < 1) return "squares_x and squares_y must be at least 1";
   if (p->num_star_segments < 2 || p->num_star_segments % 2 || p->num_star_segments > 1024)
     return "num_star_segments must be even and in [2, 1024]";
   if (int64_t(p->squares_x + 1) * (p->squares_y + 1) * (p->num_star_segments / 2) > (int64_t(1) << 24))
     return "the pattern has more than 2^24 star segments";
+  return nullptr;
+}
+
+const char* synth_check_pattern(const b200ba_pattern* p, int32_t pattern_w, int32_t pattern_h, int32_t width,
+                                int32_t height, const float* k) {
+  if (!p || !k) return "pattern and fx_fy_cx_cy are required";
+  if (pattern_w < 1 || pattern_h < 1 || width < 1 || height < 1 || pattern_w > 32768 || pattern_h > 32768 ||
+      width > 32768 || height > 32768)
+    return "sizes must lie in [1, 32768]";
+  if (const char* e = check_pattern_struct(p)) return e;
   if (!std::isfinite(k[0]) || !std::isfinite(k[1]) || k[0] == 0.f || k[1] == 0.f || !std::isfinite(k[2]) ||
       !std::isfinite(k[3]))
     return "fx and fy must be finite and non-zero, cx and cy finite";
@@ -3668,6 +3674,160 @@ int b200ba_render_pattern_images(int device, const b200ba_pattern* pattern, cons
     cs.ok(cudaGetLastError());
     cs.ok(cudaMemcpy(images + i0 * pixels, d_img, static_cast<size_t>(m) * pixels, cudaMemcpyDeviceToHost));
     if (cs.rc == 0) ms += cs.elapsed_ms(0, 1);
+  }
+  if (cs.rc == 0 && device_ms) *device_ms = ms;
+  return cs.rc;
+}
+
+// ---- feature refinement (RefineFeatureDetections; the arithmetic is specified in include/b200ba.h) ----
+namespace {
+int refine_sample_count(int32_t h) { return static_cast<int>(8.0 * (2 * h + 1) * (2 * h + 1) + 0.5); }
+}  // namespace
+
+int b200ba_feature_samples(int32_t window_half_extent, int32_t n, float* xy) {
+  if (window_half_extent < 1 || window_half_extent > B200BA_REFINE_MAX_HALF_EXTENT || !xy ||
+      n != refine_sample_count(window_half_extent)) {
+    g_create_error = "b200ba_feature_samples: needs 1 <= window_half_extent <= 32, n = (int)(8 (2h + 1)^2 + 0.5) "
+                     "and xy";
+    return 2;
+  }
+  // glibc's random_r, TYPE_3: srandom(1) (srand(0) seeds as 1), then 310 values discarded
+  int32_t r[31];
+  r[0] = 1;
+  for (int i = 1; i < 31; ++i) {
+    const int32_t hi = r[i - 1] / 127773, lo = r[i - 1] % 127773;
+    int32_t word = 16807 * lo - 2836 * hi;
+    if (word < 0) word += 2147483647;
+    r[i] = word;
+  }
+  int f = 3, b = 0;
+  auto next = [&]() {
+    r[f] = static_cast<int32_t>(static_cast<uint32_t>(r[f]) + static_cast<uint32_t>(r[b]));
+    const int32_t v = static_cast<int32_t>(static_cast<uint32_t>(r[f]) >> 1);
+    f = (f + 1) % 31;
+    b = (b + 1) % 31;
+    return v;
+  };
+  for (int i = 0; i < 310; ++i) next();
+  for (int64_t i = 0; i < 2 * static_cast<int64_t>(n); ++i)
+    xy[i] = -1.f + (2.f * static_cast<float>(next())) / static_cast<float>(2147483647);
+  return 0;
+}
+
+int b200ba_refine_features(int device, const b200ba_pattern* pattern, const uint8_t* images, int32_t width,
+                           int32_t height, int64_t n_images, const float* samples, int32_t n_samples,
+                           int32_t window_half_extent, int32_t refinement_type, int64_t n_features,
+                           const b200ba_feature_prediction* predictions, float* xy, float* final_cost,
+                           int32_t* status, double* device_ms) {
+  const char* e = nullptr;
+  if (!pattern || !samples || (n_features > 0 && (!images || !predictions || !xy || !final_cost)))
+    e = "pattern, samples, and for n_features > 0 images, predictions, xy and final_cost are required";
+  else if (width < 1 || height < 1 || width > 32768 || height > 32768)
+    e = "width and height must lie in [1, 32768]";
+  else if (n_images < 0 || n_features < 0)
+    e = "n_images and n_features must not be negative";
+  else if (window_half_extent < 1 || window_half_extent > B200BA_REFINE_MAX_HALF_EXTENT)
+    e = "window_half_extent must lie in [1, B200BA_REFINE_MAX_HALF_EXTENT]";
+  else if (n_samples != refine_sample_count(window_half_extent))
+    e = "n_samples must be (int)(8 (2 window_half_extent + 1)^2 + 0.5)";
+  else if (refinement_type < B200BA_REFINE_GRADIENTS_XY || refinement_type > B200BA_REFINE_NO_REFINEMENT)
+    e = "unknown refinement_type";
+  else
+    e = check_pattern_struct(pattern);
+  for (int64_t i = 0; !e && i < n_features; ++i) {
+    const b200ba_feature_prediction& q = predictions[i];
+    if (q.image < 0 || q.image >= n_images) e = "a prediction's image index lies outside [0, n_images)";
+    for (int k = 0; !e && k < 9; ++k)
+      if (!std::isfinite(q.local_pixel_tr_pattern[k])) e = "a prediction's local_pixel_tr_pattern is not finite";
+  }
+  if (e) {
+    g_create_error = std::string("b200ba_refine_features: ") + e;
+    return 2;
+  }
+  RefineParams rp{};
+  rp.w = width, rp.h = height, rp.half = window_half_extent;
+  rp.n_samples = n_samples;
+  rp.n_match = static_cast<int>((1 / 8.) * n_samples);
+  rp.type = refinement_type;
+  rp.num_star_segments = pattern->num_star_segments;
+  rp.squares_x = pattern->squares_x, rp.squares_y = pattern->squares_y, rp.num_tags = pattern->num_tags;
+  for (int k = 0; k < pattern->num_tags; ++k)
+    rp.tags[k] = make_int4(pattern->tags[k].x, pattern->tags[k].y, pattern->tags[k].width, pattern->tags[k].height);
+  // images per chunk: device memory bounded by about 512 MiB (B200BA_REFINE_CHUNK caps the count)
+  const int64_t pixels = static_cast<int64_t>(width) * height;
+  int64_t chunk = std::max<int64_t>(1, (int64_t(512) << 20) / pixels);
+  if (const char* env = getenv("B200BA_REFINE_CHUNK")) chunk = std::max<int64_t>(1, std::min<int64_t>(chunk, atoll(env)));
+  chunk = std::min<int64_t>(chunk, std::max<int64_t>(n_images, 1));
+  CallScope cs(&g_create_error);
+  if (int rc = cs.use_device(device)) return rc;
+  if (n_features == 0) {
+    if (device_ms) *device_ms = 0.0;
+    return 0;
+  }
+  // the features in image order (stable), so that each chunk's features are contiguous
+  std::vector<int64_t> order(n_features);
+  for (int64_t i = 0; i < n_features; ++i) order[i] = i;
+  std::stable_sort(order.begin(), order.end(),
+                   [&](int64_t a, int64_t b) { return predictions[a].image < predictions[b].image; });
+  // features per launch: at most kMaxLaunch (80 B of device memory each), so any number of features works
+  constexpr int64_t kMaxLaunch = int64_t(1) << 20;
+  int64_t max_per_chunk = 0;
+  for (int64_t lo = 0, i0 = 0; i0 < n_images; i0 += chunk) {
+    int64_t hi = lo;
+    while (hi < n_features && predictions[order[hi]].image < i0 + chunk) ++hi;
+    max_per_chunk = std::max(max_per_chunk, std::min(hi - lo, kMaxLaunch));
+    lo = hi;
+  }
+  uint8_t* d_img = nullptr;
+  float2* d_samples = nullptr;
+  b200ba_feature_prediction* d_pred = nullptr;
+  float2* d_xy = nullptr;
+  float* d_cost = nullptr;
+  int* d_status = nullptr;
+  cs.alloc(&d_img, static_cast<size_t>(chunk) * pixels);
+  cs.alloc(&d_samples, static_cast<size_t>(n_samples));
+  cs.alloc(&d_pred, static_cast<size_t>(max_per_chunk));
+  cs.alloc(&d_xy, static_cast<size_t>(max_per_chunk));
+  cs.alloc(&d_cost, static_cast<size_t>(max_per_chunk));
+  cs.alloc(&d_status, static_cast<size_t>(max_per_chunk));
+  if (cs.rc == 0) cs.ok(cudaMemcpy(d_samples, samples, sizeof(float2) * n_samples, cudaMemcpyHostToDevice));
+  std::vector<b200ba_feature_prediction> pred(max_per_chunk);
+  std::vector<float2> out_xy(max_per_chunk);
+  std::vector<float> out_cost(max_per_chunk);
+  std::vector<int> out_status(max_per_chunk);
+  double ms = 0.0;
+  for (int64_t lo = 0, i0 = 0; i0 < n_images && cs.rc == 0; i0 += chunk) {
+    const int64_t m_img = std::min<int64_t>(chunk, n_images - i0);
+    int64_t hi = lo;
+    while (hi < n_features && predictions[order[hi]].image < i0 + m_img) ++hi;
+    if (hi == lo) continue;
+    cs.ok(cudaMemcpy(d_img, images + i0 * pixels, static_cast<size_t>(m_img) * pixels, cudaMemcpyHostToDevice));
+    for (; lo < hi && cs.rc == 0; lo += kMaxLaunch) {
+      const int64_t m = std::min(hi - lo, kMaxLaunch);
+      for (int64_t k = 0; k < m; ++k) {
+        pred[k] = predictions[order[lo + k]];
+        pred[k].image -= i0;
+      }
+      cs.ok(cudaMemcpy(d_pred, pred.data(), sizeof(b200ba_feature_prediction) * m, cudaMemcpyHostToDevice));
+      if (cs.rc != 0) break;
+      cs.record(0, 0);
+      launch_refine_features(rp, m, d_pred, d_img, d_samples, d_xy, d_cost, d_status, 0);
+      cs.record(1, 0);
+      cs.ok(cudaGetLastError());
+      if (cs.rc == 0) cs.ok(cudaMemcpy(out_xy.data(), d_xy, sizeof(float2) * m, cudaMemcpyDeviceToHost));
+      if (cs.rc == 0) cs.ok(cudaMemcpy(out_cost.data(), d_cost, sizeof(float) * m, cudaMemcpyDeviceToHost));
+      if (cs.rc == 0) cs.ok(cudaMemcpy(out_status.data(), d_status, sizeof(int) * m, cudaMemcpyDeviceToHost));
+      if (cs.rc != 0) break;
+      ms += cs.elapsed_ms(0, 1);
+      for (int64_t k = 0; k < m; ++k) {
+        const int64_t i = order[lo + k];
+        xy[2 * i] = out_xy[k].x;
+        xy[2 * i + 1] = out_xy[k].y;
+        final_cost[i] = out_cost[k];
+        if (status) status[i] = out_status[k];
+      }
+    }
+    lo = hi;
   }
   if (cs.rc == 0 && device_ms) *device_ms = ms;
   return cs.rc;

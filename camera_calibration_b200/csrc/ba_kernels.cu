@@ -4369,4 +4369,516 @@ void launch_render_pattern(const SynthParams& p, int n_img, const float2* verts,
       p, poses, nv, proj, range, bits, pattern, images);
 }
 
+// ------------------------------------------------------------------------------------------
+// sub-pixel refinement of star-pattern features (feature_detector_tagged_pattern.cc:1427-1648 with the CPU path of
+// cpu_refinement_by_matching.h and cpu_refinement_by_symmetry.h; the arithmetic is specified in include/b200ba.h).
+// One warp per feature: lane l takes samples l, l + 32, ... in order and the sums are combined by an xor butterfly,
+// so every lane holds the same bits and every LM decision is warp-uniform. The arithmetic goes through the _rn
+// helpers of ba_common.h, which tests/refine_features_oracle.cc compiles too; nothing is contracted.
+// ------------------------------------------------------------------------------------------
+constexpr int kRefineWarps = 4;
+
+__device__ __forceinline__ float refine_warp_sum(float v) {
+#pragma unroll
+  for (int o = 16; o; o >>= 1) v = rf_add(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
+// Image::ContainsPixelCenterConv
+__device__ __forceinline__ bool refine_inside(const RefineParams& p, float x, float y) {
+  return x >= 0.f && y >= 0.f && x < static_cast<float>(p.w - 1) && y < static_cast<float>(p.h - 1);
+}
+
+// hnorm(M (x, y, 1)), rows ((m0 x + m1 y) + m2)
+__device__ __forceinline__ float2 refine_hnorm(const float* m, float x, float y) {
+  const float u = rf_add(rf_add(rf_mul(m[0], x), rf_mul(m[1], y)), m[2]);
+  const float v = rf_add(rf_add(rf_mul(m[3], x), rf_mul(m[4], y)), m[5]);
+  const float w = rf_add(rf_add(rf_mul(m[6], x), rf_mul(m[7], y)), m[8]);
+  return make_float2(rf_div(u, w), rf_div(v, w));
+}
+
+// PatternData::IsValidPatternCoord
+__device__ __forceinline__ bool refine_valid_pattern(const RefineParams& p, float x, float y) {
+  if (!(x >= -1.f && y >= -1.f && x <= rf_sub(static_cast<float>(p.squares_x), 1.f) &&
+        y <= rf_sub(static_cast<float>(p.squares_y), 1.f)))
+    return false;
+  for (int k = 0; k < p.num_tags; ++k) {
+    const int4 t = p.tags[k];
+    if (x >= static_cast<float>(t.x - 1) && y >= static_cast<float>(t.y - 1) &&
+        x <= static_cast<float>(t.x - 1 + t.z) && y <= static_cast<float>(t.y - 1 + t.w))
+      return false;
+  }
+  return true;
+}
+
+// the gradient image's pixel (x, y) (feature_detector_tagged_pattern.cc:273-287), from the u8 bytes
+__device__ __forceinline__ float2 refine_gradient(const uint8_t* __restrict__ im, int w, int h, int x, int y) {
+  const int mx = max(0, x - 1), px = min(w - 1, x + 1), my = max(0, y - 1), py = min(h - 1, y + 1);
+  const uint8_t* row = im + static_cast<int64_t>(y) * w;
+  const float dx = rf_div(rf_sub(static_cast<float>(__ldg(row + px)), static_cast<float>(__ldg(row + mx))),
+                          static_cast<float>(px - mx));
+  const float dy = rf_div(rf_sub(static_cast<float>(__ldg(im + static_cast<int64_t>(py) * w + x)),
+                                 static_cast<float>(__ldg(im + static_cast<int64_t>(my) * w + x))),
+                          static_cast<float>(py - my));
+  return make_float2(dx, dy);
+}
+
+// the four corners (x, y), (x + 1, y), (x, y + 1), (x + 1, y + 1) of channel 0 (and 1) of the image of kType:
+// the u8 image (INTENSITIES, and matching), the gradient magnitude or the gradient (GRADIENTS_XY)
+template <int kType>
+__device__ __forceinline__ void refine_corners(const uint8_t* __restrict__ im, const RefineParams& p, int x, int y,
+                                               float* c0, float* c1) {
+  if (kType == B200BA_REFINE_INTENSITIES) {
+    const uint8_t* row = im + static_cast<int64_t>(y) * p.w + x;
+    c0[0] = __ldg(row);
+    c0[1] = __ldg(row + 1);
+    c0[2] = __ldg(row + p.w);
+    c0[3] = __ldg(row + p.w + 1);
+  } else {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const float2 g = refine_gradient(im, p.w, p.h, x + (k & 1), y + (k >> 1));
+      if (kType == B200BA_REFINE_GRADIENT_MAGNITUDE) {
+        c0[k] = __fsqrt_rn(rf_add(rf_mul(g.x, g.x), rf_mul(g.y, g.y)));
+      } else {
+        c0[k] = g.x;
+        c1[k] = g.y;
+      }
+    }
+  }
+}
+
+// InterpolateBilinear: (((gx gy) c00 + (fx gy) c10) + (gx fy) c01) + (fx fy) c11
+__device__ __forceinline__ float refine_value(float fx, float fy, const float* c) {
+  const float gx = rf_sub(1.f, fx), gy = rf_sub(1.f, fy);
+  return rf_add(rf_add(rf_add(rf_mul(rf_mul(gx, gy), c[0]), rf_mul(rf_mul(fx, gy), c[1])),
+                       rf_mul(rf_mul(gx, fy), c[2])),
+                rf_mul(rf_mul(fx, fy), c[3]));
+}
+
+// InterpolateBilinearWithJacobian: the value and (d/dx, d/dy)
+__device__ __forceinline__ float refine_value_jac(float fx, float fy, const float* c, float* dx, float* dy) {
+  const float gx = rf_sub(1.f, fx), gy = rf_sub(1.f, fy);
+  const float top = rf_add(rf_mul(gx, c[0]), rf_mul(fx, c[1]));
+  const float bottom = rf_add(rf_mul(gx, c[2]), rf_mul(fx, c[3]));
+  *dx = rf_add(rf_mul(fy, rf_sub(c[3], c[2])), rf_mul(gy, rf_sub(c[1], c[0])));
+  *dy = rf_sub(bottom, top);
+  return rf_add(rf_mul(gy, top), rf_mul(fy, bottom));
+}
+
+// matching: the sum of squared residuals at (x, y, factor, bias); false when a sample leaves the image
+__device__ __forceinline__ bool refine_match_cost(const RefineParams& p, const uint8_t* __restrict__ im,
+                                                  const float2* __restrict__ samples, const float* tmpl, int lane,
+                                                  float x, float y, float factor, float bias, float* cost) {
+  const float h = static_cast<float>(p.half);
+  float c = 0.f;
+  bool out = false;
+  for (int i = lane; i < p.n_match; i += 32) {
+    const float2 s = __ldg(samples + i);
+    const float sx = rf_add(x, rf_mul(h, s.x)), sy = rf_add(y, rf_mul(h, s.y));
+    if (!refine_inside(p, sx, sy)) {
+      out = true;
+      break;
+    }
+    const int ix = static_cast<int>(sx), iy = static_cast<int>(sy);
+    float cr[4];
+    refine_corners<B200BA_REFINE_INTENSITIES>(im, p, ix, iy, cr, nullptr);
+    const float v = refine_value(rf_sub(sx, static_cast<float>(ix)), rf_sub(sy, static_cast<float>(iy)), cr);
+    const float r = rf_sub(rf_add(rf_mul(factor, v), bias), tmpl[i]);
+    c = rf_add(c, rf_mul(r, r));
+  }
+  if (__any_sync(0xffffffffu, out)) return false;
+  *cost = refine_warp_sum(c);
+  return true;
+}
+
+// symmetry: the pixel positions of +-t under P
+__device__ __forceinline__ void refine_sym_positions(const float* P, float tx, float ty, float2* a, float2* b) {
+  *a = refine_hnorm(P, tx, ty);
+  *b = refine_hnorm(P, -tx, -ty);
+}
+
+// d hnorm(P (t, 1)) / d(P00 P01 P02 P10 P11 P12 P20 P21) (cpu_refinement_by_symmetry.h:334-353), rows D[0..7], D[8..15]
+__device__ __forceinline__ void refine_dpos(const float* P, float tx, float ty, float* D) {
+  const float e0 = rf_div(1.f, rf_add(rf_add(rf_mul(P[6], tx), rf_mul(P[7], ty)), 1.f));
+  const float e1 = rf_mul(rf_mul(-1.f, e0), e0);
+  const float e2 = rf_mul(rf_add(rf_add(rf_mul(P[0], tx), rf_mul(P[1], ty)), P[2]), e1);
+  const float e3 = rf_mul(rf_add(rf_add(rf_mul(P[3], tx), rf_mul(P[4], ty)), P[5]), e1);
+  D[0] = rf_mul(tx, e0), D[1] = rf_mul(ty, e0), D[2] = e0, D[3] = 0.f, D[4] = 0.f, D[5] = 0.f;
+  D[6] = rf_mul(tx, e2), D[7] = rf_mul(ty, e2);
+  D[8] = 0.f, D[9] = 0.f, D[10] = 0.f, D[11] = D[0], D[12] = D[1], D[13] = D[2];
+  D[14] = rf_mul(tx, e3), D[15] = rf_mul(ty, e3);
+}
+
+// symmetry: the pattern-space sample t_i = hnorm(M ((float)h s_i, 1))
+__device__ __forceinline__ float2 refine_pattern_sample(const float* M, float h, float2 s) {
+  return refine_hnorm(M, rf_mul(h, s.x), rf_mul(h, s.y));
+}
+
+// symmetry: the cost at P (ComputeCornerRefinementCost); false when a sample leaves the image
+template <int kType>
+__device__ __forceinline__ bool refine_sym_cost(const RefineParams& p, const uint8_t* __restrict__ im,
+                                                const float2* __restrict__ samples, const float* M, const float* P,
+                                                int lane, float* cost) {
+  const float h = static_cast<float>(p.half);
+  float c = 0.f;
+  bool out = false;
+  for (int i = lane; i < p.n_samples; i += 32) {
+    const float2 t = refine_pattern_sample(M, h, __ldg(samples + i));
+    float2 pa, pb;
+    refine_sym_positions(P, t.x, t.y, &pa, &pb);
+    if (!refine_inside(p, pa.x, pa.y) || !refine_inside(p, pb.x, pb.y)) {
+      out = true;
+      break;
+    }
+    float a0[4], a1[4], b0[4], b1[4];
+    const int ax = static_cast<int>(pa.x), ay = static_cast<int>(pa.y);
+    const int bx = static_cast<int>(pb.x), by = static_cast<int>(pb.y);
+    refine_corners<kType>(im, p, ax, ay, a0, a1);
+    refine_corners<kType>(im, p, bx, by, b0, b1);
+    const float fax = rf_sub(pa.x, static_cast<float>(ax)), fay = rf_sub(pa.y, static_cast<float>(ay));
+    const float fbx = rf_sub(pb.x, static_cast<float>(bx)), fby = rf_sub(pb.y, static_cast<float>(by));
+    if (kType == B200BA_REFINE_GRADIENTS_XY) {
+      const float r0 = rf_add(refine_value(fax, fay, a0), refine_value(fbx, fby, b0));
+      const float r1 = rf_add(refine_value(fax, fay, a1), refine_value(fbx, fby, b1));
+      c = rf_add(c, rf_add(rf_mul(r0, r0), rf_mul(r1, r1)));
+    } else {
+      const float r = rf_sub(refine_value(fax, fay, a0), refine_value(fbx, fby, b0));
+      c = rf_add(c, rf_mul(r, r));
+    }
+  }
+  if (__any_sync(0xffffffffu, out)) return false;
+  *cost = refine_warp_sum(c);
+  return true;
+}
+
+// symmetry: H (packed upper 8 x 8, 36), b (8) and the cost at P (ComputeCornerRefinementCostAndJacobian)
+template <int kType>
+__device__ __forceinline__ bool refine_sym_system(const RefineParams& p, const uint8_t* __restrict__ im,
+                                                  const float2* __restrict__ samples, const float* M, const float* P,
+                                                  int lane, float* H, float* b, float* cost) {
+  const float h = static_cast<float>(p.half);
+#pragma unroll
+  for (int k = 0; k < 36; ++k) H[k] = 0.f;
+#pragma unroll
+  for (int k = 0; k < 8; ++k) b[k] = 0.f;
+  float c = 0.f;
+  bool out = false;
+  for (int i = lane; i < p.n_samples; i += 32) {
+    const float2 t = refine_pattern_sample(M, h, __ldg(samples + i));
+    float2 pa, pb;
+    refine_sym_positions(P, t.x, t.y, &pa, &pb);
+    if (!refine_inside(p, pa.x, pa.y) || !refine_inside(p, pb.x, pb.y)) {
+      out = true;
+      break;
+    }
+    float a0[4], a1[4], b0[4], b1[4];
+    const int ax = static_cast<int>(pa.x), ay = static_cast<int>(pa.y);
+    const int bx = static_cast<int>(pb.x), by = static_cast<int>(pb.y);
+    refine_corners<kType>(im, p, ax, ay, a0, a1);
+    refine_corners<kType>(im, p, bx, by, b0, b1);
+    const float fax = rf_sub(pa.x, static_cast<float>(ax)), fay = rf_sub(pa.y, static_cast<float>(ay));
+    const float fbx = rf_sub(pb.x, static_cast<float>(bx)), fby = rf_sub(pb.y, static_cast<float>(by));
+    float Da[16], Db[16];
+    refine_dpos(P, t.x, t.y, Da);
+    refine_dpos(P, -t.x, -t.y, Db);
+    if (kType == B200BA_REFINE_GRADIENTS_XY) {
+      float ga[4], gb[4];  // (channel 0 d/dx, d/dy, channel 1 d/dx, d/dy)
+      const float va0 = refine_value_jac(fax, fay, a0, &ga[0], &ga[1]);
+      const float va1 = refine_value_jac(fax, fay, a1, &ga[2], &ga[3]);
+      const float vb0 = refine_value_jac(fbx, fby, b0, &gb[0], &gb[1]);
+      const float vb1 = refine_value_jac(fbx, fby, b1, &gb[2], &gb[3]);
+      const float r[2] = {rf_add(va0, vb0), rf_add(va1, vb1)};
+#pragma unroll
+      for (int row = 0; row < 2; ++row) {
+        float J[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k)
+          J[k] = rf_add(rf_add(rf_mul(ga[2 * row], Da[k]), rf_mul(ga[2 * row + 1], Da[8 + k])),
+                        rf_add(rf_mul(gb[2 * row], Db[k]), rf_mul(gb[2 * row + 1], Db[8 + k])));
+        int q = 0;
+#pragma unroll
+        for (int u = 0; u < 8; ++u)
+#pragma unroll
+          for (int v = u; v < 8; ++v, ++q) H[q] = rf_add(H[q], rf_mul(J[u], J[v]));
+#pragma unroll
+        for (int u = 0; u < 8; ++u) b[u] = rf_add(b[u], rf_mul(r[row], J[u]));
+      }
+      c = rf_add(c, rf_add(rf_mul(r[0], r[0]), rf_mul(r[1], r[1])));
+    } else {
+      float gax, gay, gbx, gby;
+      const float va = refine_value_jac(fax, fay, a0, &gax, &gay);
+      const float vb = refine_value_jac(fbx, fby, b0, &gbx, &gby);
+      const float r = rf_sub(va, vb);
+      float J[8];
+#pragma unroll
+      for (int k = 0; k < 8; ++k)
+        J[k] = rf_sub(rf_add(rf_mul(gax, Da[k]), rf_mul(gay, Da[8 + k])),
+                      rf_add(rf_mul(gbx, Db[k]), rf_mul(gby, Db[8 + k])));
+      int q = 0;
+#pragma unroll
+      for (int u = 0; u < 8; ++u)
+#pragma unroll
+        for (int v = u; v < 8; ++v, ++q) H[q] = rf_add(H[q], rf_mul(J[u], J[v]));
+#pragma unroll
+      for (int u = 0; u < 8; ++u) b[u] = rf_add(b[u], rf_mul(r, J[u]));
+      c = rf_add(c, rf_mul(r, r));
+    }
+  }
+  if (__any_sync(0xffffffffu, out)) return false;
+#pragma unroll
+  for (int k = 0; k < 36; ++k) H[k] = refine_warp_sum(H[k]);
+#pragma unroll
+  for (int k = 0; k < 8; ++k) b[k] = refine_warp_sum(b[k]);
+  *cost = refine_warp_sum(c);
+  return true;
+}
+
+// RefineFeatureBySymmetry from the matching result m; returns the status and sets *pos and *final_cost
+template <int kType>
+__device__ __forceinline__ int refine_symmetry(const RefineParams& p, const uint8_t* __restrict__ im,
+                                            const float2* __restrict__ samples, const float* M, const float* L,
+                                            float mx, float my, float2* pos, float* final_cost) {
+  const int lane = threadIdx.x & 31;
+  float P[9];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    P[c] = rf_add(rf_add(rf_mul(1.f, L[c]), rf_mul(0.f, L[3 + c])), rf_mul(mx, L[6 + c]));
+    P[3 + c] = rf_add(rf_add(rf_mul(0.f, L[c]), rf_mul(1.f, L[3 + c])), rf_mul(my, L[6 + c]));
+    P[6 + c] = rf_add(rf_add(rf_mul(0.f, L[c]), rf_mul(0.f, L[3 + c])), rf_mul(1.f, L[6 + c]));
+  }
+  const float p22 = P[8];
+#pragma unroll
+  for (int k = 0; k < 9; ++k) P[k] = rf_div(P[k], p22);
+  const float h = static_cast<float>(p.half);
+  float lambda = -1.f, last = __int_as_float(0x7f800000), cost = 0.f;
+  *pos = make_float2(mx, my);
+  for (int iteration = 0; iteration < 30; ++iteration) {
+    float H[36], b[8];
+    if (!refine_sym_system<kType>(p, im, samples, M, P, lane, H, b, &cost)) return B200BA_REFINE_SYM_OUTSIDE;
+    if (lambda < 0.f) {
+      float d = H[0];
+      for (int k = 1, q = 8; k < 8; q += 8 - k, ++k) d = rf_add(d, H[q]);
+      lambda = rf_mul(rf_mul(0.001f, rf_div(1.f, 8.f)), d);
+    }
+    bool applied = false;
+    for (int attempt = 0; attempt < 10; ++attempt) {
+      float x[8];
+      rf_ldlt_solve<8>(H, lambda, b, x);
+      float T[9];
+#pragma unroll
+      for (int k = 0; k < 8; ++k) T[k] = rf_sub(P[k], x[k]);
+      T[8] = P[8];
+      float test_cost;
+      if (!refine_sym_cost<kType>(p, im, samples, M, T, lane, &test_cost)) return B200BA_REFINE_SYM_OUTSIDE;
+      if (test_cost < cost) {
+        cost = test_cost;
+        last = rf_add(rf_mul(x[2], x[2]), rf_mul(x[5], x[5]));
+#pragma unroll
+        for (int k = 0; k < 9; ++k) P[k] = T[k];
+        lambda = rf_mul(lambda, 0.5f);
+        applied = true;
+        break;
+      }
+      lambda = rf_mul(lambda, 2.f);
+    }
+    *final_cost = cost;
+    if (!applied) return B200BA_REFINE_ACCEPTED;
+    *pos = make_float2(P[2], P[5]);
+    if (fabsf(rf_sub(mx, P[2])) >= h || fabsf(rf_sub(my, P[5])) >= h) return B200BA_REFINE_SYM_LEFT_WINDOW;
+  }
+  return last < 1e-4f ? B200BA_REFINE_ACCEPTED : B200BA_REFINE_SYM_NOT_CONVERGED;
+}
+
+// kType: the refinement type (B200BA_REFINE_*)
+template <int kType>
+__global__ void __launch_bounds__(kRefineWarps * 32)
+refine_features_kernel(RefineParams p, int64_t n, const b200ba_feature_prediction* __restrict__ pred,
+                       const uint8_t* __restrict__ images, const float2* __restrict__ samples, float2* xy,
+                       float* cost_out, int* status_out) {
+  extern __shared__ float refine_templates[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t f = static_cast<int64_t>(blockIdx.x) * kRefineWarps + warp;
+  if (f >= n) return;
+  float* tmpl = refine_templates + warp * p.n_match;
+  const b200ba_feature_prediction& pr = pred[f];
+  const uint8_t* im = images + pr.image * static_cast<int64_t>(p.w) * p.h;
+  const float h = static_cast<float>(p.half);
+  const float x0 = pr.position[0], y0 = pr.position[1];
+  float L[9], M[9];
+#pragma unroll
+  for (int k = 0; k < 9; ++k) L[k] = pr.local_pixel_tr_pattern[k];
+  rf_inverse3(L, M);
+  int st = B200BA_REFINE_ACCEPTED;
+  float final_cost = 0.f;
+  float2 pos = make_float2(x0, y0);
+  // pre-filter (:1443-1479)
+  if (!(rf_sub(x0, h) >= 0.f && rf_sub(y0, h) >= 0.f && rf_add(x0, h) < static_cast<float>(p.w - 1) &&
+        rf_add(y0, h) < static_cast<float>(p.h - 1))) {
+    st = B200BA_REFINE_IMAGE_BORDER;
+  } else {
+    for (int corner = 0; corner < 4; ++corner) {
+      const float2 o = refine_hnorm(M, corner % 2 == 0 ? h : -h, corner / 2 == 0 ? h : -h);
+      if (!refine_valid_pattern(p, rf_add(static_cast<float>(pr.pattern_coordinate[0]), o.x),
+                                rf_add(static_cast<float>(pr.pattern_coordinate[1]), o.y))) {
+        st = B200BA_REFINE_OUTSIDE_PATTERN;
+        break;
+      }
+    }
+  }
+  float mx = x0, my = y0;
+  if (st == B200BA_REFINE_ACCEPTED) {
+    // the template (cpu_refinement_by_matching.h:247-261)
+    for (int i = lane; i < p.n_match; i += 32) {
+      const float2 s = __ldg(samples + i);
+      const float ox = rf_mul(h, s.x), oy = rf_mul(h, s.y);
+      float sum = 0.f;
+      for (int k = 0; k < 16; ++k) {
+        const float2 q = refine_hnorm(M, rf_add(ox, -0.375f + 0.25f * (k % 4)), rf_add(oy, -0.375f + 0.25f * (k / 4)));
+        sum = rf_add(sum, rf_pattern_intensity(p.num_star_segments, q.x, q.y));
+      }
+      tmpl[i] = sum;
+    }
+    __syncwarp();
+    // factor and bias (:76-114)
+    float s_qp = 0.f, s_p = 0.f, s_q = 0.f, s_pp = 0.f;
+    bool out = false;
+    for (int i = lane; i < p.n_match; i += 32) {
+      const float2 s = __ldg(samples + i);
+      const float sx = rf_add(x0, rf_mul(h, s.x)), sy = rf_add(y0, rf_mul(h, s.y));
+      if (!refine_inside(p, sx, sy)) {
+        out = true;
+        break;
+      }
+      const int ix = static_cast<int>(sx), iy = static_cast<int>(sy);
+      float cr[4];
+      refine_corners<B200BA_REFINE_INTENSITIES>(im, p, ix, iy, cr, nullptr);
+      const float v = refine_value(rf_sub(sx, static_cast<float>(ix)), rf_sub(sy, static_cast<float>(iy)), cr);
+      const float q = tmpl[i];
+      s_qp = rf_add(s_qp, rf_mul(q, v));
+      s_p = rf_add(s_p, v);
+      s_q = rf_add(s_q, q);
+      s_pp = rf_add(s_pp, rf_mul(v, v));
+    }
+    if (__any_sync(0xffffffffu, out)) st = B200BA_REFINE_MATCH_OUTSIDE;
+    s_qp = refine_warp_sum(s_qp);
+    s_p = refine_warp_sum(s_p);
+    s_q = refine_warp_sum(s_q);
+    s_pp = refine_warp_sum(s_pp);
+    const float nm = static_cast<float>(p.n_match);
+    const float den = rf_sub(s_pp, rf_div(rf_mul(s_p, s_p), nm));
+    float factor = fabsf(den) > 1e-6f ? rf_div(rf_sub(s_qp, rf_mul(rf_div(s_p, nm), s_q)), den) : 1.f;
+    float bias = rf_mul(rf_div(1.f, nm), rf_sub(s_q, rf_mul(factor, s_p)));
+    // LM on (x, y, factor, bias) (:306-417)
+    float lambda = -1.f, last = __int_as_float(0x7f800000);
+    bool converged = false;
+    for (int iteration = 0; iteration < 50 && st == B200BA_REFINE_ACCEPTED; ++iteration) {
+      float H[10], b[4], cost = 0.f;
+#pragma unroll
+      for (int k = 0; k < 10; ++k) H[k] = 0.f;
+#pragma unroll
+      for (int k = 0; k < 4; ++k) b[k] = 0.f;
+      for (int i = lane; i < p.n_match; i += 32) {
+        const float2 s = __ldg(samples + i);
+        const float sx = rf_add(mx, rf_mul(h, s.x)), sy = rf_add(my, rf_mul(h, s.y));
+        if (!refine_inside(p, sx, sy)) {
+          out = true;
+          break;
+        }
+        const int ix = static_cast<int>(sx), iy = static_cast<int>(sy);
+        float cr[4], gx, gy;
+        refine_corners<B200BA_REFINE_INTENSITIES>(im, p, ix, iy, cr, nullptr);
+        const float v = refine_value_jac(rf_sub(sx, static_cast<float>(ix)), rf_sub(sy, static_cast<float>(iy)), cr,
+                                         &gx, &gy);
+        const float r = rf_sub(rf_add(rf_mul(factor, v), bias), tmpl[i]);
+        const float J[4] = {rf_mul(factor, gx), rf_mul(factor, gy), v, 1.f};
+        int q = 0;
+#pragma unroll
+        for (int u = 0; u < 4; ++u)
+#pragma unroll
+          for (int w = u; w < 4; ++w, ++q) H[q] = rf_add(H[q], rf_mul(J[u], J[w]));
+#pragma unroll
+        for (int u = 0; u < 4; ++u) b[u] = rf_add(b[u], rf_mul(r, J[u]));
+        cost = rf_add(cost, rf_mul(r, r));
+      }
+      if (__any_sync(0xffffffffu, out)) {
+        st = B200BA_REFINE_MATCH_OUTSIDE;
+        break;
+      }
+#pragma unroll
+      for (int k = 0; k < 10; ++k) H[k] = refine_warp_sum(H[k]);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) b[k] = refine_warp_sum(b[k]);
+      cost = refine_warp_sum(cost);
+      if (lambda < 0.f) lambda = rf_mul(rf_mul(0.001f, 0.5f), rf_add(rf_add(rf_add(H[0], H[4]), H[7]), H[9]));
+      bool applied = false;
+      for (int attempt = 0; attempt < 10; ++attempt) {
+        float x[4];
+        rf_ldlt_solve<4>(H, lambda, b, x);
+        const float tx = rf_sub(mx, x[0]), ty = rf_sub(my, x[1]);
+        const float tf = rf_sub(factor, x[2]), tb = rf_sub(bias, x[3]);
+        float test_cost;
+        if (!refine_match_cost(p, im, samples, tmpl, lane, tx, ty, tf, tb, &test_cost)) {
+          st = B200BA_REFINE_MATCH_OUTSIDE;
+          break;
+        }
+        if (test_cost < cost) {
+          last = rf_add(rf_add(rf_add(rf_mul(x[0], x[0]), rf_mul(x[1], x[1])), rf_mul(x[2], x[2])),
+                        rf_mul(x[3], x[3]));
+          mx = tx, my = ty, factor = tf, bias = tb;
+          lambda = rf_mul(lambda, 0.5f);
+          applied = true;
+          break;
+        }
+        lambda = rf_mul(lambda, 2.f);
+      }
+      if (st != B200BA_REFINE_ACCEPTED) break;
+      if (!applied) {
+        converged = true;
+        break;
+      }
+      if (fabsf(rf_sub(x0, mx)) >= h || fabsf(rf_sub(y0, my)) >= h) st = B200BA_REFINE_MATCH_LEFT_WINDOW;
+    }
+    if (st == B200BA_REFINE_ACCEPTED) {
+      if (static_cast<double>(last) < 1e-8) converged = true;
+      if (!converged)
+        st = B200BA_REFINE_MATCH_NOT_CONVERGED;
+      else if (factor <= 0.f)
+        st = B200BA_REFINE_MATCH_BAD_FACTOR;
+    }
+    pos = make_float2(mx, my);
+  }
+  if (kType != B200BA_REFINE_NO_REFINEMENT && st == B200BA_REFINE_ACCEPTED) {
+    st = refine_symmetry<kType>(p, im, samples, M, L, mx, my, &pos, &final_cost);
+    // :1626-1647
+    const float dx = rf_sub(pos.x, mx), dy = rf_sub(pos.y, my);
+    if (st == B200BA_REFINE_ACCEPTED && rf_add(rf_mul(dx, dx), rf_mul(dy, dy)) > 0.75f) st = B200BA_REFINE_INCONSISTENT;
+  }
+  if (lane == 0) {
+    const bool ok = st == B200BA_REFINE_ACCEPTED;
+    xy[f] = ok ? pos : make_float2(__int_as_float(0x7fc00000), __int_as_float(0x7fc00000));
+    cost_out[f] = ok ? final_cost : -1.f;
+    status_out[f] = st;
+  }
+}
+
+void launch_refine_features(const RefineParams& p, int64_t n, const b200ba_feature_prediction* pred,
+                            const uint8_t* images, const float2* samples, float2* xy, float* cost, int* status,
+                            cudaStream_t s) {
+  if (n == 0) return;
+  const size_t smem = sizeof(float) * kRefineWarps * p.n_match;
+  const unsigned blocks = static_cast<unsigned>((n + kRefineWarps - 1) / kRefineWarps);
+  auto run = [&](auto kernel) {
+    if (smem > 48 * 1024)
+      cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+    kernel<<<blocks, kRefineWarps * 32, smem, s>>>(p, n, pred, images, samples, xy, cost, status);
+  };
+  switch (p.type) {
+    case B200BA_REFINE_GRADIENTS_XY: run(refine_features_kernel<B200BA_REFINE_GRADIENTS_XY>); break;
+    case B200BA_REFINE_GRADIENT_MAGNITUDE: run(refine_features_kernel<B200BA_REFINE_GRADIENT_MAGNITUDE>); break;
+    case B200BA_REFINE_INTENSITIES: run(refine_features_kernel<B200BA_REFINE_INTENSITIES>); break;
+    default: run(refine_features_kernel<B200BA_REFINE_NO_REFINEMENT>); break;
+  }
+}
+
 }  // namespace b200ba

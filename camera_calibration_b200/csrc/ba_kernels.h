@@ -127,6 +127,19 @@ struct SynthParams {
 void launch_render_pattern(const SynthParams& p, int n_img, const float2* verts, const int8_t* nv, const float* poses,
                            const uint8_t* pattern, double2* proj, int4* range, uint32_t* bits, uint8_t* images,
                            cudaStream_t s);
+// feature refinement of b200ba_refine_features (the arithmetic is specified in include/b200ba.h)
+struct RefineParams {
+  int w, h;                // image size
+  int half;                // window_half_extent
+  int n_samples, n_match;  // symmetry and matching sample counts
+  int type;                // B200BA_REFINE_*
+  int num_star_segments, squares_x, squares_y, num_tags;
+  int4 tags[B200BA_PATTERN_MAX_TAGS];  // x, y, width, height
+};
+// n predictions whose image indices are relative to `images` ([..][h][w]); one warp per feature.
+void launch_refine_features(const RefineParams& p, int64_t n, const b200ba_feature_prediction* pred,
+                            const uint8_t* images, const float2* samples, float2* xy, float* cost, int* status,
+                            cudaStream_t s);
 void launch_generic_block_inverse(int bs, int nb, int nd, const double* D, const double* B, const double* b1,
                                   double* DinvB, double* Dinvb, cudaStream_t s);
 void launch_symmetrize(int n, double* M, cudaStream_t s);

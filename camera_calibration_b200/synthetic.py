@@ -532,3 +532,60 @@ def intersection_lists(seed: int = 0, d: int = 2, config: int = 2):
             group.append(pts[rng.permutation(len(pts))].astype(np.float32))
         lists.append(group)
     return lists
+
+
+def pattern_feature_predictions(pattern, pattern_size, camera_tr_global, fx_fy_cx_cy, image_size,
+                                max_offset: float = 3.0, seed: int = 0):
+    """Ground truth and displaced predictions of the star-pattern features in images rendered by
+    api.RenderPatternImages (pattern: a dict of io.LoadPatternYAML; pattern_size = (w, h) of the pattern image;
+    camera_tr_global [n_images, 12] as api.SyntheticPoses returns it; image_size = (w, h)).
+
+    For every valid feature coordinate (PatternData::IsValidFeatureCoord) of every image, in double: the feature's
+    pattern-image point (the mapping pattern coordinate -> mm -> px of include/b200ba.h), projected by the pinhole
+    pose, minus 0.5 (pixel-centre convention), and the plane's exact local homography T(-p) H T(c) normalised to
+    (2, 2) = 1, where H maps pattern coordinates to pixel centres. Features behind the camera or with the exact
+    position outside [0, w - 1] x [0, h - 1] are left out. The prediction is the exact position moved by a seeded
+    offset of length at most max_offset in a uniform direction.
+
+    Returns a dict: image [n] int64, pattern_coordinate [n, 2] int32, position [n, 2] float64 (exact),
+    local_pixel_tr_pattern [n, 3, 3] float64, prediction [n, 2] float32."""
+    pw, ph = pattern_size
+    width, height = image_size
+    sx, sy = int(pattern["squares_x"]), int(pattern["squares_y"])
+    f32 = lambda key: float(np.float32(pattern[key]))  # noqa: E731
+    kx, ky = pw / f32("page_width_mm"), ph / f32("page_height_mm")
+    wx, wy = f32("pattern_end_x_mm") - f32("pattern_start_x_mm"), f32("pattern_end_y_mm") - f32("pattern_start_y_mm")
+    A = np.array([[kx * wx / sx, 0, kx * (f32("pattern_start_x_mm") + wx / sx)],
+                  [0, ky * wy / sy, ky * (f32("pattern_start_y_mm") + wy / sy)], [0, 0, 1]])
+    fx, fy, cx, cy = (float(v) for v in np.asarray(fx_fy_cx_cy, np.float32).reshape(4))
+    K = np.array([[fx, 0, cx - 0.5], [0, fy, cy - 0.5], [0, 0, 1]])
+    coords = [(x, y) for y in range(sy - 1) for x in range(sx - 1)
+              if not any(x >= t["x"] - 1 and y >= t["y"] - 1 and x <= t["x"] - 1 + t["width"] and
+                         y <= t["y"] - 1 + t["height"] for t in pattern.get("tags", []))]
+    c = np.array(coords, np.float64).reshape(-1, 2)
+    rng = np.random.default_rng(seed)
+    out = {k: [] for k in ("image", "pattern_coordinate", "position", "local_pixel_tr_pattern", "prediction")}
+    poses = np.asarray(camera_tr_global, np.float64).reshape(-1, 12)
+    for i, pose in enumerate(poses):
+        R, t = pose[:9].reshape(3, 3), pose[9:]
+        H = K @ np.column_stack([R[:, 0], R[:, 1], t]) @ A
+        q = np.column_stack([c, np.ones(len(c))]) @ H.T
+        p = q[:, :2] / q[:, 2:]
+        keep = (q[:, 2] > 0) & (p[:, 0] >= 0) & (p[:, 1] >= 0) & (p[:, 0] <= width - 1) & (p[:, 1] <= height - 1)
+        for k in np.nonzero(keep)[0]:
+            T1 = np.array([[1, 0, -p[k, 0]], [0, 1, -p[k, 1]], [0, 0, 1]])
+            T2 = np.array([[1, 0, c[k, 0]], [0, 1, c[k, 1]], [0, 0, 1]])
+            L = T1 @ H @ T2
+            out["image"].append(i)
+            out["pattern_coordinate"].append(c[k])
+            out["position"].append(p[k])
+            out["local_pixel_tr_pattern"].append(L / L[2, 2])
+        n = int(keep.sum())
+        ang = rng.uniform(0, 2 * np.pi, n)
+        rad = max_offset * rng.uniform(0, 1, n)
+        out["prediction"].extend(p[keep] + np.column_stack([np.cos(ang), np.sin(ang)]) * rad[:, None])
+    return {"image": np.asarray(out["image"], np.int64),
+            "pattern_coordinate": np.asarray(out["pattern_coordinate"], np.int32).reshape(-1, 2),
+            "position": np.asarray(out["position"], np.float64).reshape(-1, 2),
+            "local_pixel_tr_pattern": np.asarray(out["local_pixel_tr_pattern"], np.float64).reshape(-1, 3, 3),
+            "prediction": np.asarray(out["prediction"], np.float32).reshape(-1, 2)}

@@ -707,6 +707,134 @@ B200BA_API int b200ba_render_pattern_images(int device, const b200ba_pattern* pa
                                             const float* fx_fy_cx_cy, int64_t n, const double* camera_tr_global,
                                             uint8_t* images, double* device_ms);
 
+/* ---- sub-pixel refinement of star-pattern features (APP/feature_detection/feature_detector_tagged_pattern.cc:
+ * 1427-1648, FeatureDetectorTaggedPattern::RefineFeatureDetections with the CPU path of
+ * cpu_refinement_by_matching.h and cpu_refinement_by_symmetry.h). Every float operation below is rounded on its own
+ * in the order written (no fused multiply-add); "(float)", "(double)" and "(int)" are C conversions ((int)
+ * truncates; outside the int range and for NaN it gives INT_MIN, as x86-64 does).
+ *
+ * Samples (feature_detector_tagged_pattern.cc:239-248): n = (int)(8.0 * (2h + 1)^2 + 0.5) offsets in [-1, 1]^2,
+ * h = window_half_extent. The reference calls srand(0) and then Vec2f::Random() per sample, x then y, each
+ * coordinate -1.f + (2.f * (float)r) / (float)RAND_MAX (Eigen 3.3's float Random()) with r the next value of glibc's
+ * rand(): the TYPE_3 additive generator of random_r (31 words, separation 3, seeded as srandom(1) because seed 0 is
+ * taken as 1, 310 values discarded), restated here so that the samples do not depend on the platform's rand(). The
+ * first sample is (0.68037546, -0.21123415). Matching uses the first n_m = (int)((1 / 8.) * n) = (2h + 1)^2
+ * samples, symmetry all n. */
+#define B200BA_REFINE_MAX_HALF_EXTENT 32
+/* Returns 2 unless 1 <= window_half_extent <= B200BA_REFINE_MAX_HALF_EXTENT, n equals the count above and xy
+ * ([n][2]) is given. Host only. */
+B200BA_API int b200ba_feature_samples(int32_t window_half_extent, int32_t n, float* xy);
+
+/* The refinement types, numbered as the reference's FeatureRefinement enum. */
+#define B200BA_REFINE_GRADIENTS_XY 0
+#define B200BA_REFINE_GRADIENT_MAGNITUDE 1
+#define B200BA_REFINE_INTENSITIES 2
+#define B200BA_REFINE_NO_REFINEMENT 3
+/* Per-feature status: why a feature was rejected (final_cost -1, position NaN), or 0. */
+#define B200BA_REFINE_ACCEPTED 0
+#define B200BA_REFINE_IMAGE_BORDER 1        /* the window around the prediction leaves the image (:1448-1455) */
+#define B200BA_REFINE_OUTSIDE_PATTERN 2     /* a window corner leaves the repeating pattern area (:1457-1474) */
+#define B200BA_REFINE_MATCH_OUTSIDE 3       /* matching: a sample left the image (in a trial step) */
+#define B200BA_REFINE_MATCH_LEFT_WINDOW 4   /* matching: the position moved >= h from the prediction */
+#define B200BA_REFINE_MATCH_NOT_CONVERGED 5 /* matching: 50 iterations and a last step with |x|^2 >= 1e-8 */
+#define B200BA_REFINE_MATCH_BAD_FACTOR 6    /* matching: the affine intensity factor is <= 0 */
+#define B200BA_REFINE_SYM_OUTSIDE 7         /* symmetry: a sample left the image */
+#define B200BA_REFINE_SYM_LEFT_WINDOW 8     /* symmetry: the position moved >= h from the matching result */
+#define B200BA_REFINE_SYM_NOT_CONVERGED 9   /* symmetry: 30 iterations and a last translation step >= 1e-4f */
+#define B200BA_REFINE_INCONSISTENT 10       /* symmetry and matching results lie more than 0.75 px^2 apart */
+/* One predicted feature (the reference's FeatureDetection plus its image). position: pixel-centre convention
+ * (pixel (0, 0)'s centre is (0, 0)). local_pixel_tr_pattern: row-major; it maps the local pattern coordinate
+ * (0 at the feature, one unit per square) to the pixel offset from the feature. */
+typedef struct b200ba_feature_prediction {
+  int64_t image;                   /* index into images */
+  float position[2];               /* x, y */
+  int32_t pattern_coordinate[2];   /* the feature's integer pattern coordinate */
+  float local_pixel_tr_pattern[9];
+} b200ba_feature_prediction;
+/* Refines every prediction, with the arithmetic of the reference's CPU path:
+ *   Images: images [n_images][height][width] grey u8 (all one size). Bilinear interpolation (libvis'
+ *     InterpolateBilinear / ...WithJacobian) at p: i = (int)p.x, j = (int)p.y, fx = p.x - (float)i, gx = 1 - fx
+ *     (y alike); value = (((gx gy) v00 + (fx gy) v10) + (gx fy) v01) + (fx fy) v11; with the Jacobian instead
+ *     top = gx v00 + fx v10, bottom = gx v01 + fx v11, value = gy top + fy bottom, d/dx = fy (v11 - v01) +
+ *     gy (v10 - v00), d/dy = bottom - top, where for u8 images the differences are int subtractions converted to
+ *     float. Gradient images are not stored: the pixel (x, y) of the gradient image is dx = ((float)I(x+, y) -
+ *     (float)I(x-, y)) / (float)(x+ - x-) with x- = max(0, x - 1), x+ = min(W - 1, x + 1) (dy alike) and the
+ *     gradient magnitude is sqrtf(dx dx + dy dy). A position p is inside when p.x >= 0, p.y >= 0,
+ *     p.x < (float)(W - 1), p.y < (float)(H - 1).
+ *   Pre-filter (:1443-1479): a prediction p passes when p.x - h >= 0, p.y - h >= 0, p.x + h < (float)(W - 1) and
+ *     p.y + h < (float)(H - 1) (each in float), else status IMAGE_BORDER; then local_pattern_tr_pixel = the inverse
+ *     of local_pixel_tr_pattern (rf_inverse3 of camera_calibration_b200/csrc/ba_common.h: the adjugate times
+ *     1 / det), and each window corner c = (+-h, +-h) (corner k: x sign + for even k, y sign + for k < 2) maps to
+ *     the pattern as hnorm(M (c, 1)) (rows ((m0 c.x + m1 c.y) + m2), hnorm divides x and y by z) plus
+ *     (float)pattern_coordinate; it must satisfy PatternData::IsValidPatternCoord (in [-1, squares - 1] and in no
+ *     tag's [tag - 1, tag - 1 + size] box), else status OUTSIDE_PATTERN.
+ *   Matching (cpu_refinement_by_matching.h:232-417), on the u8 image with the first n_m samples s_i:
+ *     template q_i = sum over k = 0..15 (in order, from 0.f) of PatternIntensityAt(hnorm(M (h s_i + o_k, 1))),
+ *       o_k = (-0.375 + 0.25 (k % 4), -0.375 + 0.25 (k / 4)), h s_i = ((float)h s_i.x, (float)h s_i.y);
+ *       PatternIntensityAt(p): c.x = p.x - (float)(sgn (int)(|p.x| + 0.5f)) with sgn = 1 for p.x > 0, else -1 (y
+ *       alike); 0.5f when c.x c.x + c.y c.y < 1e-8f; else a = (float)((double)rf_atan2(c.y, c.x) - pi / 2),
+ *       a = (float)((double)a + 2 pi) when a < 0, and 1.f when (int)((double)((float)num_star_segments * a) /
+ *       (2 pi)) is even, else 0.f.
+ *     sample positions are position + (float)h s_i (x and y each one addition); factor and bias start at
+ *       factor = (S_qp - (S_p / n_m) S_q) / D when |D| > 1e-6f with D = S_pp - (S_p S_p) / n_m, else 1; bias =
+ *       (1.f / n_m) (S_q - factor S_p); S_* are the sums of q p, p, q, p p over the samples (p the interpolated
+ *       value) and n_m is converted to float.
+ *     LM on (x, y, factor, bias), at most 50 iterations: residual r = (factor I + bias) - q_i, Jacobian
+ *       (factor dI/dx, factor dI/dy, I, 1); H += J^T J (upper triangle, each entry J_a J_b added), b += r J,
+ *       cost += r r. lambda = (0.001f * 0.5f) * (((H00 + H11) + H22) + H33) on the first iteration. Up to 10
+ *       attempts: x = rf_ldlt_solve<4>(H, lambda, b) (ba_common.h: unpivoted LDL^T in double, a zero pivot's
+ *       solution component set to 0 as Eigen's LDLT sets it); the trial is
+ *       position - x[0..1], factor - x2, bias - x3; its cost (the sum of r r) below the current cost accepts it
+ *       (last step = ((x0 x0 + x1 x1) + x2 x2) + x3 x3, lambda *= 0.5f), else lambda *= 2.f. No accepted
+ *       attempt ends the loop as converged. After an accepted step, |x - x0| >= h or |y - y0| >= h (float, from
+ *       the prediction) rejects with MATCH_LEFT_WINDOW. After the loop, not converged and (double)last >= 1e-8
+ *       rejects with MATCH_NOT_CONVERGED, then factor <= 0 with MATCH_BAD_FACTOR. A sample outside the image in
+ *       any cost evaluation rejects with MATCH_OUTSIDE.
+ *   Symmetry (cpu_refinement_by_symmetry.h:40-580), skipped for NO_REFINEMENT (final_cost 0): the pattern
+ *     samples are t_i = hnorm(M ((float)h s_i, 1)) for all n samples; P = T(m) * local_pixel_tr_pattern (each entry
+ *     (T_r0 L_0c + T_r1 L_1c) + T_r2 L_2c, T = [1 0 m.x; 0 1 m.y; 0 0 1], m the matching result), then every entry
+ *     divided by P22. Per sample a = hnorm(P (t_i, 1)) and b = hnorm(P (-t_i, 1)); both must be inside
+ *     (SYM_OUTSIDE). INTENSITIES (u8 image) and GRADIENT_MAGNITUDE (gradient-magnitude image): r = I(a) - I(b),
+ *     J = grad I(a) * D(a) - grad I(b) * D(b); GRADIENTS_XY (gradient image): r = g(a) + g(b) (2-vector),
+ *     J = Grad g(a) D(a) + Grad g(b) D(b) (each entry (G_r0 D_0c + G_r1 D_1c)), its two rows added in turn. D(t) is
+ *     d hnorm(P (t, 1)) / d(P00 P01 P02 P10 P11 P12 P20 P21): e0 = 1 / ((P20 t.x + P21 t.y) + 1), e1 = (-1 e0) e0,
+ *     e2 = ((P00 t.x + P01 t.y) + P02) e1, e3 = ((P10 t.x + P11 t.y) + P12) e1; row 0 = (t.x e0, t.y e0, e0, 0, 0,
+ *     0, t.x e2, t.y e2), row 1 = (0, 0, 0, t.x e0, t.y e0, e0, t.x e3, t.y e3). H += J^T J, b += r J, cost +=
+ *     r r (r.x r.x + r.y r.y for GRADIENTS_XY). LM: at most 30 iterations, lambda = (0.001f * (1.f / 8)) *
+ *     (diagonal sum, index order) on the first; up to 10 attempts of x = rf_ldlt_solve<8>, P - x (P22 kept),
+ *     (a textureless window makes H = 0 and lambda = 0; the zero pivots give x = 0, so the LM ends converged at m
+ *     with final_cost 0, as the reference's does),
+ *     accepted when the trial cost is lower (last step = x2 x2 + x5 x5, lambda *= 0.5f, position = (P02, P12)),
+ *     else lambda *= 2.f; no accepted attempt ends as converged; an accepted step with |P02 - m.x| >= h or
+ *     |P12 - m.y| >= h rejects with SYM_LEFT_WINDOW; 30 iterations end converged only when last step < 1e-4f, else
+ *     SYM_NOT_CONVERGED. final_cost is the cost at the result.
+ *   Final test (:1626-1647): (dx dx + dy dy) > 0.75f between the symmetry and the matching result rejects with
+ *     INCONSISTENT.
+ *   Sums: every sum above over samples is taken in one order, that of one warp: lane l (0..31) adds samples l,
+ *     l + 32, l + 64, ... in order into its own float accumulator (from 0.f), then the 32 lane values are
+ *     combined by butterflies v_l = v_l + v_(l xor o) for o = 16, 8, 4, 2, 1. The reference adds into one running
+ *     float sum per accumulator instead; the difference this order makes is stated in DESIGN.md section 7.
+ *   Pinned here: the reference's pattern is d->patterns[0], one per call; its CUDA path handles at most 128
+ *     features per call and only GRADIENTS_XY and INTENSITIES, neither applies. The LDL^T is unpivoted (Eigen's
+ *     pivots), and the inverse and atan2 are this library's (ba_common.h).
+ * Outputs: xy [n_features][2] (NaN for a rejected feature), final_cost [n_features] (-1 for a rejected feature;
+ * the reference leaves a rejected feature's position partly written), status [n_features] (nullable), device_ms
+ * (nullable): device time of the refinement kernels, without the uploads. samples: [n_samples][2], normally
+ * b200ba_feature_samples(window_half_extent); callers may pass their own. Images go to the device in chunks bounded
+ * in device memory (about 512 MiB; the environment variable B200BA_REFINE_CHUNK lowers the images per chunk), and the
+ * features of a chunk in launches of at most 2^20 (80 bytes of device memory each), so any number of images and
+ * features works; the outputs do not depend on the chunking or on the order of the features.
+ * Stand-alone (allocates, computes, frees). Returns 2 for a bad argument before any CUDA call: NULL pointers, width
+ * or height below 1 or above 2^15, n_images < 0, n_features < 0, the pattern checks of
+ * b200ba_render_pattern_images, window_half_extent outside [1, B200BA_REFINE_MAX_HALF_EXTENT], n_samples other than
+ * the count for it, an unknown refinement_type, an image index outside [0, n_images), a non-finite
+ * local_pixel_tr_pattern entry. Returns 3 without a device. */
+B200BA_API int b200ba_refine_features(int device, const b200ba_pattern* pattern, const uint8_t* images, int32_t width,
+                                      int32_t height, int64_t n_images, const float* samples, int32_t n_samples,
+                                      int32_t window_half_extent, int32_t refinement_type, int64_t n_features,
+                                      const b200ba_feature_prediction* predictions, float* xy, float* final_cost,
+                                      int32_t* status, double* device_ms);
+
 /* ---- multi-GPU: imagesets sharded over ranks, one NCCL all-reduce per H/b build --- */
 #define B200BA_NCCL_UNIQUE_ID_BYTES 128
 B200BA_API int b200ba_nccl_unique_id(uint8_t id[B200BA_NCCL_UNIQUE_ID_BYTES]);

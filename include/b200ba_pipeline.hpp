@@ -1250,4 +1250,56 @@ inline int RenderSyntheticDataset(const std::string& path,
   return EXIT_SUCCESS;
 }
 
+// ---- feature refinement (FeatureDetectorTaggedPattern::RefineFeatureDetections) -----------------------------------
+// The reference's sample offsets for window_half_extent (b200ba_feature_samples); empty for a bad extent.
+inline std::vector<Vec2f> FeatureSamples(int window_half_extent) {
+  const int n = static_cast<int>(8.0 * (2 * window_half_extent + 1) * (2 * window_half_extent + 1) + 0.5);
+  std::vector<Vec2f> samples(std::max(n, 0));
+  if (b200ba_feature_samples(window_half_extent, n, reinterpret_cast<float*>(samples.data())) != 0) samples.clear();
+  return samples;
+}
+
+// The reference's FeatureDetection (feature_detector_tagged_pattern.h:291-317) plus the index of its image.
+struct FeatureDetection {
+  Vec2f position;            // pixel-centre convention
+  Vec2i pattern_coordinate;  // integer feature coordinate in the pattern
+  float final_cost = 0;      // negative for a rejected feature
+  float local_pixel_tr_pattern[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};  // row-major
+  int64_t image = 0;         // index into the images passed to RefineFeatureDetections
+};
+
+// RefineFeatureDetections (feature_detector_tagged_pattern.cc:1427-1648) for the features of any number of grey
+// images of one size (images: n_images * width * height bytes), on the device (b200ba_refine_features, the
+// arithmetic of the reference's CPU path for all four refinement types, B200BA_REFINE_*). output[i] is
+// predicted_features[i] with the refined position and final_cost, or final_cost -1 and a NaN position when it is
+// rejected; status (nullable) receives the reason codes. Returns the library's return code (0 on success).
+inline int RefineFeatureDetections(const b200ba_pattern& pattern, const uint8_t* images, int width, int height,
+                                   int64_t n_images, int window_half_extent, int refinement_type, int num_features,
+                                   const FeatureDetection* predicted_features, FeatureDetection* output,
+                                   std::vector<int32_t>* status = nullptr, int device = -1) {
+  const std::vector<Vec2f> samples = FeatureSamples(window_half_extent);
+  std::vector<b200ba_feature_prediction> pred(std::max(num_features, 0));
+  for (int i = 0; i < num_features; ++i) {
+    const FeatureDetection& f = predicted_features[i];
+    pred[i].image = f.image;
+    pred[i].position[0] = f.position.x, pred[i].position[1] = f.position.y;
+    pred[i].pattern_coordinate[0] = f.pattern_coordinate.x, pred[i].pattern_coordinate[1] = f.pattern_coordinate.y;
+    std::copy(f.local_pixel_tr_pattern, f.local_pixel_tr_pattern + 9, pred[i].local_pixel_tr_pattern);
+  }
+  std::vector<float> xy(2 * pred.size()), cost(pred.size());
+  std::vector<int32_t> st(pred.size());
+  const int rc = b200ba_refine_features(device, &pattern, images, width, height, n_images,
+                                        reinterpret_cast<const float*>(samples.data()),
+                                        static_cast<int32_t>(samples.size()), window_half_extent, refinement_type,
+                                        num_features, pred.data(), xy.data(), cost.data(), st.data(), nullptr);
+  if (rc != 0) return rc;
+  for (int i = 0; i < num_features; ++i) {
+    output[i] = predicted_features[i];
+    output[i].position = Vec2f{xy[2 * i], xy[2 * i + 1]};
+    output[i].final_cost = cost[i];
+  }
+  if (status) *status = st;
+  return 0;
+}
+
 }  // namespace b200ba_shim

@@ -24,6 +24,7 @@
 namespace b200ba_shim {
 
 struct Vec2f { float x, y; };
+struct Vec2i { int32_t x, y; };
 struct Vec2d { double x, y; };
 struct Vec3d { double x, y, z; };
 

@@ -405,7 +405,7 @@ __device__ __forceinline__ void process_observation(const ProblemDev& pb, const 
     P[1][2] = (M1.z - m1d * d.z) * ilen;
     int x0, y0;
     double fu, fv;
-    locate(c, px, py, x0, y0, fu, fv);
+    locate_support(c, px, py, x0, y0, fu, fv);
     cell = x0 + y0 * c.gw;
     if (COMPACT) {
       // d unproj / d G_k = w_k / |s| (I - u u^T) and M u = 0 (the columns of A are orthogonal to u), so
@@ -463,7 +463,7 @@ __device__ __forceinline__ void process_observation(const ProblemDev& pb, const 
     P[1][2] = Ri10 * nt1.z + Ri11 * nt2.z;
     int x0, y0;
     double fu, fv;
-    locate(c, px, py, x0, y0, fu, fv);
+    locate_support(c, px, py, x0, y0, fu, fv);
     cell = x0 + y0 * c.gw;
     if (!L.localize_only) {
       double wx[4], dwx[4], wy[4], dwy[4];

@@ -182,6 +182,32 @@ class BundleAdjuster:
         return {"H": H, "b": b, "S": S, "rhs": rhs, "x": x, "lambda": lam_used.value, "nbd": nbd,
                 "info": {k: int(v) for k, v in zip(names, info)}}
 
+    def debug_apply_update(self, opt: Options, x) -> FlatState:
+        """The retraction of one LM attempt (``b200ba_debug_apply_update``): the current state minus the update
+        ``x`` (``build_system``'s variable order), computed into the trial slot and returned; the current state
+        is unchanged. The returned ``last_projection`` is None."""
+        p = self.problem
+        x = np.ascontiguousarray(x, dtype=np.float64)
+        st = FlatState(np.zeros((p.n_points, 3)), np.zeros((p.n_imagesets, 7)), np.zeros((p.n_cameras, 7)),
+                       [np.zeros(c.intrinsics_size()) for c in p.cameras], None)
+        cs = st.c_struct()
+        _check(self.lib.b200ba_debug_apply_update(self._h, C.byref(opt), _dp(x), len(x), C.byref(cs)), self._h)
+        return st
+
+    def debug_nice_orientation(self) -> np.ndarray:
+        """ChooseNiceCameraOrientation applied to every camera of the device-resident state
+        (``b200ba_debug_nice_orientation``). Returns the [n_cameras, 3, 3] rotations."""
+        rot = np.zeros((self.problem.n_cameras, 3, 3))
+        _check(self.lib.b200ba_debug_nice_orientation(self._h, _dp(rot)), self._h)
+        return rot
+
+    def debug_lm_events(self) -> np.ndarray:
+        """Outcome of each LM attempt of the last ``optimize`` (``cabi.LM_*``), in order."""
+        n = int(self.lib.b200ba_debug_lm_events(self._h, None, 0))
+        codes = np.zeros(max(n, 1), np.int32)
+        self.lib.b200ba_debug_lm_events(self._h, codes.ctypes.data_as(C.POINTER(C.c_int32)), n)
+        return codes[:n]
+
     def calibration_report(self, with_errors: bool = False):
         """CreateCalibrationReport's numbers (calibration_report.cc:83-98) for every camera on the device-resident
         state (``b200ba_calibration_report``). Returns (reports, errors, device_ms): one ``cabi.CameraReport``
@@ -434,6 +460,19 @@ def dense_cholesky_solve(A, b, block_width: int = 256, device: int = -1):
     fm, sm = C.c_double(0), C.c_double(0)
     _check(lib.b200ba_dense_cholesky_solve(device, n, int(block_width), _dp(A), _dp(b), _dp(x), C.byref(fm), C.byref(sm)))
     return x, fm.value, sm.value
+
+
+def debug_cost_compare(trial, base=None, residual=None, device: int = -1) -> np.ndarray:
+    """The LM's cost comparison and totals (``b200ba_debug_cost_compare``) on host arrays: ``trial`` [n],
+    ``base`` [n] or None, ``residual`` [2, n] or None. Returns the 6 sums (see the header)."""
+    lib = cabi.load_library()
+    t = np.ascontiguousarray(trial, dtype=np.float64)
+    b = None if base is None else np.ascontiguousarray(base, dtype=np.float64)
+    r = None if residual is None else np.ascontiguousarray(residual, dtype=np.float64)
+    out = np.zeros(6)
+    _check(lib.b200ba_debug_cost_compare(device, len(t), _dp(t), None if b is None else _dp(b),
+                                         None if r is None else _dp(r), _dp(out)))
+    return out
 
 
 def schur_solve(block_size: int, D, B, Cm, b1, b2, device: int = -1) -> np.ndarray:

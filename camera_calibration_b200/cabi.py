@@ -535,7 +535,14 @@ SYMBOLS = {
     "b200ba_debug_eval_counts": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint16)]),
     "b200ba_debug_solve_step": (C.c_int, [C.c_void_p, C.POINTER(Options), C.c_double, C.c_int32, _D, _D, _D, _D, _D, _D,
                                           _I32]),
+    "b200ba_debug_apply_update": (C.c_int, [C.c_void_p, C.POINTER(Options), _D, C.c_int32, C.POINTER(State)]),
+    "b200ba_debug_cost_compare": (C.c_int, [C.c_int, C.c_int64, _D, _D, _D, _D]),
+    "b200ba_debug_nice_orientation": (C.c_int, [C.c_void_p, _D]),
+    "b200ba_debug_lm_events": (C.c_int32, [C.c_void_p, _I32, C.c_int32]),
 }
+
+# b200ba_debug_lm_events codes (the oracle reports a NaN update as LM_REFUSED_PIVOT)
+LM_ACCEPTED, LM_REJECTED_COST, LM_REFUSED_PIVOT = 1, 2, 3
 
 
 class LibraryMissing(RuntimeError):

@@ -167,6 +167,7 @@ struct b200ba_handle {
   // between the Schur phase and the factorisation; null in every other call
   double* capture_S = nullptr;
   double* capture_rhs = nullptr;
+  std::vector<int32_t> lm_events;         // B200BA_LM_* per LM attempt of the last b200ba_optimize
   std::vector<double> grp_sums;           // [sx | sy | count] per Schur block (see build_groups)
   int force_grouped = -1;                 // B200BA_GROUPED=0|1 overrides the cost model
   bool compact_j = true;                  // B200BA_COMPACT_J=0: expanded Jacobian buffer also for central-generic cameras
@@ -1969,6 +1970,7 @@ int b200ba_optimize(b200ba_handle* h, const b200ba_options* opt, b200ba_report* 
   if (int rc = check_ready(h, opt)) return rc;
   memset(report, 0, sizeof(*report));
   memset(&h->timings, 0, sizeof(h->timings));
+  h->lm_events.clear();
   cudaEvent_t ev_total_a = get_event(h), ev_total_b = get_event(h);
   cudaEventRecord(ev_total_a, h->stream);
   const Layout& L = h->L;
@@ -2037,6 +2039,7 @@ int b200ba_optimize(b200ba_handle* h, const b200ba_options* opt, b200ba_report* 
       if (!spd) {
         // A non-positive pivot: the analogue of the reference's NaN-update rejection
         // (lm_optimizer.h:905-913) -- increase the damping and retry.
+        h->lm_events.push_back(B200BA_LM_REFUSED_PIVOT);
         lambda = 2.f * lambda;
         if (opt->print_progress) fprintf(stderr, "[b200ba]   [%d, %d] factorisation failed, new lambda %g\n", iteration + 1, lm_iteration + 1, lambda);
         continue;
@@ -2060,6 +2063,7 @@ int b200ba_optimize(b200ba_handle* h, const b200ba_options* opt, b200ba_report* 
       const double trial_cost = h->h_scal[3];
       // CostIsSmallerThan (lm_optimizer.h:993-1011)
       if (count > 0 && left < right) {
+        h->lm_events.push_back(B200BA_LM_ACCEPTED);
         h->cur = trial;
         stat_valid = h->h_scal[4];
         stat_sumsq = h->h_scal[5];
@@ -2070,6 +2074,7 @@ int b200ba_optimize(b200ba_handle* h, const b200ba_options* opt, b200ba_report* 
         if (opt->print_progress) fprintf(stderr, "[b200ba] [%d] update accepted, cost %.12g\n", iteration + 1, trial_cost);
         break;
       } else {
+        h->lm_events.push_back(B200BA_LM_REJECTED_COST);
         lambda = 2.f * lambda;
         if (opt->print_progress) fprintf(stderr, "[b200ba]   [%d, %d of %d] update rejected (bad cost: %.12g), new lambda: %g\n", iteration + 1, lm_iteration + 1, opt->max_lm_attempts, trial_cost, lambda);
       }
@@ -2308,6 +2313,83 @@ int b200ba_debug_solve_step(b200ba_handle* h, const b200ba_options* opt, double 
   dense_variants(&info[3], &info[4], &info[5], &info[6]);
   info[7] = h->own_dense ? h->dn.NB : 0;
   return 0;
+}
+
+// Diagnostics / tests: the retraction of one LM attempt (update_state_kernel) from the current state
+// with the caller's update, downloaded from the trial slot. The current state is not changed.
+int b200ba_debug_apply_update(b200ba_handle* h, const b200ba_options* opt, const double* x, int32_t n,
+                              b200ba_state* out) {
+  if (int rc = check_ready(h, opt)) return rc;
+  const Layout& L = h->L;
+  if (n != L.dof || !x || !out) {
+    h->error = "b200ba_debug_apply_update: n does not equal the number of unknowns, or an argument is NULL";
+    return 2;
+  }
+  CUDA_TRY(h, cudaMemcpyAsync(h->d_x, x, static_cast<size_t>(n) * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  launch_update_state(h->pb, L, h->st[h->cur], h->st[1 - h->cur], h->d_x, h->n_control_total, h->n_param_total,
+                      h->stream);
+  CUDA_TRY(h, cudaGetLastError());
+  b200ba_state o = *out;
+  o.last_projection = nullptr;  // the warm-start cache is not part of the retraction
+  h->cur = 1 - h->cur;
+  const int rc = b200ba_get_state(h, &o);
+  h->cur = 1 - h->cur;
+  return rc;
+}
+
+// Diagnostics / tests: launch_cost_reduce on caller's arrays (trial [n], base [n] or NULL,
+// residual [2n] as all x then all y, or NULL); stand-alone, one scoped device call.
+int b200ba_debug_cost_compare(int device, int64_t n, const double* trial, const double* base, const double* residual,
+                              double out[6]) {
+  if (n < 0 || (n > 0 && !trial) || !out) {
+    g_create_error = "b200ba_debug_cost_compare: bad argument";
+    return 2;
+  }
+  CallScope cs(&g_create_error);
+  if (int rc = cs.use_device(device)) return rc;
+  const size_t m = static_cast<size_t>(std::max<int64_t>(1, n));
+  double *d_t = nullptr, *d_b = nullptr, *d_r = nullptr, *d_partial = nullptr, *d_out = nullptr;
+  cs.alloc(&d_t, m);
+  if (base) cs.alloc(&d_b, m);
+  if (residual) cs.alloc(&d_r, 2 * m);
+  cs.alloc(&d_partial, cost_reduce_partial_size());
+  cs.alloc(&d_out, 6);
+  if (cs.rc == 0 && n > 0) {
+    cs.ok(cudaMemcpy(d_t, trial, n * sizeof(double), cudaMemcpyHostToDevice));
+    if (base) cs.ok(cudaMemcpy(d_b, base, n * sizeof(double), cudaMemcpyHostToDevice));
+    if (residual) cs.ok(cudaMemcpy(d_r, residual, 2 * n * sizeof(double), cudaMemcpyHostToDevice));
+  }
+  if (cs.rc == 0) {
+    launch_cost_reduce(n, d_t, d_b, d_r, d_partial, d_out, 0);
+    cs.ok(cudaGetLastError());
+    cs.ok(cudaMemcpy(out, d_out, 6 * sizeof(double), cudaMemcpyDeviceToHost));
+  }
+  return cs.rc;
+}
+
+// Diagnostics / tests: ChooseNiceCameraOrientation of every camera applied to the current state, as
+// b200ba_run_bundle_adjustment does after each iteration; rot [9 * n_cameras] receives the rotations.
+int b200ba_debug_nice_orientation(b200ba_handle* h, double* rot) {
+  if (!h) return 1;
+  if (!rot || !h->have_state) {
+    h->error = "b200ba_debug_nice_orientation: rot is NULL, or no state";
+    return 2;
+  }
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  if (!h->d_rot && dev_alloc(h, &h->d_rot, 9 * static_cast<size_t>(h->n_cameras))) return 1;
+  launch_nice_orientation(h->pb, h->st[h->cur], h->n_cameras, h->d_rot, h->stream);
+  CUDA_TRY(h, cudaGetLastError());
+  CUDA_TRY(h, cudaMemcpyAsync(rot, h->d_rot, 9 * sizeof(double) * h->n_cameras, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  return 0;
+}
+
+// Diagnostics / tests: the outcome of every LM attempt of the last b200ba_optimize (B200BA_LM_*).
+int32_t b200ba_debug_lm_events(const b200ba_handle* h, int32_t* codes, int32_t cap) {
+  if (!h) return -1;
+  const int32_t n = static_cast<int32_t>(h->lm_events.size());
+  for (int32_t i = 0; i < n && i < cap && codes; ++i) codes[i] = h->lm_events[i];
+  return n;
 }
 
 // Diagnostics / tests: evaluation budget of the main Jacobian pass (default 16); 1 forces every

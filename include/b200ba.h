@@ -901,6 +901,29 @@ B200BA_API int b200ba_debug_eval_counts(b200ba_handle* h, uint16_t* counts);
 B200BA_API int b200ba_debug_solve_step(b200ba_handle* h, const b200ba_options* opt, double lambda, int32_t n,
                                        double* H, double* b, double* S, double* rhs, double* x,
                                        double* lambda_used, int32_t info[8]);
+/* The retraction of one LM attempt (the reference's JointOptimizationState::operator-=) with the
+ * caller's update x [n] (n = the number of unknowns, b200ba_build_system's variable order), from the
+ * current state into the trial slot; the trial state is downloaded into out (last_projection is not
+ * written). The current state is not changed. */
+B200BA_API int b200ba_debug_apply_update(b200ba_handle* h, const b200ba_options* opt, const double* x, int32_t n,
+                                         b200ba_state* out);
+/* The LM's cost comparison (CostIsSmallerThan) and totals, on the caller's arrays: trial [n], base [n]
+ * (nullable), residual [2n] as all x then all y (nullable); a negative cost marks an invalid residual.
+ * out [6]: trial sum and base sum over the residuals valid in both, their count, total trial cost,
+ * number of valid trial residuals, sum |r|^2 over those. Stand-alone; returns 3 without a device. */
+B200BA_API int b200ba_debug_cost_compare(int device, int64_t n, const double* trial, const double* base,
+                                         const double* residual, double out[6]);
+/* ChooseNiceCameraOrientation applied to every camera of the current state, as
+ * b200ba_run_bundle_adjustment does after each iteration (grids and camera_tr_rig are rotated);
+ * rot [9 * n_cameras] receives each rotation, row-major (the identity for models other than
+ * central-generic). */
+B200BA_API int b200ba_debug_nice_orientation(b200ba_handle* h, double* rot);
+/* Outcome of each LM attempt of the last b200ba_optimize, in order, over all its iterations. */
+#define B200BA_LM_ACCEPTED 1       /* cost comparison accepted the update */
+#define B200BA_LM_REJECTED_COST 2  /* cost comparison rejected the update */
+#define B200BA_LM_REFUSED_PIVOT 3  /* factorisation met a non-positive pivot; the update was not evaluated */
+/* Copies up to cap codes; returns the number of attempts (-1 for a NULL handle). */
+B200BA_API int32_t b200ba_debug_lm_events(const b200ba_handle* h, int32_t* codes, int32_t cap);
 
 #ifdef __cplusplus
 }

@@ -1748,6 +1748,9 @@ bool cost_is_smaller_than(const std::vector<double>& left, const std::vector<dou
   return count > 0 && ls < rs;
 }
 
+// outcome of each LM attempt of the last oracle_optimize (B200BA_LM_*; a NaN update is B200BA_LM_REFUSED_PIVOT)
+std::vector<int32_t> g_lm_events;
+
 double now_seconds() {
   using namespace std::chrono;
   return duration_cast<duration<double>>(steady_clock::now().time_since_epoch()).count();
@@ -1775,6 +1778,7 @@ int oracle_optimize(const b200ba_problem* pb, b200ba_state* state, const b200ba_
                     b200ba_report* report) {
   if (!check_options(pb, opt) || !state || !report) return 1;
   memset(report, 0, sizeof(*report));
+  g_lm_events.clear();
   const b200ba_problem& P = *pb;
   Layout L = make_layout(P, *opt);
   State S = load_state(P, *state);
@@ -1914,6 +1918,7 @@ int oracle_optimize(const b200ba_problem* pb, b200ba_state* state, const b200ba_
       }
       report->solve_time += now_seconds() - ts;
       if (std::isnan(x[0])) {
+        g_lm_events.push_back(B200BA_LM_REFUSED_PIVOT);
         lambda = 2.f * lambda;
         continue;
       }
@@ -1928,6 +1933,7 @@ int oracle_optimize(const b200ba_problem* pb, b200ba_state* state, const b200ba_
       cf.compute(false, updated, &test);
       report->cost_and_jacobian_evaluation_time += now_seconds() - tc;
       if (cost_is_smaller_than(test_costs, residual_cost_vector)) {
+        g_lm_events.push_back(B200BA_LM_ACCEPTED);
         S = updated;
         lambda = 0.5f * lambda;
         applied_update = true;
@@ -1936,6 +1942,7 @@ int oracle_optimize(const b200ba_problem* pb, b200ba_state* state, const b200ba_
         final_costs = test_costs;
         break;
       } else {
+        g_lm_events.push_back(B200BA_LM_REJECTED_COST);
         lambda = 2.f * lambda;
       }
     }
@@ -1982,6 +1989,12 @@ int oracle_optimize(const b200ba_problem* pb, b200ba_state* state, const b200ba_
   store_state(P, S, state);
   if (state->last_projection) std::copy(last_proj.begin(), last_proj.end(), state->last_projection);
   return 0;
+}
+
+int32_t oracle_lm_events(int32_t* codes, int32_t cap) {
+  const int32_t n = static_cast<int32_t>(g_lm_events.size());
+  for (int32_t i = 0; i < n && i < cap && codes; ++i) codes[i] = g_lm_events[i];
+  return n;
 }
 
 int oracle_evaluate(const b200ba_problem* pb, b200ba_state* state, const b200ba_options* opt,

@@ -27,6 +27,9 @@ extern "C" {
 /* OptimizeJointly (joint_optimization.cc:757-953). state is in/out. */
 int oracle_optimize(const b200ba_problem* problem, b200ba_state* state,
                     const b200ba_options* opt, b200ba_report* report);
+/* Outcome of each LM attempt of the last oracle_optimize (B200BA_LM_*; an update with a NaN is
+ * B200BA_LM_REFUSED_PIVOT). Copies up to cap codes; returns the number of attempts. */
+int32_t oracle_lm_events(int32_t* codes, int32_t cap);
 
 /* JointOptimizationCostFunction::Compute<compute_jacobians> (joint_optimization.cc:240-306).
  * Outputs are nullable. Jacobian outputs as in b200ba_get_jacobians(); has_jacobian[i]=0

@@ -74,6 +74,8 @@ def lib():
         l.oracle_solve_dense.argtypes = [C.c_int32, _D, _D, _D]
         l.oracle_apply_update.restype = C.c_int
         l.oracle_apply_update.argtypes = [C.POINTER(Problem), C.POINTER(State), C.POINTER(Options), _D]
+        l.oracle_lm_events.restype = C.c_int32
+        l.oracle_lm_events.argtypes = [_I32, C.c_int32]
         l.oracle_project.restype = C.c_int
         l.oracle_project.argtypes = [C.POINTER(Camera), _D, C.c_int64, _D, _D, _I32]
         l.oracle_unproject.restype = C.c_int
@@ -118,6 +120,15 @@ def optimize(problem: FlatProblem, state: FlatState, opt: Options):
     if rc != 0:
         raise RuntimeError(f"oracle_optimize failed ({rc})")
     return st, rep
+
+
+def lm_events() -> np.ndarray:
+    """Outcome of each LM attempt of the last ``optimize`` in this process (``cabi.LM_*``; a NaN update is
+    reported as ``cabi.LM_REFUSED_PIVOT``), in order."""
+    n = int(lib().oracle_lm_events(None, 0))
+    codes = np.zeros(max(n, 1), np.int32)
+    lib().oracle_lm_events(_p(codes, C.c_int32), n)
+    return codes[:n]
 
 
 def evaluate(problem: FlatProblem, state: FlatState, opt: Options, compute_jacobians: bool, K: int = 0):

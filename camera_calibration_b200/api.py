@@ -22,6 +22,7 @@ from __future__ import annotations
 
 import ctypes as C
 import enum
+import time
 from dataclasses import dataclass
 from typing import Dict, List, Optional, Sequence, Tuple
 
@@ -239,6 +240,25 @@ class BundleAdjuster:
                                              C.byref(ms)), self._h)
         return {"observation_directions": od, "error_directions": ed, "error_magnitudes": em,
                 "n_sites": int(n_sites.value), "device_ms": ms.value}
+
+    def delete_outliers(self, camera: int, outlier_removal_factor: float, imageset_used, with_image: bool = True):
+        """DeleteOutlierFeatures' quartile rule (calibration.cc:62-184) for one camera on the device-resident state
+        (``b200ba_delete_outliers``). ``imageset_used`` ([n_imagesets] of the problem) is read and not modified.
+        Returns (report, imageset_used, remove, image, device_ms): a ``cabi.OutlierReport``, the updated
+        [n_imagesets] bool array, the [n_obs] bool removal mask in the problem's observation order and, with
+        ``with_image``, the [h, w, 3] uint8 image of the removed features (else None). The state and
+        last_projection are left as they were."""
+        used = np.ascontiguousarray(np.asarray(imageset_used, dtype=bool).astype(np.uint8))
+        if used.shape != (self.problem.n_imagesets,):
+            raise B200BAError(f"imageset_used needs {self.problem.n_imagesets} entries, not {used.shape}")
+        remove = np.zeros(max(self.problem.n_obs, 1), np.uint8)
+        cam = self.problem.cameras[camera] if 0 <= camera < self.problem.n_cameras else None
+        image = np.zeros((cam.height, cam.width, 3), np.uint8) if with_image and cam is not None else None
+        report = cabi.OutlierReport()
+        ms = C.c_double(0)
+        _check(self.lib.b200ba_delete_outliers(self._h, int(camera), float(outlier_removal_factor), _u8p(used),
+                                               _u8p(remove), _u8p(image), C.byref(report), C.byref(ms)), self._h)
+        return report, used.astype(bool), remove[:self.problem.n_obs].astype(bool), image, ms.value
 
     def timings(self) -> cabi.Timings:
         t = cabi.Timings()
@@ -904,6 +924,7 @@ class Dataset:
         self.m_num_cameras = num_cameras
         self.image_sizes = [np.zeros(2, dtype=np.int64) for _ in range(num_cameras)]
         self.m_imagesets: List[Imageset] = []
+        self.first_imageset_indices_for_datasets: List[int] = [0]
         self._b200_context = None
 
     def num_cameras(self): return self.m_num_cameras
@@ -921,6 +942,36 @@ class Dataset:
         self._b200_context = None
 
     def DeleteLastImageset(self): self.DeleteImageset(len(self.m_imagesets) - 1)
+
+    def Merge(self, other: "Dataset") -> bool:
+        """APP/dataset.cc:78-130: appends the imagesets and known geometries of ``other``. Refused (False, nothing
+        changed) where the camera counts or image sizes differ. Every known geometry stays separate: the feature ids
+        of ``other`` and of its geometries are offset by 1 + the largest feature id of this dataset's geometries (by
+        1 when it has none). The first imageset index of ``other`` is appended to
+        ``first_imageset_indices_for_datasets``."""
+        if self.m_num_cameras != other.m_num_cameras:
+            return False
+        if any(not np.array_equal(a, b) for a, b in zip(self.image_sizes, other.image_sizes)):
+            return False
+        from .io import KnownGeometry
+        mine = getattr(self, "known_geometries", [])
+        offset = max([0] + [fid for g in mine for fid in g.feature_id_to_position]) + 1
+        merged = list(mine)
+        for g in getattr(other, "known_geometries", []):
+            kg = KnownGeometry()
+            kg.cell_length_in_meters = g.cell_length_in_meters
+            kg.feature_id_to_position = {fid + offset: pos for fid, pos in g.feature_id_to_position.items()}
+            merged.append(kg)
+        self.known_geometries = merged
+        self.first_imageset_indices_for_datasets.append(len(self.m_imagesets))
+        for src in other.m_imagesets:
+            s = self.NewImageset()
+            s.SetFilename(src.GetFilename())
+            for c in range(self.m_num_cameras):
+                f = src.FeaturesOfCamera(c)
+                s.m_features[c] = dict(xy=f["xy"].copy(), id=(f["id"] + np.int32(offset)).astype(np.int32),
+                                       index=f["index"].copy(), last_projection=f["last_projection"].copy())
+        return True
     def GetImageset(self, index) -> Imageset: return self.m_imagesets[index]
     def ImagesetCount(self) -> int: return len(self.m_imagesets)
 
@@ -1019,7 +1070,9 @@ class _Context:
         cams = [m.c_camera() for m in state.intrinsics]
         self.cam_bytes = [bytes(c) for c in cams]
         self.problem = FlatProblem(cams, len(used), len(state.points), oi, oc, op, oxy)
+        t0 = time.perf_counter()
         self.adjuster = BundleAdjuster(self.problem)
+        self.build_seconds = time.perf_counter() - t0  # b200ba_create: upload and layout of the problem
 
     def matches(self, state: BAState, flat) -> bool:
         used, slices, oi, oc, op, oxy = flat

@@ -216,6 +216,19 @@ class CameraReport(C.Structure):
     ]
 
 
+class OutlierReport(C.Structure):
+    """b200ba_outlier_report: the quartile rule of one camera's outlier round."""
+    _fields_ = [
+        ("count", C.c_int64),
+        ("q1", C.c_double),
+        ("q3", C.c_double),
+        ("threshold", C.c_double),
+        ("removed", C.c_int64),
+        ("failed", C.c_int64),
+        ("skipped", C.c_int32),
+    ]
+
+
 class FittingReport(C.Structure):
     """b200ba_fitting_report: CreateFittingErrorReport's numbers for two models of one camera."""
     _fields_ = [
@@ -513,6 +526,8 @@ SYMBOLS = {
     "b200ba_calibration_report": (C.c_int, [C.c_void_p, C.POINTER(CameraReport), _D, _D]),
     "b200ba_report_images": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_uint8), C.POINTER(C.c_uint8),
                                        C.POINTER(C.c_uint8), C.POINTER(C.c_int64), _D]),
+    "b200ba_delete_outliers": (C.c_int, [C.c_void_p, C.c_int32, C.c_float, C.POINTER(C.c_uint8), C.POINTER(C.c_uint8),
+                                         C.POINTER(C.c_uint8), C.POINTER(OutlierReport), _D]),
     "b200ba_render_voronoi": (C.c_int, [C.c_int, C.c_int32, C.c_int32, C.c_int64, _I32, C.POINTER(C.c_float),
                                         C.POINTER(C.c_uint8), _D]),
     "b200ba_visualize_camera": (C.c_int, [C.c_int, C.c_int32, C.c_int32, _D, C.POINTER(C.c_uint8), _D, _D, _D]),

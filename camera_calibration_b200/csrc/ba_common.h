@@ -134,6 +134,21 @@ struct ReportDev {
   ReportCam* cams;       // [n_cameras]
 };
 
+// Outlier round of one camera (b200ba_delete_outliers): device buffers of one call. n is the camera's observation count.
+struct OutlierDev {
+  int64_t* range;               // [2] {0, n}
+  double* mag;                  // [n] |e| on used imagesets where Project succeeded, else NaN
+  double* partial;              // report_partial_size(1)
+  unsigned int* select_hist;    // [2 * 256]
+  ReportCam* stats;             // [2] count, q1 (.median of [0]) and q3 (.median of [1])
+  uint8_t* used;                // [n_imagesets] imageset_used, in / out
+  int* kept;                    // [n_imagesets] kept features of the camera
+  unsigned long long* counts;   // [2] removed, failed
+  uint8_t* remove;              // [n_obs] caller order
+  uint32_t* owner;              // [w * h] 1 + the largest caller index removed at the pixel, or NULL (no image)
+  uint8_t* image;               // [3 * w * h] or NULL
+};
+
 // Model comparison (b200ba_compare_models): device buffers of one call.
 struct CompareDev {
   double* mag;                  // [w * h] |re-projection error|, NaN where A's un-projection or B's Project fails

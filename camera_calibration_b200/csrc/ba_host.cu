@@ -1952,6 +1952,97 @@ int b200ba_report_images(b200ba_handle* h, int32_t camera, uint8_t* observation_
   return cs.rc;
 }
 
+// DeleteOutlierFeatures (calibration.cc:62-184) for one camera on the state held by the handle: the report's error
+// pass, the exact quartiles by radix select, the removal mask, the imageset rule and the outlier image.
+int b200ba_delete_outliers(b200ba_handle* h, int32_t camera, float outlier_removal_factor, uint8_t* imageset_used,
+                           uint8_t* remove, uint8_t* image, b200ba_outlier_report* report, double* device_ms) {
+  if (!h) return 1;
+  if (!imageset_used || !report) {
+    h->error = "b200ba_delete_outliers: imageset_used and report must not be NULL";
+    return 2;
+  }
+  if (h->comm || h->n_ranks > 1) {
+    h->error = "b200ba_delete_outliers: the handle is joined to a communicator and holds one shard of the "
+               "observations; the outlier round needs all of them (use a single-rank handle)";
+    return 2;
+  }
+  if (camera < 0 || camera >= h->n_cameras) {
+    h->error = "b200ba_delete_outliers: camera index out of range";
+    return 2;
+  }
+  if (!h->have_state) {
+    h->error = "no state: call b200ba_set_state first";
+    return 2;
+  }
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  if (setup_report(h)) return 1;
+  const int nc = h->n_cameras, ni = h->n_imagesets;
+  const b200ba_camera& cam = h->cams_host[camera];
+  int64_t cam_off[2] = {0, 0};
+  CUDA_TRY(h, cudaMemcpy(cam_off, h->rep.cam_off + camera, sizeof(cam_off), cudaMemcpyDeviceToHost));
+  const int64_t a = cam_off[0], n = cam_off[1] - cam_off[0];
+  const int64_t pixels = static_cast<int64_t>(cam.width) * cam.height;
+  const int64_t range[2] = {0, n};
+  OutlierDev d{};
+  CallScope cs(&h->error);
+  cs.alloc(&d.range, 2);
+  cs.alloc(&d.mag, std::max<int64_t>(1, n));
+  cs.alloc(&d.partial, report_partial_size(1));
+  cs.alloc(&d.select_hist, 2 * 256);
+  cs.alloc(&d.stats, 2);
+  cs.alloc(&d.used, std::max(1, ni));
+  cs.alloc(&d.kept, std::max(1, ni));
+  cs.alloc(&d.counts, 2);
+  cs.alloc(&d.remove, std::max<int64_t>(1, h->n_obs));
+  if (image) {
+    cs.alloc(&d.owner, std::max<int64_t>(1, pixels));
+    cs.alloc(&d.image, std::max<int64_t>(1, 3 * pixels));
+  }
+  if (cs.rc == 0) {
+    cs.ok(cudaMemcpyAsync(d.range, range, sizeof(range), cudaMemcpyHostToDevice, h->stream));
+    cs.ok(cudaMemcpyAsync(d.used, imageset_used, ni, cudaMemcpyHostToDevice, h->stream));
+    cs.ok(cudaMemsetAsync(d.kept, 0, sizeof(int) * std::max(1, ni), h->stream));
+    cs.ok(cudaMemsetAsync(d.counts, 0, 2 * sizeof(unsigned long long), h->stream));
+    cs.ok(cudaMemsetAsync(d.remove, 0, h->n_obs, h->stream));
+    if (image) {
+      cs.ok(cudaMemsetAsync(d.owner, 0, sizeof(uint32_t) * pixels, h->stream));
+      cs.ok(cudaMemsetAsync(d.image, 0, 3 * pixels, h->stream));
+    }
+  }
+  ReportCam st[2];
+  unsigned long long counts[2] = {0, 0};
+  if (cs.rc == 0) {
+    Layout L{};
+    L.n_points = h->n_points;
+    L.n_imagesets = ni;
+    L.n_cameras = nc;
+    cs.record(0, h->stream);
+    launch_prepare_state(h->pb, L, h->st[h->cur], h->n_control_total, h->stream);
+    launch_report_errors(h->pb, nc, h->st[h->cur], h->rep, h->stream);
+    launch_delete_outliers(h->pb, ni, h->rep, h->d_perm, a, n, outlier_removal_factor, cam.width, cam.height, d, h->stream);
+    cs.record(1, h->stream);
+    cs.ok(cudaGetLastError());
+    cs.ok(cudaMemcpyAsync(st, d.stats, sizeof(st), cudaMemcpyDeviceToHost, h->stream));
+    cs.ok(cudaMemcpyAsync(counts, d.counts, sizeof(counts), cudaMemcpyDeviceToHost, h->stream));
+    cs.ok(cudaMemcpyAsync(imageset_used, d.used, ni, cudaMemcpyDeviceToHost, h->stream));
+    if (remove && h->n_obs > 0) cs.ok(cudaMemcpyAsync(remove, d.remove, h->n_obs, cudaMemcpyDeviceToHost, h->stream));
+    if (image) cs.ok(cudaMemcpyAsync(image, d.image, 3 * pixels, cudaMemcpyDeviceToHost, h->stream));
+    cs.ok(cudaStreamSynchronize(h->stream));
+  }
+  if (cs.rc == 0) {
+    const bool skipped = st[0].count < 8;
+    report->count = st[0].count;
+    report->q1 = skipped ? nan("") : st[0].median;
+    report->q3 = skipped ? nan("") : st[1].median;
+    report->threshold = skipped ? nan("") : report->q3 + static_cast<double>(outlier_removal_factor) * (report->q3 - report->q1);
+    report->removed = static_cast<int64_t>(counts[0]);
+    report->failed = static_cast<int64_t>(counts[1]);
+    report->skipped = skipped ? 1 : 0;
+    if (device_ms) *device_ms = cs.elapsed_ms(0, 1);
+  }
+  return cs.rc;
+}
+
 int32_t b200ba_degrees_of_freedom(const b200ba_handle* h, const b200ba_options* opt) {
   if (!h || !opt) return -1;
   int n_intr = 0;

@@ -1853,17 +1853,18 @@ __global__ void report_reduce_stage2(int n_cameras, const double* __restrict__ p
 
 // Median (WriteReportInfoFile, :685-693: sorted(|e|)[count / 2]) by radix select on the bit patterns:
 // non-negative doubles order like their uint64 patterns. 8 passes of 8 bits; pass p histograms digit
-// 7 - p of the values whose higher digits equal the prefix chosen so far.
+// 7 - p of the values whose higher digits equal the prefix chosen so far. Every range can select
+// `ranks` ranks at once: slot s = range * ranks + j keeps its own prefix, rank and histogram.
 constexpr int kSelectBlocks = 132;
 __global__ void __launch_bounds__(kReportThreads)
-    report_select_hist_kernel(int pass, const int64_t* __restrict__ cam_off, const double* __restrict__ mag,
+    report_select_hist_kernel(int pass, int ranks, const int64_t* __restrict__ cam_off, const double* __restrict__ mag,
                               const ReportCam* __restrict__ rc, unsigned int* __restrict__ hist) {
-  const int cam = blockIdx.y;
+  const int slot = blockIdx.y, cam = slot / ranks;
   __shared__ unsigned int h[256];
   h[threadIdx.x] = 0;
   __syncthreads();
   const int shift = 56 - 8 * pass;
-  const unsigned long long prefix = rc[cam].select_prefix;
+  const unsigned long long prefix = rc[slot].select_prefix;
   for (int64_t o = cam_off[cam] + blockIdx.x * static_cast<int64_t>(kReportThreads) + threadIdx.x; o < cam_off[cam + 1];
        o += static_cast<int64_t>(kSelectBlocks) * kReportThreads) {
     const double m = mag[o];
@@ -1873,14 +1874,14 @@ __global__ void __launch_bounds__(kReportThreads)
     atomicAdd(&h[(bits >> shift) & 255], 1u);
   }
   __syncthreads();
-  if (h[threadIdx.x]) atomicAdd(&hist[cam * 256 + threadIdx.x], h[threadIdx.x]);
+  if (h[threadIdx.x]) atomicAdd(&hist[slot * 256 + threadIdx.x], h[threadIdx.x]);
 }
-__global__ void report_select_scan_kernel(int pass, int n_cameras, unsigned int* __restrict__ hist,
+__global__ void report_select_scan_kernel(int pass, int n_slots, unsigned int* __restrict__ hist,
                                           ReportCam* __restrict__ rc) {
-  const int cam = threadIdx.x;
-  if (cam >= n_cameras) return;
-  ReportCam& r = rc[cam];
-  unsigned int* h = hist + cam * 256;
+  const int slot = threadIdx.x;
+  if (slot >= n_slots) return;
+  ReportCam& r = rc[slot];
+  unsigned int* h = hist + slot * 256;
   long long k = r.select_rank;
   int digit = 255;
   for (int d = 0; d < 256; ++d) {
@@ -2060,10 +2061,18 @@ void launch_report_statistics(int n_ranges, const int64_t* off, const double* ma
                               unsigned int* select_hist, ReportCam* rc, cudaStream_t s) {
   report_reduce_stage1<<<dim3(kReportBlocks, n_ranges), kReportThreads, 0, s>>>(off, mag, partial);
   report_reduce_stage2<<<1, 32, 0, s>>>(n_ranges, partial, rc);
-  cudaMemsetAsync(select_hist, 0, sizeof(unsigned int) * 256 * n_ranges, s);
+  launch_report_select(n_ranges, 1, off, mag, select_hist, rc, s);
+}
+
+// The radix select of launch_report_statistics alone: rc[range * ranks + j].select_rank (set by the caller, prefix 0)
+// becomes the value of that rank among the non-NaN mag of the range, in .median (its bits in .select_prefix).
+void launch_report_select(int n_ranges, int ranks, const int64_t* off, const double* mag, unsigned int* select_hist,
+                          ReportCam* rc, cudaStream_t s) {
+  cudaMemsetAsync(select_hist, 0, sizeof(unsigned int) * 256 * n_ranges * ranks, s);
   for (int pass = 0; pass < 8; ++pass) {
-    report_select_hist_kernel<<<dim3(kSelectBlocks, n_ranges), kReportThreads, 0, s>>>(pass, off, mag, rc, select_hist);
-    report_select_scan_kernel<<<1, 32, 0, s>>>(pass, n_ranges, select_hist, rc);
+    report_select_hist_kernel<<<dim3(kSelectBlocks, n_ranges * ranks), kReportThreads, 0, s>>>(pass, ranks, off, mag, rc,
+                                                                                              select_hist);
+    report_select_scan_kernel<<<1, 32, 0, s>>>(pass, n_ranges * ranks, select_hist, rc);
   }
 }
 
@@ -2082,6 +2091,113 @@ int report_partial_size(int n_cameras) { return n_cameras * kReportBlocks * 3; }
 void launch_report_errors(const ProblemDev& pb, int n_cameras, const StateDev& st, const ReportDev& r, cudaStream_t s) {
   const int64_t n = pb.n_obs;
   if (n > 0) report_errors_kernel<<<static_cast<unsigned>((n + 127) / 128), 128, 0, s>>>(pb, n_cameras, st, r.err, r.mag);
+}
+
+// ------------------------------------------------------------------------------------------
+// outlier round of one camera (DeleteOutlierFeatures, APP/calibration.cc:62-184) on the report's errors
+// ------------------------------------------------------------------------------------------
+// The camera's observations are the device range [a, a + n). All arithmetic that decides a rank, a
+// threshold or a colour is rounded operation by operation (no contraction), in the reference's order.
+
+// |e| of the observations on used imagesets (NaN where the imageset is unused or Project failed)
+__global__ void outlier_mag_kernel(ProblemDev pb, int64_t a, int64_t n, const double* __restrict__ rmag,
+                                   const uint8_t* __restrict__ used, double* __restrict__ mag) {
+  const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (i >= n) return;
+  mag[i] = used[pb.obs_imageset[a + i]] ? rmag[a + i] : nan("");
+}
+
+// ranks of the quartiles, reprojection_errors[0.25f * size + 0.5f] and [0.75f * size + 0.5f]: float
+// arithmetic, truncated to size_t
+__global__ void outlier_ranks_kernel(ReportCam* __restrict__ st) {
+  const long long count = st[0].count;
+  const float c = static_cast<float>(count);
+  st[1] = st[0];
+  st[0].select_rank = static_cast<long long>(__fadd_rn(__fmul_rn(0.25f, c), 0.5f));
+  st[1].select_rank = static_cast<long long>(__fadd_rn(__fmul_rn(0.75f, c), 0.5f));
+  st[0].select_prefix = st[1].select_prefix = 0;
+}
+
+// threshold = q3 + (double)factor * (q3 - q1)
+__device__ __forceinline__ double outlier_threshold(const ReportCam* st, float factor) {
+  const double q1 = st[0].median, q3 = st[1].median;
+  return __dadd_rn(q3, __dmul_rn(static_cast<double>(factor), __dadd_rn(q3, -q1)));
+}
+
+// the pixel ((u32)x, (u32)y) of a feature, or -1 where a truncated coordinate is outside the image
+__device__ __forceinline__ int64_t outlier_pixel(float2 xy, int w, int h) {
+  const float tx = truncf(xy.x), ty = truncf(xy.y);
+  if (!(tx >= 0.f && tx < static_cast<float>(w) && ty >= 0.f && ty < static_cast<float>(h))) return -1;
+  return static_cast<int64_t>(ty) * w + static_cast<int64_t>(tx);
+}
+
+// remove = !ok || |e| > threshold for the observations on used imagesets; counts kept features per
+// imageset, removed / failed features, and marks each pixel with 1 + the largest caller index removed there
+__global__ void outlier_decide_kernel(ProblemDev pb, int64_t a, int64_t n, const double* __restrict__ rmag,
+                                      const uint32_t* __restrict__ perm, OutlierDev d, float factor, int w, int h) {
+  const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (i >= n || d.stats[0].count < 8) return;
+  const int64_t o = a + i;
+  const uint32_t iset = pb.obs_imageset[o];
+  if (!d.used[iset]) return;
+  const double m = rmag[o];
+  if (!isnan(m) && !(m > outlier_threshold(d.stats, factor))) {
+    atomicAdd(&d.kept[iset], 1);
+    return;
+  }
+  const uint32_t caller = perm[o];
+  d.remove[caller] = 1;
+  atomicAdd(&d.counts[0], 1ull);
+  if (isnan(m)) atomicAdd(&d.counts[1], 1ull);
+  if (d.owner) {
+    const int64_t p = outlier_pixel(pb.obs_xy[o], w, h);
+    if (p >= 0) atomicMax(&d.owner[p], caller + 1);
+  }
+}
+
+// the colour of the last removed feature (caller's order) at every marked pixel
+__global__ void outlier_colour_kernel(ProblemDev pb, int64_t a, int64_t n, const double* __restrict__ rmag,
+                                      const uint32_t* __restrict__ perm, OutlierDev d, int w, int h) {
+  const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (i >= n) return;
+  const int64_t o = a + i;
+  const int64_t p = outlier_pixel(pb.obs_xy[o], w, h);
+  if (p < 0 || d.owner[p] != perm[o] + 1) return;
+  const double m = rmag[o];
+  uint8_t r = 255, g = 255, b = 255;
+  if (isnan(m)) {
+    r = g = b = 127;
+  } else if (m > 10) {
+    g = b = 0;
+  } else if (m > 5) {
+    g = 127;
+    b = 0;
+  } else if (m > 1) {
+    b = 0;
+  }
+  d.image[3 * p] = r;
+  d.image[3 * p + 1] = g;
+  d.image[3 * p + 2] = b;
+}
+
+// imagesets left with fewer than 3 features of the camera become unused
+__global__ void outlier_drop_kernel(int n_imagesets, OutlierDev d) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_imagesets || d.stats[0].count < 8) return;
+  if (d.used[i] && d.kept[i] < 3) d.used[i] = 0;
+}
+
+void launch_delete_outliers(const ProblemDev& pb, int n_imagesets, const ReportDev& r, const uint32_t* perm,
+                            int64_t a, int64_t n, float factor, int w, int h, const OutlierDev& d, cudaStream_t s) {
+  const unsigned blocks = static_cast<unsigned>(std::max<int64_t>(1, (n + 255) / 256));
+  outlier_mag_kernel<<<blocks, 256, 0, s>>>(pb, a, n, r.mag, d.used, d.mag);
+  report_reduce_stage1<<<dim3(kReportBlocks, 1), kReportThreads, 0, s>>>(d.range, d.mag, d.partial);
+  report_reduce_stage2<<<1, 32, 0, s>>>(1, d.partial, d.stats);
+  outlier_ranks_kernel<<<1, 1, 0, s>>>(d.stats);
+  launch_report_select(1, 2, d.range, d.mag, d.select_hist, d.stats, s);
+  outlier_decide_kernel<<<blocks, 256, 0, s>>>(pb, a, n, r.mag, perm, d, factor, w, h);
+  if (d.owner) outlier_colour_kernel<<<blocks, 256, 0, s>>>(pb, a, n, r.mag, perm, d, w, h);
+  outlier_drop_kernel<<<std::max(1, (n_imagesets + 255) / 256), 256, 0, s>>>(n_imagesets, d);
 }
 
 // ------------------------------------------------------------------------------------------

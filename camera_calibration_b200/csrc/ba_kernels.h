@@ -84,6 +84,14 @@ void launch_line_outputs(const CamDev& c, const double center[3], const LineOffs
                          int64_t n_obj, cudaStream_t s);
 // re-projection errors of every observation into r.err / r.mag (the first kernel of launch_calibration_report)
 void launch_report_errors(const ProblemDev& pb, int n_cameras, const StateDev& st, const ReportDev& r, cudaStream_t s);
+// the radix select of the report: rc[range * ranks + j].select_rank of every range [off[k], off[k + 1]) of the non-NaN
+// mag, the value in rc[...].median (n_ranges * ranks <= 32)
+void launch_report_select(int n_ranges, int ranks, const int64_t* off, const double* mag, unsigned int* select_hist,
+                          ReportCam* rc, cudaStream_t s);
+// outlier round of one camera (b200ba_delete_outliers) on the report's errors r.mag (launch_report_errors must have run):
+// the camera is the device range [a, a + n); perm maps device positions to caller indices; w x h is its image size
+void launch_delete_outliers(const ProblemDev& pb, int n_imagesets, const ReportDev& r, const uint32_t* perm,
+                            int64_t a, int64_t n, float factor, int w, int h, const OutlierDev& d, cudaStream_t s);
 // Voronoi coverage rendering of n sites (quarter-pixel int2, kVoronoiNoSite.x = skipped) with nch = 3 or 6 float
 // colours per site into the RGB images img0 (channels 0-2) and img1 (channels 3-5, nch == 6), both [h * w * 3],
 // nullable. g's geometry must be set (voronoi_grid_geometry) and its buffers allocated.

@@ -10,14 +10,17 @@ the ``--compare_calibrations`` tool (``CompareCalibrations``, tools/compare_cali
 ``--compare_reconstructions`` tool (``CompareReconstructions``, tools/bundle_adjustment.cc:223-392) and the calibration
 visualisation tools (``VisualizeKalibrCalibration``, ``VisualizeColmapCalibration``, tools/visualize_calibration.cc;
 ``CreateLegends``, tools/create_legends.cc) and the ``--render_synthetic_dataset`` tool (``RenderSyntheticDataset``,
-tools/render_synthetic_dataset.cc).
+tools/render_synthetic_dataset.cc), and calibration from an existing state (``Calibrate``, calibration.cc:918-1143, with
+the device outlier round ``DeleteOutlierFeaturesOnDevice``, and the tool ``CalibrateFromState``, :1240-1342).
 Host logic only; every numerical step (un-projection, the LM iteration, the report's statistics) runs in
 ``libb200ba.so``.
 """
 from __future__ import annotations
 
 import math
-from typing import Callable, List, Optional
+import sys
+import time
+from typing import Callable, Dict, List, Optional
 
 import numpy as np
 
@@ -200,6 +203,59 @@ def DeleteOutlierFeatures(camera_index: int, dataset: Dataset, state: BAState, o
     return removed
 
 
+def _outlier_round_on_context(ctx, cameras, dataset: Dataset, state: BAState, outlier_removal_factor: float,
+                              outlier_visualization_path: Optional[str]):
+    """The outlier round of ``cameras``, in order, on the device-resident state of ``ctx`` (``b200ba_delete_outliers``),
+    applied to the host containers after each camera. Returns one ``cabi.OutlierReport`` per camera."""
+    import os
+    from . import io
+    used = np.array([bool(state.image_used[i]) for i in ctx.used])
+    reports = []
+    any_removed = False
+    for c in cameras:
+        rep, used, remove, image, _ = ctx.adjuster.delete_outliers(c, outlier_removal_factor, used,
+                                                                   with_image=outlier_visualization_path is not None)
+        reports.append(rep)
+        if rep.skipped:
+            continue
+        for i, cam, a, b in ctx.slices:
+            if cam != c or not remove[a:b].any():
+                continue
+            f = dataset.GetImageset(i).FeaturesOfCamera(c)
+            keep = ~remove[a:b]
+            for key in list(f.keys()):
+                f[key] = f[key][keep]
+        for k, i in enumerate(ctx.used):
+            state.image_used[i] = bool(used[k])
+        any_removed |= rep.removed > 0
+        print(f"Outlier detection removed {rep.removed} outlier features.", file=sys.stderr)
+        if outlier_visualization_path is not None:
+            path = f"{outlier_visualization_path}_camera{c}_removed_outliers.png"
+            if os.path.dirname(path):
+                os.makedirs(os.path.dirname(path), exist_ok=True)
+            if not io.WritePNG(path, image):
+                print(f"Cannot write file: {path}", file=sys.stderr)
+    if any_removed:
+        ctx.adjuster.close()
+        dataset._b200_context = None
+    return reports
+
+
+def DeleteOutlierFeaturesOnDevice(camera_index: int, dataset: Dataset, state: BAState, outlier_removal_factor: float,
+                                  outlier_visualization_path: Optional[str] = None):
+    """DeleteOutlierFeatures (calibration.cc:62-184) for one camera with every step on the device: the report's error
+    pass, the exact quartiles and the removal decisions of ``b200ba_delete_outliers`` on the cached device context of
+    (dataset, state). The result is applied like the reference applies it: the removed features are erased (the
+    survivors keep their order and last_projection), imagesets left with fewer than 3 features of the camera are marked
+    unused, and the cached context is dropped when a feature was removed. With ``outlier_visualization_path``, writes
+    ``<path>_camera<i>_removed_outliers.png`` unless the camera was skipped (fewer than 8 successful projections).
+    Returns the ``cabi.OutlierReport``. (``Calibrate`` runs the round of every camera on the handle that just finished
+    BA, without this upload.)"""
+    ctx = api._report_context(dataset, state)
+    return _outlier_round_on_context(ctx, [camera_index], dataset, state, outlier_removal_factor,
+                                     outlier_visualization_path)[0]
+
+
 def ScaleToMetric(dataset: Dataset, state: BAState) -> float:
     """calibration.cc:307-370: geometric-mean ratio of the known pattern cell length to the
     optimised distance of neighbouring corners (right and down neighbours), applied with
@@ -360,6 +416,218 @@ def ResampleModelsIfNecessary(dataset: Dataset, state: BAState, model_type: Came
                 state.intrinsics[c] = new
                 count += 1
     return count
+
+
+class _Phases:
+    """Wall time per phase of Calibrate (seconds, accumulated), each phase ended by a device synchronisation."""
+
+    def __init__(self, sink: Optional[Dict[str, float]]):
+        self.sink = sink
+
+    def __call__(self, name: str, fn, *args, **kwargs):
+        if self.sink is None:
+            return fn(*args, **kwargs)
+        t0 = time.perf_counter()
+        out = fn(*args, **kwargs)
+        self.sink[name] = self.sink.get(name, 0.0) + time.perf_counter() - t0
+        return out
+
+
+def _device_bundle_adjustment(schur_mode: SchurMode, regularization_weight: float, phases: "_Phases"):
+    """The default BA step of Calibrate: RunBundleAdjustment with the state resident on the device, printing the
+    reference's ``[i] Cost:`` lines. A device context built by the call (``b200ba_create``, where the problem changed)
+    is timed as the phase ``handle build`` and not as BA."""
+    def run(dataset, state, max_iteration_count, cost_reduction_threshold, state_output_path, label):
+        before = getattr(dataset, "_b200_context", None)
+
+        def on_iteration(it, cost):
+            print(f"[{it + 1}] Cost: {cost:g}", file=sys.stderr)
+        costs = phases(label, RunBundleAdjustment, False, schur_mode, max_iteration_count, cost_reduction_threshold,
+                       dataset, state, regularization_weight, False, state_output_path=state_output_path,
+                       on_iteration=on_iteration)
+        ctx = dataset._b200_context
+        if phases.sink is not None and ctx is not before:
+            phases.sink[label] -= ctx.build_seconds
+            phases.sink["handle build"] = phases.sink.get("handle build", 0.0) + ctx.build_seconds
+        return costs
+    return run
+
+
+def _device_outlier_round(dataset, state, outlier_removal_factor, outlier_visualization_path, upload: bool = False):
+    """The default outlier round of Calibrate: every camera on one handle. After the default device BA that handle is
+    the one that just finished BA and holds the state (no upload); after another BA step (``upload``) the state is
+    uploaded first."""
+    if upload:
+        ctx = api._report_context(dataset, state)
+    else:
+        ctx, _ = api._prepare(dataset, state)
+    reports = _outlier_round_on_context(ctx, range(state.num_cameras()), dataset, state, outlier_removal_factor,
+                                        outlier_visualization_path)
+    return [0 if r.skipped else int(r.removed) for r in reports]
+
+
+def Calibrate(dataset: Dataset, state: BAState, model_type: CameraModel.Type, num_pyramid_levels: int = 3,
+              approx_pixels_per_cell: int = 25, regularization_weight: float = 0.0, outlier_removal_factor: float = 6.0,
+              localize_only: bool = False, schur_mode: SchurMode = SchurMode.Dense,
+              outlier_visualization_path: Optional[str] = None, dataset_output_path: Optional[str] = None,
+              state_output_path: Optional[str] = None, run_bundle_adjustment=None, outlier_round=None,
+              fit_fn=None, unproject_many=None, timings: Optional[Dict[str, float]] = None) -> bool:
+    """Calibrate() (calibration.cc:918-1143) from a loaded state, with ``use_cuda = false`` as CalibrateBatch passes:
+      1. fewer than 3 imagesets: refused;
+      2. ResampleModelsIfNecessary on the coarsest pyramid level, then ComputeFeatureIdToPointsIndex;
+      3. the full grid resolution of every camera with a grid;
+      4. per pyramid level above 0: the grid resolutions are checked against CalcGridResolutionForLevel, BA (10, 1e-4)
+         and BA (50, 1), then every gridded camera is resampled to the next level;
+      5. with outlier_removal_factor > 0: BA (100 on a single level, else 10; 1e-4), the outlier round of every camera in
+         order, and the pruned dataset saved to ``dataset_output_path``;
+      6. BA (100, 1e-4); 7. ScaleToMetric.
+    BA steps write the state to ``state_output_path`` after every iteration. Returns True, or False with a message
+    on stderr where the reference CHECKs, aborts or computes garbage: ``localize_only`` (needs the dense
+    initialization's localization), an OpenCV camera that would have to become a generic model (no OpenCV
+    un-projection on the device), a model without a grid when num_pyramid_levels > 1, a grid resolution that a failed
+    resampling left different from the level's, and a dataset without neighbouring known-geometry corners
+    (ScaleToMetric would divide by zero).
+
+    Hooks (default: the device): ``run_bundle_adjustment(dataset, state, max_iteration_count,
+    cost_reduction_threshold, state_output_path, label)`` -> costs, ``outlier_round(dataset, state, factor,
+    outlier_visualization_path)`` -> removed count per camera, and ``fit_fn`` / ``unproject_many`` of
+    ResampleModel. ``timings``: filled with the wall time of each phase."""
+    T = CameraModel.Type
+    model_type = T(model_type)
+    phases = _Phases(timings)
+    if dataset.ImagesetCount() < 3:
+        print(f"Calibration failed: too few input images given ({dataset.ImagesetCount()}), calibration requires at "
+              "least 3. (In practice, many more should be used.)", file=sys.stderr)
+        return False
+    if localize_only:
+        print("Calibrate: localize_only needs the dense initialization's localization, which is not built here.",
+              file=sys.stderr)
+        return False
+    for c, model in enumerate(state.intrinsics):
+        if model.type() == T.CentralOpenCV and model_type != T.CentralOpenCV:
+            print(f"Calibrate: camera {c} is an OpenCV model and would have to be resampled into a generic model, "
+                  "which needs an OpenCV un-projection on the device (not built).", file=sys.stderr)
+            return False
+        if model.type() != model_type and model_type not in (T.CentralGeneric, T.NoncentralGeneric):
+            print(f"Calibrate: camera {c} would have to be fitted by a {model_type.name} model; only the generic "
+                  "models are resampling targets here.", file=sys.stderr)
+            return False
+    run_ba = run_bundle_adjustment or _device_bundle_adjustment(schur_mode, regularization_weight, phases)
+    if outlier_round is None:
+        upload = run_bundle_adjustment is not None
+
+        def outlier_round(dataset, state, factor, path):
+            return _device_outlier_round(dataset, state, factor, path, upload=upload)
+
+    phases("resampling", ResampleModelsIfNecessary, dataset, state, model_type, approx_pixels_per_cell,
+           num_pyramid_levels - 1, fit_fn=fit_fn, unproject_many=unproject_many)
+    state.ComputeFeatureIdToPointsIndex(dataset)
+    full = [ComputeGridResolutionForModel(m, approx_pixels_per_cell) if m.GetGridResolution() else None
+            for m in state.intrinsics]
+    for level in range(num_pyramid_levels - 1, 0, -1):
+        print(f"Bundle adjustment with pyramid level: {level}", file=sys.stderr)
+        for c, model in enumerate(state.intrinsics):
+            if full[c] is None:
+                print(f"Calibrate: camera {c} has a model without a grid, which the pyramid scheme needs; set "
+                      "num_pyramid_levels to 1.", file=sys.stderr)
+                return False
+            want = CalcGridResolutionForLevel(level, *full[c])
+            if tuple(model.GetGridResolution()) != want:
+                print(f"Calibrate: camera {c} has grid resolution {model.GetGridResolution()} on pyramid level {level}, "
+                      f"not {want} (a resampling failed).", file=sys.stderr)
+                return False
+            print(f"Grid resolution on pyramid level {level} for camera {c}: {want[0]} x {want[1]}", file=sys.stderr)
+        run_ba(dataset, state, 10, 1e-4, state_output_path, f"BA level {level}")
+        run_ba(dataset, state, 50, 1.0, state_output_path, f"BA level {level}")
+        for c, model in enumerate(state.intrinsics):
+            target = CalcGridResolutionForLevel(level - 1, *full[c])
+            ok, new = phases("resampling", ResampleModel, model, state.camera_tr_rig[c], model.calibration_min_x(),
+                             model.calibration_min_y(), model.calibration_max_x(), model.calibration_max_y(), model_type,
+                             target[0], target[1], fit_fn=fit_fn, unproject_many=unproject_many)
+            if ok:
+                state.intrinsics[c] = new
+    for c, model in enumerate(state.intrinsics):
+        if full[c] is not None:
+            if tuple(model.GetGridResolution()) != full[c]:
+                print(f"Calibrate: camera {c} has grid resolution {model.GetGridResolution()}, not {full[c]} (a "
+                      "resampling failed).", file=sys.stderr)
+                return False
+            print(f"Bundle adjustment with final grid resolution for camera {c}: {full[c][0]} x {full[c][1]} ...",
+                  file=sys.stderr)
+    if outlier_removal_factor > 0:
+        run_ba(dataset, state, 100 if num_pyramid_levels == 1 else 10, 1e-4, state_output_path, "BA level 0")
+        phases("outlier round", outlier_round, dataset, state, outlier_removal_factor, outlier_visualization_path)
+        if dataset_output_path:
+            from . import io
+            io.SaveDataset(dataset_output_path, dataset)
+    run_ba(dataset, state, 100, 1e-4, state_output_path, "BA level 0")
+    try:
+        ScaleToMetric(dataset, state)
+    except ValueError as e:
+        print(f"Calibrate: {e}", file=sys.stderr)
+        return False
+    return True
+
+
+def CalibrateFromState(dataset_files, state_directory: str, output_directory: str,
+                       model_type=CameraModel.Type.CentralGeneric, num_pyramid_levels: int = 3,
+                       cell_length_in_pixels: int = 25, regularization_weight: float = 0.0,
+                       outlier_removal_factor: float = 6.0, schur_mode: SchurMode = SchurMode.Dense,
+                       timings: Optional[Dict[str, float]] = None, **hooks) -> int:
+    """CalibrateBatch's dataset-file path (calibration.cc:1272-1334) from a state directory: load ``dataset_files`` and
+    merge them in order (Dataset.Merge), load the state, ``Calibrate`` with the state checkpoint in
+    ``output_directory``, then write ``output_directory``'s state, ``dataset.bin`` and the calibration report
+    ``report`` (visualizations and line offsets; the outlier images share its base path). ``model_type`` is a
+    ``CameraModel.Type`` or its name in the reference's flag spelling (``central_generic``, ``noncentral_generic``,
+    ``central_opencv``). ``hooks`` go to Calibrate. Returns EXIT_SUCCESS / EXIT_FAILURE; on failure no final state
+    is written."""
+    import os
+    from . import io
+    if isinstance(model_type, str):
+        names = {"central_generic": CameraModel.Type.CentralGeneric, "noncentral_generic": CameraModel.Type.NoncentralGeneric,
+                 "central_opencv": CameraModel.Type.CentralOpenCV}
+        if model_type not in names:
+            print(f"Model type not handled: {model_type}", file=sys.stderr)
+            return 1
+        model_type = names[model_type]
+    paths = list(dataset_files)
+    if not paths:
+        print("CalibrateFromState needs at least one dataset file", file=sys.stderr)
+        return 1
+    dataset = None
+    for i, path in enumerate(paths):
+        print(f"Dataset {i}: {path}", file=sys.stderr)
+        ds = io.LoadDataset(path)
+        if ds is None:
+            print(f"Cannot read file: {path}", file=sys.stderr)
+            return 1
+        if dataset is None:
+            dataset = ds
+        elif not dataset.Merge(ds):
+            print(f"Cannot merge dataset {path}: its camera count or image sizes differ", file=sys.stderr)
+            return 1
+    state = io.LoadBAState(state_directory)
+    if state is None:
+        print(f"Cannot load state: {state_directory}", file=sys.stderr)
+        return 1
+    if state.num_cameras() != dataset.num_cameras() or len(state.image_used) != dataset.ImagesetCount():
+        print(f"The state in {state_directory} has {state.num_cameras()} cameras and {len(state.image_used)} "
+              f"imagesets, the dataset {dataset.num_cameras()} and {dataset.ImagesetCount()}.", file=sys.stderr)
+        return 1
+    report_base = os.path.join(output_directory, "report")
+    if not Calibrate(dataset, state, model_type, num_pyramid_levels, cell_length_in_pixels, regularization_weight,
+                     outlier_removal_factor, False, schur_mode, outlier_visualization_path=report_base,
+                     dataset_output_path=os.path.join(output_directory, "dataset.bin"),
+                     state_output_path=output_directory, timings=timings, **hooks):
+        print("Calibration failed.", file=sys.stderr)
+        return 1
+    phases = _Phases(timings)
+    if not io.SaveBAState(output_directory, state):
+        print(f"Cannot write the state to: {output_directory}", file=sys.stderr)
+        return 1
+    io.SaveDataset(os.path.join(output_directory, "dataset.bin"), dataset)
+    phases("report", CreateCalibrationReport, dataset, state, report_base, visualizations=True, line_offsets=True)
+    return 0
 
 
 def BundleAdjustment(state_directory: str, model_input_directory: str, model_output_directory: str,

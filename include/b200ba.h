@@ -257,6 +257,36 @@ B200BA_API int b200ba_report_images(b200ba_handle* h, int32_t camera, uint8_t* o
                                     uint8_t* error_directions, uint8_t* error_magnitudes, int64_t* n_sites,
                                     double* device_ms);
 
+/* ---- outlier round ------------------------------------------------------------ */
+/* DeleteOutlierFeatures (calibration.cc:62-184) for one camera, on the state held by the handle. Every observation
+ * of `camera` on an imageset with imageset_used[i] != 0 gets |e| from the report's error pass (bit-identical to
+ * b200ba_calibration_report's errors). With count = the successful projections among them:
+ *   count < 8        nothing is removed, imageset_used and remove stay as they are, image stays black; skipped = 1.
+ *   otherwise        q1, q3 are the exact k-th smallest |e| (0-based), k = (size_t)(0.25f * (float)count + 0.5f)
+ *                    and (size_t)(0.75f * (float)count + 0.5f) in float arithmetic; threshold = q3 + (double)factor
+ *                    * (q3 - q1); a feature is removed where Project fails or |e| > threshold; every used imageset
+ *                    with fewer than 3 kept features of the camera (0 included) becomes unused.
+ * imageset_used  [n_imagesets of the handle] in / out. Callers that process several cameras pass it from one camera
+ *                to the next, so a later camera's statistics exclude the imagesets an earlier one dropped.
+ * remove         [n_obs] out, caller order, nullable: 1 for a removed observation, 0 otherwise.
+ * image          [h*w*3] out, nullable: `<base>_camera<i>_removed_outliers.png`. Black; every removed feature
+ *                colours the pixel ((u32)x, (u32)y) (truncation), the one latest in the caller's order winning:
+ *                grey 127 where Project failed, else |e| > 10 red, > 5 (255,127,0), > 1 (255,255,0), else white.
+ *                A feature whose truncated x or y is outside [0, w) x [0, h) colours nothing (the reference
+ *                writes out of bounds there); -1 < x < 0 truncates to 0 and is drawn.
+ * device_ms (nullable): device time. Reads the state and writes none of it (nor last_projection). Single-rank
+ * handles only; returns 2 for a bad camera index, NULL imageset_used or report, or no state. */
+typedef struct b200ba_outlier_report {
+  int64_t count;                /* successful projections on used imagesets */
+  double q1, q3, threshold;     /* NaN when skipped */
+  int64_t removed;              /* removed features, failed projections included */
+  int64_t failed;               /* removed because Project failed */
+  int32_t skipped;              /* 1: count < 8, nothing removed */
+} b200ba_outlier_report;
+B200BA_API int b200ba_delete_outliers(b200ba_handle* h, int32_t camera, float outlier_removal_factor,
+                                      uint8_t* imageset_used, uint8_t* remove, uint8_t* image,
+                                      b200ba_outlier_report* report, double* device_ms);
+
 /* ---- building blocks, exposed for parity tests and profiling -------------- */
 /* One pass of JointOptimizationCostFunction::Compute<compute_jacobians>
  * (joint_optimization.cc:240-306) at the current state.

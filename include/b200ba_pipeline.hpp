@@ -1,5 +1,5 @@
 // b200ba_pipeline.hpp -- C++ host logic of the callers either side of the hot path (SURVEY.md 8f-3 / 8f-4):
-// the outlier deletion between bundle-adjustment rounds, the metric rescaling, the pyramid resampling of the generic
+// the outlier deletion between bundle-adjustment rounds (host-driven, and on the device), the metric rescaling, the pyramid resampling of the generic
 // models, the calibration report's info files, the comparison of two calibrations, the localization accuracy test and
 // the --bundle_adjustment / --compare_reconstructions tools, the calibration visualisation tools and the
 // --render_synthetic_dataset tool, over the containers of
@@ -12,6 +12,7 @@
 
 #include <algorithm>
 #include <cmath>
+#include <cstdio>
 #include <cstdlib>
 #include <filesystem>
 #include <fstream>
@@ -110,6 +111,101 @@ inline int DeleteOutlierFeatures(int camera_index, Dataset* dataset, BAState* st
     if (kept < 3) state->image_used[span.imageset] = false;
   }
   return removed;
+}
+
+namespace detail {
+// b200ba_create on a flattening (problem arrays point into f)
+inline b200ba_handle* create_handle(Flat& f, size_t n_points) {
+  b200ba_problem pb{};
+  pb.n_cameras = static_cast<int32_t>(f.cams.size());
+  pb.cameras = f.cams.data();
+  pb.n_imagesets = static_cast<int32_t>(f.used.size());
+  pb.n_points = static_cast<int32_t>(n_points);
+  pb.n_obs = static_cast<int64_t>(f.oi.size());
+  pb.obs_imageset = f.oi.data();
+  pb.obs_camera = f.oc.data();
+  pb.obs_point = f.op.data();
+  pb.obs_xy = f.oxy.data();
+  b200ba_handle* h = nullptr;
+  if (b200ba_create(&pb, -1, &h) != 0) throw std::runtime_error(std::string("b200ba_create: ") + b200ba_last_error(nullptr));
+  return h;
+}
+// the state held in f (after b200ba_get_state) back into the containers: poses, points, last_projection; the intrinsics
+// were written in place through flat_intrinsics()
+inline void read_back(const Flat& f, Dataset* dataset, BAState* state) {
+  for (size_t c = 0; c < state->camera_tr_rig.size(); ++c) state->camera_tr_rig[c] = pose_at(f.ctr, c);
+  for (size_t s = 0; s < f.used.size(); ++s) state->rig_tr_global[f.used[s]] = pose_at(f.rtg, s);
+  for (size_t p = 0; p < state->points.size(); ++p) state->points[p] = Vec3d{f.points[3 * p], f.points[3 * p + 1], f.points[3 * p + 2]};
+  size_t o = 0;
+  for (size_t seq = 0; seq < f.used.size(); ++seq)
+    for (int c = 0; c < dataset->num_cameras(); ++c)
+      for (PointFeature& ft : dataset->GetImageset(f.used[seq])->FeaturesOfCamera(c)) {
+        ft.last_projection = Vec2d{f.lastp[2 * o], f.lastp[2 * o + 1]};
+        ++o;
+      }
+}
+// The outlier round of `cameras`, in order, on one handle with the state uploaded once: b200ba_delete_outliers per
+// camera with imageset_used carried from one camera to the next, the reference's count line and image per camera that
+// is not skipped, then the removals and the imageset rule applied to the containers.
+inline std::vector<b200ba_outlier_report> outlier_round(const std::vector<int>& cameras, Dataset* dataset, BAState* state,
+                                                        float outlier_removal_factor, const char* outlier_visualization_path) {
+  Flat f;
+  flatten(*dataset, state, &f);
+  b200ba_handle* h = create_handle(f, state->points.size());
+  b200ba_state st{f.points.data(), f.rtg.data(), f.ctr.data(), f.intr.data(), f.lastp.data()};
+  std::vector<uint8_t> used(std::max<size_t>(f.used.size(), 1), 1), remove(std::max<size_t>(f.oi.size(), 1), 0),
+      removed_any(f.oi.size(), 0);
+  std::vector<b200ba_outlier_report> reports;
+  int rc = b200ba_set_state(h, &st);
+  for (size_t k = 0; rc == 0 && k < cameras.size(); ++k) {
+    const int camera = cameras[k];
+    const bool in_range = camera >= 0 && camera < static_cast<int>(state->intrinsics.size());
+    const bool with_image = outlier_visualization_path != nullptr && in_range;
+    const CameraModel* cam = in_range ? state->intrinsics[camera].get() : nullptr;
+    std::vector<uint8_t> image(with_image ? 3 * static_cast<size_t>(cam->width()) * cam->height() : 0);
+    b200ba_outlier_report report{};
+    rc = b200ba_delete_outliers(h, camera, outlier_removal_factor, used.data(), remove.data(),
+                                with_image ? image.data() : nullptr, &report, nullptr);
+    if (rc) break;
+    reports.push_back(report);
+    if (report.skipped) continue;
+    for (size_t o = 0; o < f.oi.size(); ++o) removed_any[o] |= remove[o];
+    std::cerr << "Outlier detection removed " << report.removed << " outlier features." << std::endl;
+    if (with_image) {
+      const std::string path = std::string(outlier_visualization_path) + "_camera" + std::to_string(camera) + "_removed_outliers.png";
+      const std::filesystem::path parent = std::filesystem::path(path).parent_path();
+      if (!parent.empty()) std::filesystem::create_directories(parent);
+      if (!WritePNG(path, cam->width(), cam->height(), 3, image.data())) std::cerr << "Cannot write file: " << path << std::endl;
+    }
+  }
+  const std::string err = rc ? b200ba_last_error(h) : "";
+  b200ba_destroy(h);
+  if (rc) throw std::runtime_error("b200ba_delete_outliers: " + err);
+  size_t o = 0;
+  for (size_t seq = 0; seq < f.used.size(); ++seq)
+    for (int c = 0; c < dataset->num_cameras(); ++c) {
+      std::vector<PointFeature>& features = dataset->GetImageset(f.used[seq])->FeaturesOfCamera(c);
+      size_t kept = 0;
+      for (size_t j = 0; j < features.size(); ++j, ++o)
+        if (!removed_any[o]) features[kept++] = features[j];
+      features.resize(kept);
+    }
+  for (size_t seq = 0; seq < f.used.size(); ++seq) state->image_used[f.used[seq]] = used[seq] != 0;
+  return reports;
+}
+}  // namespace detail
+
+// DeleteOutlierFeatures (calibration.cc:62-184) for one camera with every step in the library: one handle on the
+// flattening OptimizeJointly uses, one b200ba_delete_outliers (the report's error pass, the exact quartiles, the
+// decisions). The removed features are erased (the survivors keep their order and last_projection), imagesets left with
+// fewer than 3 features of the camera are marked unused and, with outlier_visualization_path and unless the camera was
+// skipped (fewer than 8 successful projections), <path>_camera<i>_removed_outliers.png is written. Prints the
+// reference's count line to stderr when the camera is not skipped. Returns the library's report; throws on a library
+// error. The Python mirror is pipeline.DeleteOutlierFeaturesOnDevice.
+inline b200ba_outlier_report DeleteOutlierFeaturesOnDevice(int camera_index, Dataset* dataset, BAState* state,
+                                                           float outlier_removal_factor,
+                                                           const char* outlier_visualization_path = nullptr) {
+  return detail::outlier_round({camera_index}, dataset, state, outlier_removal_factor, outlier_visualization_path)[0];
 }
 
 // calibration.cc:307-370 -- geometric-mean ratio of the known pattern cell length to the optimised distance of
@@ -594,6 +690,258 @@ inline std::vector<b200ba_camera_report> CreateCalibrationReport(const Dataset& 
       throw std::runtime_error("CreateCalibrationReport: cannot write the line-offset files of " + base);
   }
   return reports;
+}
+
+// ---- calibration from a state ----------------------------------------------------------------------------------
+// RunBundleAdjustment (calibration.cc:187-304) as Calibrate runs it: one handle, the device-resident loop of
+// b200ba_run_bundle_adjustment, the reference's "[i] Cost:" line on stderr and, with state_output_path, the state
+// directory written after every iteration (the reference's checkpoint). Returns the cost after each iteration.
+inline std::vector<double> RunBundleAdjustmentWithCheckpoints(SchurMode schur_mode, int max_iteration_count,
+                                                              double cost_reduction_threshold, Dataset* dataset, BAState* state,
+                                                              double regularization_weight, const char* state_output_path) {
+  detail::Flat f;
+  detail::flatten(*dataset, state, &f);
+  b200ba_handle* h = detail::create_handle(f, state->points.size());
+  b200ba_state st{f.points.data(), f.rtg.data(), f.ctr.data(), f.intr.data(), f.lastp.data()};
+  b200ba_options opt;
+  b200ba_default_options(&opt);
+  opt.max_iteration_count = 1;
+  opt.init_lambda = -1;             // calibration.cc:203
+  opt.numerical_diff_delta = 1e-4;  // calibration.cc:201
+  opt.regularization_weight = regularization_weight;
+  opt.localize_only = 0;
+  opt.eliminate_points = 0;  // the product passes false (calibration.cc:232)
+  opt.schur_mode = static_cast<int32_t>(schur_mode);
+  opt.print_progress = 0;
+  struct Ctx {
+    b200ba_handle* h;
+    b200ba_state* st;
+    detail::Flat* f;
+    Dataset* dataset;
+    BAState* state;
+    const char* path;
+    std::vector<double> costs;
+    bool failed;
+  } ctx{h, &st, &f, dataset, state, state_output_path, {}, false};
+  auto on_iteration = [](void* user, int32_t iteration, double cost) -> int {
+    Ctx* c = static_cast<Ctx*>(user);
+    c->costs.push_back(cost);
+    if (c->path) {
+      if (b200ba_get_state(c->h, c->st) != 0) {
+        c->failed = true;
+        return 1;
+      }
+      detail::read_back(*c->f, c->dataset, c->state);
+      SaveBAState(c->path, *c->state);
+    }
+    std::fprintf(stderr, "[%d] Cost: %g\n", iteration + 1, cost);
+    return 0;
+  };
+  b200ba_ba_report rep;
+  int rc = b200ba_set_state(h, &st);
+  if (rc == 0) rc = b200ba_run_bundle_adjustment(h, &opt, max_iteration_count, cost_reduction_threshold, &rep, on_iteration, &ctx);
+  if (rc == 0 && ctx.failed) rc = 1;
+  if (rc == 0) rc = b200ba_get_state(h, &st);
+  const std::string err = rc ? b200ba_last_error(h) : "";
+  b200ba_destroy(h);
+  if (rc) throw std::runtime_error("b200ba_run_bundle_adjustment: " + err);
+  detail::read_back(f, dataset, state);
+  return ctx.costs;
+}
+
+// (dataset, state, max_iteration_count, cost_reduction_threshold, state_output_path): one RunBundleAdjustment of Calibrate
+using CalibrateBundleAdjustment = std::function<void(Dataset*, BAState*, int, double, const char*)>;
+// (dataset, state, outlier_removal_factor, outlier_visualization_path): the outlier round of every camera
+using CalibrateOutlierRound = std::function<void(Dataset*, BAState*, float, const char*)>;
+
+namespace detail {
+inline const char* model_type_name(CameraModel::Type t) {
+  switch (t) {
+    case CameraModel::Type::CentralGeneric: return "CentralGeneric";
+    case CameraModel::Type::NoncentralGeneric: return "NoncentralGeneric";
+    case CameraModel::Type::CentralRadial: return "CentralRadial";
+    case CameraModel::Type::CentralThinPrismFisheye: return "CentralThinPrismFisheye";
+    case CameraModel::Type::CentralOpenCV: return "CentralOpenCV";
+    default: return "InvalidType";
+  }
+}
+inline std::string resolution_text(int x, int y) { return "(" + std::to_string(x) + ", " + std::to_string(y) + ")"; }
+}  // namespace detail
+
+// Calibrate() (calibration.cc:918-1143) from a loaded state, with use_cuda = false as CalibrateBatch passes: the same
+// schedule, messages and refusals as pipeline.Calibrate (its docstring lists them). The defaults of the hooks run every
+// numerical step in the library: BA through RunBundleAdjustmentWithCheckpoints, the outlier round of every camera on one
+// handle (detail::outlier_round), the resampling through b200ba_unproject / b200ba_fit_directions.
+inline bool Calibrate(Dataset* dataset, BAState* state, CameraModel::Type model_type, int num_pyramid_levels = 3,
+                      int approx_pixels_per_cell = 25, double regularization_weight = 0, float outlier_removal_factor = 6,
+                      bool localize_only = false, SchurMode schur_mode = SchurMode::Dense,
+                      const char* outlier_visualization_path = nullptr, const char* dataset_output_path = nullptr,
+                      const char* state_output_path = nullptr, CalibrateBundleAdjustment run_bundle_adjustment = nullptr,
+                      CalibrateOutlierRound outlier_round = nullptr, const UnprojectMany& unproject_many = UnprojectManyOnDevice,
+                      const FitGridPoints& fit = FitGridPointsOnDevice) {
+  using T = CameraModel::Type;
+  if (dataset->ImagesetCount() < 3) {
+    std::cerr << "Calibration failed: too few input images given (" << dataset->ImagesetCount()
+              << "), calibration requires at least 3. (In practice, many more should be used.)" << std::endl;
+    return false;
+  }
+  if (localize_only) {
+    std::cerr << "Calibrate: localize_only needs the dense initialization's localization, which is not built here." << std::endl;
+    return false;
+  }
+  for (int c = 0; c < state->num_cameras(); ++c) {
+    const T type = state->intrinsics[c]->type();
+    if (type == T::CentralOpenCV && model_type != T::CentralOpenCV) {
+      std::cerr << "Calibrate: camera " << c << " is an OpenCV model and would have to be resampled into a generic model, "
+                   "which needs an OpenCV un-projection on the device (not built)." << std::endl;
+      return false;
+    }
+    if (type != model_type && model_type != T::CentralGeneric && model_type != T::NoncentralGeneric) {
+      std::cerr << "Calibrate: camera " << c << " would have to be fitted by a " << detail::model_type_name(model_type)
+                << " model; only the generic models are resampling targets here." << std::endl;
+      return false;
+    }
+  }
+  if (!run_bundle_adjustment)
+    run_bundle_adjustment = [&](Dataset* ds, BAState* st, int max_iteration_count, double threshold, const char* path) {
+      RunBundleAdjustmentWithCheckpoints(schur_mode, max_iteration_count, threshold, ds, st, regularization_weight, path);
+    };
+  if (!outlier_round)
+    outlier_round = [](Dataset* ds, BAState* st, float factor, const char* path) {
+      std::vector<int> cameras(st->num_cameras());
+      for (int c = 0; c < st->num_cameras(); ++c) cameras[c] = c;
+      detail::outlier_round(cameras, ds, st, factor, path);
+    };
+  ResampleModelsIfNecessary(*dataset, state, model_type, approx_pixels_per_cell, num_pyramid_levels - 1, unproject_many, fit);
+  state->ComputeFeatureIdToPointsIndex(dataset);
+  const int nc = state->num_cameras();
+  std::vector<int> full_x(nc, -1), full_y(nc, -1);
+  for (int c = 0; c < nc; ++c) {
+    const CameraModel& m = *state->intrinsics[c];
+    int rx, ry;
+    if (m.GetGridResolution(&rx, &ry))
+      ComputeGridResolution(m.calibration_max_x() - m.calibration_min_x() + 1, m.calibration_max_y() - m.calibration_min_y() + 1, 1,
+                            approx_pixels_per_cell, &full_x[c], &full_y[c]);
+  }
+  for (int level = num_pyramid_levels - 1; level > 0; --level) {
+    std::cerr << "Bundle adjustment with pyramid level: " << level << std::endl;
+    for (int c = 0; c < nc; ++c) {
+      if (full_x[c] < 0) {
+        std::cerr << "Calibrate: camera " << c << " has a model without a grid, which the pyramid scheme needs; set "
+                     "num_pyramid_levels to 1." << std::endl;
+        return false;
+      }
+      int want_x, want_y, rx = 0, ry = 0;
+      CalcGridResolutionForLevel(level, full_x[c], full_y[c], &want_x, &want_y);
+      state->intrinsics[c]->GetGridResolution(&rx, &ry);
+      if (rx != want_x || ry != want_y) {
+        std::cerr << "Calibrate: camera " << c << " has grid resolution " << detail::resolution_text(rx, ry) << " on pyramid level "
+                  << level << ", not " << detail::resolution_text(want_x, want_y) << " (a resampling failed)." << std::endl;
+        return false;
+      }
+      std::cerr << "Grid resolution on pyramid level " << level << " for camera " << c << ": " << want_x << " x " << want_y << std::endl;
+    }
+    run_bundle_adjustment(dataset, state, 10, 1e-4, state_output_path);
+    run_bundle_adjustment(dataset, state, 50, 1.0, state_output_path);
+    for (int c = 0; c < nc; ++c) {
+      CameraModel& model = *state->intrinsics[c];
+      int target_x, target_y;
+      CalcGridResolutionForLevel(level - 1, full_x[c], full_y[c], &target_x, &target_y);
+      std::shared_ptr<CameraModel> fresh = ResampleModel(model, model.calibration_min_x(), model.calibration_min_y(),
+                                                         model.calibration_max_x(), model.calibration_max_y(), model_type,
+                                                         target_x, target_y, unproject_many, fit);
+      if (fresh) state->intrinsics[c] = fresh;
+    }
+  }
+  for (int c = 0; c < nc; ++c) {
+    if (full_x[c] < 0) continue;
+    int rx = 0, ry = 0;
+    state->intrinsics[c]->GetGridResolution(&rx, &ry);
+    if (rx != full_x[c] || ry != full_y[c]) {
+      std::cerr << "Calibrate: camera " << c << " has grid resolution " << detail::resolution_text(rx, ry) << ", not "
+                << detail::resolution_text(full_x[c], full_y[c]) << " (a resampling failed)." << std::endl;
+      return false;
+    }
+    std::cerr << "Bundle adjustment with final grid resolution for camera " << c << ": " << full_x[c] << " x " << full_y[c]
+              << " ..." << std::endl;
+  }
+  if (outlier_removal_factor > 0) {
+    run_bundle_adjustment(dataset, state, num_pyramid_levels == 1 ? 100 : 10, 1e-4, state_output_path);
+    outlier_round(dataset, state, outlier_removal_factor, outlier_visualization_path);
+    if (dataset_output_path) SaveDataset(dataset_output_path, *dataset);
+  }
+  run_bundle_adjustment(dataset, state, 100, 1e-4, state_output_path);
+  try {
+    ScaleToMetric(*dataset, state);
+  } catch (const std::runtime_error&) {
+    std::cerr << "Calibrate: ScaleToMetric: no neighbouring corners with known geometry (the reference divides by zero here)"
+              << std::endl;
+    return false;
+  }
+  return true;
+}
+
+// CalibrateBatch's dataset-file path (calibration.cc:1272-1334) from a state directory, like pipeline.CalibrateFromState
+// (same messages, same files): load and merge dataset_files in order, load the state, Calibrate with the checkpoint in
+// output_directory, then write output_directory's state, dataset.bin and the report (visualizations and line offsets;
+// the outlier images share its base path). model_type in the reference's flag spelling: central_generic,
+// noncentral_generic or central_opencv. Returns EXIT_SUCCESS / EXIT_FAILURE; on failure no final state is written.
+inline int CalibrateFromState(const std::vector<std::string>& dataset_files, const std::string& state_directory,
+                              const std::string& output_directory, const std::string& model_type = "central_generic",
+                              int num_pyramid_levels = 3, int cell_length_in_pixels = 25, double regularization_weight = 0,
+                              float outlier_removal_factor = 6, SchurMode schur_mode = SchurMode::Dense) {
+  using T = CameraModel::Type;
+  T type;
+  if (model_type == "central_generic") type = T::CentralGeneric;
+  else if (model_type == "noncentral_generic") type = T::NoncentralGeneric;
+  else if (model_type == "central_opencv") type = T::CentralOpenCV;
+  else {
+    std::cerr << "Model type not handled: " << model_type << std::endl;
+    return EXIT_FAILURE;
+  }
+  if (dataset_files.empty()) {
+    std::cerr << "CalibrateFromState needs at least one dataset file" << std::endl;
+    return EXIT_FAILURE;
+  }
+  std::shared_ptr<Dataset> dataset;
+  for (size_t i = 0; i < dataset_files.size(); ++i) {
+    std::cerr << "Dataset " << i << ": " << dataset_files[i] << std::endl;
+    std::shared_ptr<Dataset> ds;
+    if (!LoadDataset(dataset_files[i].c_str(), &ds)) {
+      std::cerr << "Cannot read file: " << dataset_files[i] << std::endl;
+      return EXIT_FAILURE;
+    }
+    if (!dataset) {
+      dataset = ds;
+    } else if (!dataset->Merge(*ds)) {
+      std::cerr << "Cannot merge dataset " << dataset_files[i] << ": its camera count or image sizes differ" << std::endl;
+      return EXIT_FAILURE;
+    }
+  }
+  BAState state;
+  if (!LoadBAState(state_directory.c_str(), &state, nullptr)) {
+    std::cerr << "Cannot load state: " << state_directory << std::endl;
+    return EXIT_FAILURE;
+  }
+  if (state.num_cameras() != dataset->num_cameras() || static_cast<int>(state.image_used.size()) != dataset->ImagesetCount()) {
+    std::cerr << "The state in " << state_directory << " has " << state.num_cameras() << " cameras and " << state.image_used.size()
+              << " imagesets, the dataset " << dataset->num_cameras() << " and " << dataset->ImagesetCount() << "." << std::endl;
+    return EXIT_FAILURE;
+  }
+  const std::string report_base = (std::filesystem::path(output_directory) / "report").string();
+  const std::string dataset_path = (std::filesystem::path(output_directory) / "dataset.bin").string();
+  if (!Calibrate(dataset.get(), &state, type, num_pyramid_levels, cell_length_in_pixels, regularization_weight,
+                 outlier_removal_factor, false, schur_mode, report_base.c_str(), dataset_path.c_str(), output_directory.c_str())) {
+    std::cerr << "Calibration failed." << std::endl;
+    return EXIT_FAILURE;
+  }
+  if (!SaveBAState(output_directory.c_str(), state)) {
+    std::cerr << "Cannot write the state to: " << output_directory << std::endl;
+    return EXIT_FAILURE;
+  }
+  SaveDataset(dataset_path.c_str(), *dataset);
+  CreateCalibrationReport(*dataset, state, report_base, true, true);
+  return EXIT_SUCCESS;
 }
 
 // ---- comparison of two calibrations ----------------------------------------------------------------------------

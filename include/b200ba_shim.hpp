@@ -10,6 +10,7 @@
 // Header-only; link with -lb200ba. No CPU fallback: errors are returned, not hidden.
 #pragma once
 
+#include <algorithm>
 #include <cmath>
 #include <cstdint>
 #include <memory>
@@ -208,6 +209,33 @@ class Dataset {
   std::shared_ptr<const Imageset> GetImageset(int i) const { return m_imagesets[i]; }
   int ImagesetCount() const { return static_cast<int>(m_imagesets.size()); }
   int num_cameras() const { return m_num_cameras; }
+  // dataset.cc:78-130: appends the imagesets and known geometries of `other`; false (nothing changed) where the camera
+  // counts or image sizes differ. The feature ids of `other` and of its geometries are offset by 1 + the largest id of
+  // this dataset's geometries (1 without any), so every geometry stays separate.
+  bool Merge(const Dataset& other) {
+    if (m_num_cameras != other.m_num_cameras || m_image_sizes != other.m_image_sizes) return false;
+    int max_feature_id = 0;
+    for (const KnownGeometry& g : m_known_geometries)
+      for (const auto& entry : g.feature_id_to_position) max_feature_id = std::max(max_feature_id, entry.first);
+    const int offset = max_feature_id + 1;
+    for (const KnownGeometry& g : other.m_known_geometries) {
+      KnownGeometry kg;
+      kg.cell_length_in_meters = g.cell_length_in_meters;
+      for (const auto& entry : g.feature_id_to_position) kg.feature_id_to_position.emplace_back(entry.first + offset, entry.second);
+      m_known_geometries.push_back(kg);
+    }
+    first_imageset_indices_for_datasets.push_back(ImagesetCount());
+    for (const std::shared_ptr<Imageset>& src : other.m_imagesets) {
+      std::shared_ptr<Imageset> s = NewImageset();
+      s->SetFilename(src->GetFilename());
+      for (int c = 0; c < m_num_cameras; ++c) {
+        s->FeaturesOfCamera(c) = src->FeaturesOfCamera(c);
+        for (PointFeature& f : s->FeaturesOfCamera(c)) f.id += offset;
+      }
+    }
+    return true;
+  }
+  std::vector<int> first_imageset_indices_for_datasets{0};
  private:
   int m_num_cameras;
   std::vector<std::pair<int, int>> m_image_sizes;

@@ -165,7 +165,7 @@ class BundleAdjuster:
         """One LM attempt's linear solve at the current state (``b200ba_debug_solve_step``): the reduced
         system ``S`` (n_d x n_d, lower triangle valid) and right-hand side ``rhs`` the dense factorisation
         receives, the update ``x``, and (``with_system``) ``H``, ``b`` of the same build. ``lam`` < 0: the LM's
-        first lambda. ``info`` names the path taken and the dense-phase variants in effect."""
+        first lambda. ``info`` names the path taken."""
         n = self.degrees_of_freedom(opt)
         H = np.zeros((n, n)) if with_system else None
         b = np.zeros(n) if with_system else None
@@ -179,9 +179,8 @@ class BundleAdjuster:
         _check(self.lib.b200ba_debug_solve_step(self._h, C.byref(opt), float(lam), n, None if H is None else _dp(H),
                                                 None if b is None else _dp(b), _dp(S), _dp(rhs), _dp(x),
                                                 C.byref(lam_used), info.ctypes.data_as(C.POINTER(C.c_int32))), self._h)
-        names = ("spd", "use_grouped", "n_groups", "gemm", "panel", "trsv", "aux", "nb")
-        return {"H": H, "b": b, "S": S, "rhs": rhs, "x": x, "lambda": lam_used.value, "nbd": nbd,
-                "info": {k: int(v) for k, v in zip(names, info)}}
+        info = {k: int(info[i]) for i, k in ((0, "spd"), (1, "use_grouped"), (2, "n_groups"), (7, "nb"))}
+        return {"H": H, "b": b, "S": S, "rhs": rhs, "x": x, "lambda": lam_used.value, "nbd": nbd, "info": info}
 
     def debug_apply_update(self, opt: Options, x) -> FlatState:
         """The retraction of one LM attempt (``b200ba_debug_apply_update``): the current state minus the update

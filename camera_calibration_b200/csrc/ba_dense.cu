@@ -3,7 +3,7 @@
 // The reduced system of the Schur-complement solve (LV/lm_optimizer.h:1246-1369) is formed and
 // factorised with the kernels of this file instead of library calls:
 //
-//   dgemm_nt_kernel     C (+)= alpha * A B^T on 128 x 64 (default) or 128 x 128 tiles, 32 x 32 warp tiles, FP64
+//   dgemm_nt_kernel     C (+)= alpha * A B^T on 128 x 64 tiles, 32 x 32 warp tiles, FP64
 //                       `mma.sync.m16n8k4` (SASS DMMA.16x8x4), operands staged through shared memory
 //                       by a 4-stage cp.async pipeline. One kernel, three uses:
 //                         * LOWER + plain epilogue: trailing update S22 -= L21 L21^T of the blocked Cholesky
@@ -14,7 +14,8 @@
 //                           compact panel of one group of Schur blocks, scattered straight into S through
 //                           the group's column list (the reference contracts with Eigen / cublasXtDgemm,
 //                           LV/lm_optimizer.h:1328,1371-1430) -- no m_g x m_g temporary, no scatter pass.
-//   potrf_tile_kernel   Cholesky of one 128 x 128 diagonal tile in shared memory + its explicit inverse.
+//   potrf_trinv_tile_kernel
+//                       Cholesky of one 128 x 128 diagonal tile + its explicit inverse (ba_tile.cuh).
 //   small helpers       lambda on the diagonal, column-block copies.
 //
 // All operands of dgemm_nt are "k-strided": element (i, k) of A lives at A[k * lda + i] (i contiguous),
@@ -23,7 +24,6 @@
 
 #include <algorithm>
 #include <cstdio>
-#include <cstdlib>
 
 #include "ba_kernels.h"
 #include "ba_tile.cuh"
@@ -126,10 +126,10 @@ struct TileLoader {
 }  // namespace
 
 // C(i, j) at Cbase + col_off(j) + i, where col_off maps a column to its storage offset (see DenseMap).
-// CTA tile 128 x BN_ (BN_ = 128: 16 warps, one CTA per SM; BN_ = 64: 8 warps, two CTAs per SM so that one
-// CTA's read-modify-write epilogue overlaps the other's tensor-core main loop).
+// CTA tile 128 x BN_ (instantiated at BN_ = 64: 8 warps, two CTAs per SM so that one CTA's read-modify-write
+// epilogue overlaps the other's tensor-core main loop).
 template <bool LOWER, int EPI, int BN_, int BK, int STAGES>
-__global__ void __launch_bounds__(gemm_threads(BN_), BN_ == 64 ? 2 : 1) dgemm_nt_kernel(GemmArgs g) {
+__global__ void __launch_bounds__(gemm_threads(BN_), 2) dgemm_nt_kernel(GemmArgs g) {
   constexpr int THREADS = gemm_threads(BN_);
   constexpr int LDB = BN_ + 4;
   extern __shared__ __align__(16) double smem_d[];
@@ -138,8 +138,7 @@ __global__ void __launch_bounds__(gemm_threads(BN_), BN_ == 64 ? 2 : 1) dgemm_nt
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int wm = (warp & 3) * 32, wn = (warp >> 2) * 32;  // warp tile 32 (m) x 32 (n)
   const int lr = lane >> 2, lc = lane & 3;
-  // Persistent CTAs: the grid is capped (launch_dgemm_nt leaves a few SMs to the panel stream of the
-  // factorisation, whose small kernels would otherwise queue behind whole tiles) and every CTA walks the
+  // Persistent CTAs (unless one_tile_per_cta): the grid is capped at two CTAs per SM and every CTA walks the
   // tile list with stride gridDim.x. LOWER: only the tiles that intersect i >= j, enumerated row by row:
   // row tm holds min(q (tm + 1), tiles_n) tiles with q = 128 / BN_.
   constexpr int Q = BM / BN_;
@@ -171,7 +170,6 @@ __global__ void __launch_bounds__(gemm_threads(BN_), BN_ == 64 ? 2 : 1) dgemm_nt
       const int blk = (g.col_base + n0) / g.map.nb;
       if (blk % g.map.ranks != g.rank) continue;
     }
-    const bool same = (BN_ == BM) && LOWER && (tm == tn) && (g.A == g.B) && (g.lda == g.ldb);  // diagonal syrk tile
     __syncthreads();  // the previous tile's shared-memory stages are free
 
     double acc[4][4][2];
@@ -184,12 +182,12 @@ __global__ void __launch_bounds__(gemm_threads(BN_), BN_ == 64 ? 2 : 1) dgemm_nt
     TileLoader<BK, BM, THREADS> la;
     TileLoader<BK, BN_, THREADS> lb;
     la.init(g.A, g.lda, g.M, m0, g.a_aligned);
-    if (!same) lb.init(g.B, g.ldb, g.N, n0, g.b_aligned);
+    lb.init(g.B, g.ldb, g.N, n0, g.b_aligned);
 #pragma unroll
     for (int s = 0; s < STAGES - 1; ++s) {
       if (s < nk) {
         la.issue(As + s * BK * LDT, s * BK, g.K, g.A, g.lda);
-        if (!same) lb.issue(Bs + s * BK * LDB, s * BK, g.K, g.B, g.ldb);
+        lb.issue(Bs + s * BK * LDB, s * BK, g.K, g.B, g.ldb);
       }
       cp_async_commit();
     }
@@ -202,20 +200,19 @@ __global__ void __launch_bounds__(gemm_threads(BN_), BN_ == 64 ? 2 : 1) dgemm_nt
         if (nt < nk) {
           const int s = nt % STAGES;
           la.issue(As + s * BK * LDT, nt * BK, g.K, g.A, g.lda);
-          if (!same) lb.issue(Bs + s * BK * LDB, nt * BK, g.K, g.B, g.ldb);
+          lb.issue(Bs + s * BK * LDB, nt * BK, g.K, g.B, g.ldb);
         }
         cp_async_commit();
       }
       const double* a_s = As + (kt % STAGES) * BK * LDT;
-      const double* b_s = same ? a_s : (Bs + (kt % STAGES) * BK * LDB);
-      const int ldb_s = same ? LDT : LDB;
+      const double* b_s = Bs + (kt % STAGES) * BK * LDB;
 #pragma unroll
       for (int ks = 0; ks < BK / 4; ++ks) {
         // af[i] = A(row wm + 8 i + lr, k = 4 ks + lc), bf = B(column wn + 8 j + lr, same k). Rows 16 b .. 16 b + 15
         // of the warp tile are accumulator rows 2 b (m = lr) and 2 b + 1 (m = lr + 8): one m16n8k4 per (b, j).
         double af[4];
         const double* ap = a_s + (ks * 4 + lc) * LDT + wm + lr;
-        const double* bp = b_s + (ks * 4 + lc) * ldb_s + wn + lr;
+        const double* bp = b_s + (ks * 4 + lc) * LDB + wn + lr;
 #pragma unroll
         for (int i = 0; i < 4; ++i) af[i] = ap[8 * i];
 #pragma unroll
@@ -265,61 +262,28 @@ __global__ void __launch_bounds__(gemm_threads(BN_), BN_ == 64 ? 2 : 1) dgemm_nt
   }  // tile loop
 }
 
-static int g_gemm_reserve_sms = 0;
-void set_gemm_sm_reserve(int n) { g_gemm_reserve_sms = n < 0 ? 0 : n; }
-
-namespace {
-template <int BN_, int BK, int STAGES>
-void configure_gemm_variant() {
-  const int smem = static_cast<int>(gemm_smem(BN_, BK, STAGES));
-  cudaFuncSetAttribute(dgemm_nt_kernel<true, 0, BN_, BK, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-  cudaFuncSetAttribute(dgemm_nt_kernel<false, 0, BN_, BK, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-  cudaFuncSetAttribute(dgemm_nt_kernel<true, 1, BN_, BK, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-  cudaFuncSetAttribute(dgemm_nt_kernel<true, 2, BN_, BK, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-}
-template <int BN_, int BK, int STAGES>
-void launch_gemm_variant(const GemmArgs& g, bool lower, bool scatter, unsigned grid, cudaStream_t s) {
-  const size_t smem = gemm_smem(BN_, BK, STAGES);
-  constexpr int T = gemm_threads(BN_);
-  if (g.owned_only)
-    dgemm_nt_kernel<true, 2, BN_, BK, STAGES><<<grid, T, smem, s>>>(g);
-  else if (scatter)
-    dgemm_nt_kernel<true, 1, BN_, BK, STAGES><<<grid, T, smem, s>>>(g);
-  else if (lower)
-    dgemm_nt_kernel<true, 0, BN_, BK, STAGES><<<grid, T, smem, s>>>(g);
-  else
-    dgemm_nt_kernel<false, 0, BN_, BK, STAGES><<<grid, T, smem, s>>>(g);
-}
-// B200BA_GEMM=64 (default: 128 x 64 tiles, BK 16 x 4 stages, 2 CTAs / SM) | 128 (128 x 128 tiles, BK 32 x 3
-// stages, 1 CTA / SM) | 12816 (128 x 128, BK 16 x 4 stages). Read once per process.
-int gemm_variant() {
-  static int variant = -1;
-  if (variant < 0) variant = getenv("B200BA_GEMM") ? atoi(getenv("B200BA_GEMM")) : 64;
-  return variant;
-}
-}  // namespace
-
-int launch_dgemm_nt(const GemmArgs& g_in, bool lower, bool scatter, cudaStream_t s, bool leave_sms, bool one_tile_per_cta) {
+int launch_dgemm_nt(const GemmArgs& g_in, bool lower, bool scatter, cudaStream_t s, bool one_tile_per_cta) {
   if (g_in.M <= 0 || g_in.N <= 0) return 0;
+  // 128 x 64 tiles, BK 16 x 4 stages, 2 CTAs / SM
+  constexpr int BN = 64, BK = 16, STAGES = 4;
+  constexpr int T = gemm_threads(BN);
+  constexpr int smem = static_cast<int>(gemm_smem(BN, BK, STAGES));
   static bool configured_dev[64] = {};
   static int sm_count[64] = {};
   int dev = 0;
   cudaGetDevice(&dev);
   bool& configured = configured_dev[dev & 63];  // function attributes are per device
-  const int variant = gemm_variant();
   if (!configured) {
-    configure_gemm_variant<64, 16, 4>();
-    configure_gemm_variant<128, 32, 3>();
-    configure_gemm_variant<128, 16, 4>();
+    cudaFuncSetAttribute(dgemm_nt_kernel<true, 0, BN, BK, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaFuncSetAttribute(dgemm_nt_kernel<false, 0, BN, BK, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaFuncSetAttribute(dgemm_nt_kernel<true, 1, BN, BK, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaFuncSetAttribute(dgemm_nt_kernel<true, 2, BN, BK, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     cudaDeviceGetAttribute(&sm_count[dev & 63], cudaDevAttrMultiProcessorCount, dev);
     configured = true;
   }
   GemmArgs g = g_in;
-  // an in-place product (C aliases A: the panel solve X <- X Linv^T, N = K = 128) must see ONE tile per row block:
-  // with 64-wide tiles the CTA of columns 0..63 would overwrite operand columns the CTA of columns 64..127 still reads
-  const int bn = (variant == 64 && !g.in_place) ? 64 : 128;
-  const int q = BM / bn;
-  const int64_t tm = (g.M + BM - 1) / BM, tn = (g.N + bn - 1) / bn;
+  constexpr int q = BM / BN;
+  const int64_t tm = (g.M + BM - 1) / BM, tn = (g.N + BN - 1) / BN;
   const bool tri_enum = lower || scatter || g.owned_only;
   int64_t n_tiles;
   if (tri_enum) {
@@ -329,157 +293,22 @@ int launch_dgemm_nt(const GemmArgs& g_in, bool lower, bool scatter, cudaStream_t
   } else {
     n_tiles = tm * tn;
   }
-  const int per_sm = (bn == 64) ? 2 : 1;
-  const int cap = std::max(1, (sm_count[dev & 63] - (leave_sms ? g_gemm_reserve_sms : 0)) * per_sm);
+  const int cap = std::max(1, sm_count[dev & 63] * 2);
   // one_tile_per_cta: an ordinary grid (the hardware scheduler can then hand SMs to a higher-priority stream
   // between tiles) instead of persistent CTAs
   const unsigned grid = static_cast<unsigned>(one_tile_per_cta ? n_tiles : std::min<int64_t>(n_tiles, cap));
-  if (variant == 64 && !g.in_place)
-    launch_gemm_variant<64, 16, 4>(g, tri_enum, scatter, grid, s);
-  else if (variant == 12816)
-    launch_gemm_variant<128, 16, 4>(g, tri_enum, scatter, grid, s);
+  if (g.owned_only)
+    dgemm_nt_kernel<true, 2, BN, BK, STAGES><<<grid, T, smem, s>>>(g);
+  else if (scatter)
+    dgemm_nt_kernel<true, 1, BN, BK, STAGES><<<grid, T, smem, s>>>(g);
+  else if (tri_enum)
+    dgemm_nt_kernel<true, 0, BN, BK, STAGES><<<grid, T, smem, s>>>(g);
   else
-    launch_gemm_variant<128, 32, 3>(g, tri_enum, scatter, grid, s);
+    dgemm_nt_kernel<false, 0, BN, BK, STAGES><<<grid, T, smem, s>>>(g);
   return cudaGetLastError() == cudaSuccess ? 0 : 1;
 }
 
-// ------------------------------------------------------------------------------------------
-// 128 x 128 diagonal tile: Cholesky in shared memory, then the explicit inverse of the factor
-// ------------------------------------------------------------------------------------------
-// potrf_tile_kernel (1 CTA)   A: column-major tile (leading dimension lda), lower triangle read; on exit
-//                             its lower triangle holds L. n <= 128 is the live size (last tile of the
-//                             matrix); the rest is treated as identity. info[0] is raised when a pivot is
-//                             not positive (the LM loop then rejects the attempt).
-// trinv_tile_kernel (8 CTAs)  Linv: 128 x 128 column-major (leading dimension 128), lower triangle = L^-1,
-//                             strict upper = 0. The columns of the inverse are independent: each warp
-//                             solves L x = e_c for one column by forward substitution with x spread over
-//                             the lanes' registers (a 128-step dependency chain of 4 FMAs + one warp
-//                             reduction), 16 columns per CTA.
-constexpr int PT = 128;        // tile size
-constexpr int PLD = PT + 1;    // odd pitch: column walks and row walks are both conflict-free
-constexpr int POTRF_THREADS = 512;
-constexpr size_t kTileSmem = static_cast<size_t>(PT) * PLD * sizeof(double);
-
-__device__ __forceinline__ void load_lower_tile(double* L, const double* __restrict__ A, int64_t lda, int n) {
-  for (int e = threadIdx.x; e < PT * PT; e += POTRF_THREADS) {
-    const int j = e >> 7, i = e & 127;
-    double v = (i == j) ? 1.0 : 0.0;
-    if (i < n && j < n && i >= j) v = A[static_cast<int64_t>(j) * lda + i];
-    L[j * PLD + i] = (i >= j) ? v : 0.0;
-  }
-}
-
-// Register-resident right-looking Cholesky: thread t owns row r = t & 127 and the columns c = (t >> 7) + 4 m of
-// the tile in registers, as a window that slides with the factorisation: a[i] is column grp + 4 (jo + i) while
-// the outer iteration jo handles the four columns 4 jo .. 4 jo + 3 (one per thread group), after which the
-// window shifts by one register. All register indices are compile-time constants with a loop body of a few
-// hundred instructions (a fully unrolled 128-step version is 180 KB of code and streams through the
-// instruction cache on every launch). Step j: the owners of column j publish it un-scaled through a
-// double-buffered shared-memory column, the owner of the diagonal adds 1 / sqrt(a_jj) (the only
-// transcendental on the critical path); after ONE barrier everybody updates its own columns c > j with
-// a(r, c) -= a(r, j) a(c, j) / a_jj, and the owners store L(r, j) = a(r, j) / sqrt(a_jj) straight to memory.
-// The window length W shrinks in four segments (32, 24, 16, 8 live columns).
-template <int W>
-__device__ __forceinline__ void potrf_segment(double (&a)[32], double (*colbuf)[2 * PT + 1], int jo_begin, int jo_end, int r,
-                                              int grp, double* __restrict__ A, int64_t lda, int n, bool& bad) {
-#pragma unroll 1
-  for (int jo = jo_begin; jo < jo_end; ++jo) {
-#pragma unroll
-    for (int g4 = 0; g4 < 4; ++g4) {
-      const int j = 4 * jo + g4;
-      double* cb = colbuf[g4 & 1];
-      if (grp == g4) {
-        cb[r] = (r >= j) ? a[0] : 0.0;
-        if (r == j) cb[2 * PT] = rsqrt(a[0]);
-      }
-      __syncthreads();
-      const double d = cb[j], rs = cb[2 * PT];
-      bad |= !(d > 0.0);
-      const double lrj = cb[r] * (rs * rs);
-      const double* cc = cb + grp + 4 * jo;  // cc[4 i] = a(c_i, j) for this thread's window columns
-#pragma unroll
-      for (int i = 0; i < W; ++i)
-        if (i > 0 || grp > g4) a[i] = fma(-lrj, cc[4 * i], a[i]);
-      if (grp == g4 && r >= j && r < n && j < n) A[static_cast<int64_t>(j) * lda + r] = cb[r] * rs;  // L(r, j)
-    }
-#pragma unroll
-    for (int i = 0; i + 1 < W; ++i) a[i] = a[i + 1];
-    a[W - 1] = 0.0;
-  }
-}
-
-__global__ void __launch_bounds__(POTRF_THREADS, 1)
-    potrf_tile_kernel(double* __restrict__ A, int64_t lda, int n, int* __restrict__ info) {
-  // column j un-scaled in [0, 128); zeros in [128, 256) (window columns beyond the tile); 1 / sqrt(a_jj) last
-  __shared__ double colbuf[2][2 * PT + 1];
-  const int tid = threadIdx.x;
-  const int r = tid & 127, grp = tid >> 7;
-  for (int e = tid; e < 2 * (2 * PT + 1); e += POTRF_THREADS) (&colbuf[0][0])[e] = 0.0;
-  double a[32];
-#pragma unroll
-  for (int m = 0; m < 32; ++m) {
-    const int c = grp + 4 * m;
-    double v = (r == c) ? 1.0 : 0.0;
-    if (r < n && c < n && r >= c) v = A[static_cast<int64_t>(c) * lda + r];
-    a[m] = v;
-  }
-  __syncthreads();
-  bool bad = false;
-  potrf_segment<32>(a, colbuf, 0, 8, r, grp, A, lda, n, bad);
-  potrf_segment<24>(a, colbuf, 8, 16, r, grp, A, lda, n, bad);
-  potrf_segment<16>(a, colbuf, 16, 24, r, grp, A, lda, n, bad);
-  potrf_segment<8>(a, colbuf, 24, 32, r, grp, A, lda, n, bad);
-  if (tid == 0 && bad) info[0] = 1;
-}
-
-// Inverse of the lower-triangular tile: one warp per column c solves L x = e_c by column-oriented forward
-// substitution with the residual spread over the lanes' registers (lane l: rows l, l + 32, l + 64, l + 96).
-// Per row only a multiply, one shuffle broadcast and the FMAs of the residual update are on the dependency
-// chain (the L entries are loaded ahead, the reciprocal diagonal is precomputed).
-constexpr int TRINV_CTAS = 8;
-__global__ void __launch_bounds__(POTRF_THREADS, 1)
-    trinv_tile_kernel(const double* __restrict__ A, int64_t lda, int n, double* __restrict__ Linv) {
-  extern __shared__ __align__(16) double sm[];
-  double* L = sm;  // [PT][PLD] column-major: L(i, j) at L[j * PLD + i]
-  __shared__ double invd[PT];
-  load_lower_tile(L, A, lda, n);
-  __syncthreads();
-  if (threadIdx.x < PT) invd[threadIdx.x] = 1.0 / L[threadIdx.x * PLD + threadIdx.x];
-  __syncthreads();
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int c = blockIdx.x * (POTRF_THREADS / 32) + warp;  // 16 warps x 8 CTAs = 128 columns
-  double res[4], x[4];
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    res[q] = (lane + 32 * q == c) ? 1.0 : 0.0;
-    x[q] = 0.0;
-  }
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    for (int ii = 0; ii < 32; ++ii) {
-      const int i = 32 * q + ii;
-      if (i < c) continue;  // warp-uniform
-      const double* col = L + i * PLD;
-      // entries of column i below the diagonal (independent of x_i: loaded before the broadcast completes)
-      double l0 = 0, l1 = 0, l2 = 0, l3 = 0;
-      if (q <= 0) l0 = col[lane];
-      if (q <= 1) l1 = col[lane + 32];
-      if (q <= 2) l2 = col[lane + 64];
-      l3 = col[lane + 96];
-      const double mine = res[q] * invd[i];
-      const double xi = __shfl_sync(0xffffffffu, mine, ii);
-      if (lane == ii) x[q] = xi;
-      // rows k > i (entries with k <= i of column i are zero or the diagonal: masked)
-      if (q <= 0) res[0] = (lane > i) ? fma(-l0, xi, res[0]) : res[0];
-      if (q <= 1) res[1] = (lane + 32 > i) ? fma(-l1, xi, res[1]) : res[1];
-      if (q <= 2) res[2] = (lane + 64 > i) ? fma(-l2, xi, res[2]) : res[2];
-      res[3] = (lane + 96 > i) ? fma(-l3, xi, res[3]) : res[3];
-    }
-  }
-  double* out = Linv + c * PT;
-#pragma unroll
-  for (int q = 0; q < 4; ++q) out[lane + 32 * q] = x[q];
-}
+constexpr int PT = 128;  // diagonal tile size
 
 // The blocked tile step (ba_tile.cuh): factor + inverse in one launch of 8 CTAs.
 struct TileDeviceExec {
@@ -516,21 +345,6 @@ int launch_potrf_trinv_tile(const double* Ain, int64_t lda_in, int n, double* Lo
   return cudaGetLastError() == cudaSuccess ? 0 : 1;
 }
 
-int launch_potrf_tile(double* A, int64_t lda, int n, double* Linv, int* info, cudaStream_t s) {
-  static bool configured_dev[64] = {};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  bool& configured = configured_dev[dev & 63];
-  if (!configured) {
-    cudaFuncSetAttribute(potrf_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kTileSmem));
-    cudaFuncSetAttribute(trinv_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kTileSmem));
-    configured = true;
-  }
-  potrf_tile_kernel<<<1, POTRF_THREADS, 0, s>>>(A, lda, n, info);
-  trinv_tile_kernel<<<TRINV_CTAS, POTRF_THREADS, kTileSmem, s>>>(A, lda, n, Linv);
-  return cudaGetLastError() == cudaSuccess ? 0 : 1;
-}
-
 // ------------------------------------------------------------------------------------------
 // small helpers
 // ------------------------------------------------------------------------------------------
@@ -548,98 +362,9 @@ void launch_add_diagonal_map(int n, double* S, const DenseMap& map, double lambd
 // ------------------------------------------------------------------------------------------
 // The factor lives in packed block-column panels: panel k holds rows k0 .. n of the columns k0 .. k0 + NB
 // (k0 = k * NB) column-major with leading dimension hk = even(n - k0); element L(i, c) = P_k[(c - k0) * hk +
-// (i - k0)]. Every 128 x 128 diagonal tile also has its explicit inverse (Linv tiles, from potrf_tile).
+// (i - k0)]. Every 128 x 128 diagonal tile also has its explicit inverse (Linv tiles, from potrf_trinv_tile).
 //
-// forward step, tile t (columns c0 .. c0 + 128): y_t = Linv_t b_t ; b_i -= sum_c L(i, c) y_c for i below.
-// One launch per tile. Every CTA recomputes y_t (a 128 x 128 product out of L2) and owns 64 rows below,
-// each row's 128-term dot product split over 4 threads (32 independent loads in flight per thread
-// group instead of a 128-deep chain). CTA 0 also publishes y_t (into `yout`, a separate vector: the
-// other CTAs are still reading b_t).
-// y_i = sum_{c = c_lo, c_lo + 2, ... <= c_hi} M[c * PT + i] * v[c] for this thread's (row i, parity) with the loads of
-// eight terms issued together (a plain loop left them in a load -> FMA chain: one L2 round trip per term).
-__device__ __forceinline__ double tile_dot_strided(const double* __restrict__ M, const double* v, int i, int c_lo, int c_hi) {
-  double acc0 = 0.0, acc1 = 0.0;
-  int c = c_lo;
-  for (; c + 14 <= c_hi; c += 16) {
-    double l[8];
-#pragma unroll
-    for (int q = 0; q < 8; ++q) l[q] = __ldg(M + (c + 2 * q) * PT + i);
-#pragma unroll
-    for (int q = 0; q < 8; q += 2) {
-      acc0 = fma(l[q], v[c + 2 * q], acc0);
-      acc1 = fma(l[q + 1], v[c + 2 * q + 2], acc1);
-    }
-  }
-  for (; c <= c_hi; c += 2) acc0 = fma(__ldg(M + c * PT + i), v[c], acc0);
-  return acc0 + acc1;
-}
-// same for the transposed product: x_j = sum_{i = i_lo, i_lo + 2, ... <= i_hi} M[j * PT + i] * v[i]
-__device__ __forceinline__ double tile_dot_contig(const double* __restrict__ M, const double* v, int j, int i_lo, int i_hi) {
-  double acc0 = 0.0, acc1 = 0.0;
-  int i = i_lo;
-  const double* col = M + j * PT;
-  for (; i + 14 <= i_hi; i += 16) {
-    double l[8];
-#pragma unroll
-    for (int q = 0; q < 8; ++q) l[q] = __ldg(col + i + 2 * q);
-#pragma unroll
-    for (int q = 0; q < 8; q += 2) {
-      acc0 = fma(l[q], v[i + 2 * q], acc0);
-      acc1 = fma(l[q + 1], v[i + 2 * q + 2], acc1);
-    }
-  }
-  for (; i <= i_hi; i += 2) acc0 = fma(__ldg(col + i), v[i], acc0);
-  return acc0 + acc1;
-}
-
-constexpr int TS_THREADS = 256;
-constexpr int TS_ROWS = 64;
-__global__ void __launch_bounds__(TS_THREADS)
-    trsv_forward_step_kernel(const double* __restrict__ P, int64_t hk, int off_in_panel, int live, int rows_below,
-                             const double* __restrict__ Linv, double* __restrict__ b /* at row c0 */,
-                             double* __restrict__ yout /* at row c0 */) {
-  __shared__ double y[PT];
-  __shared__ double bs[PT];
-  __shared__ double part[4][TS_ROWS];
-  const int tid = threadIdx.x;
-  if (tid < PT) bs[tid] = (tid < live) ? b[tid] : 0.0;
-  __syncthreads();
-  {
-    // y_i = sum_{c <= i} Linv(i, c) b_c : 2 threads per row (even / odd c), combined through shared memory
-    const int i = tid & 127, half = tid >> 7;
-    const double acc = (i < live) ? tile_dot_strided(Linv, bs, i, half, i) : 0.0;
-    if (half == 1) y[i] = acc;
-    __syncthreads();
-    if (half == 0) y[i] += acc;
-    __syncthreads();
-  }
-  if (blockIdx.x == 0 && tid < live) yout[tid] = y[tid];
-  const int r = blockIdx.x * TS_ROWS + (tid & 63);  // row below the tile
-  const int cg = tid >> 6;                          // column group: columns cg * 32 .. cg * 32 + 31
-  double acc = 0.0;
-  if (r < rows_below) {
-    const double* Lp = P + static_cast<int64_t>(off_in_panel + cg * 32) * hk + off_in_panel + PT + r;
-    const double* yc = y + cg * 32;
-    const int cmax = min(32, live - cg * 32);
-    double acc1 = 0.0;
-    int c = 0;
-    for (; c + 8 <= cmax; c += 8) {
-      double l[8];
-#pragma unroll
-      for (int q = 0; q < 8; ++q) l[q] = Lp[static_cast<int64_t>(c + q) * hk];
-#pragma unroll
-      for (int q = 0; q < 8; q += 2) {
-        acc = fma(l[q], yc[c + q], acc);
-        acc1 = fma(l[q + 1], yc[c + q + 1], acc1);
-      }
-    }
-    for (; c < cmax; ++c) acc = fma(Lp[static_cast<int64_t>(c) * hk], yc[c], acc);
-    acc += acc1;
-  }
-  part[cg][tid & 63] = acc;
-  __syncthreads();
-  if (cg == 0 && r < rows_below) b[PT + r] -= (part[0][tid] + part[1][tid]) + (part[2][tid] + part[3][tid]);
-}
+// y_0 = Linv_0 b_0 (forward) or x_{T-1} = Linv_{T-1}^T y_{T-1} (backward, transpose): the first tile of each sweep
 __global__ void trsv_store_tile_kernel(const double* __restrict__ Linv, const double* __restrict__ b, int live,
                                        double* __restrict__ out, bool transpose) {
   const int tid = threadIdx.x;
@@ -653,49 +378,11 @@ __global__ void trsv_store_tile_kernel(const double* __restrict__ Linv, const do
   out[tid] = acc;
 }
 
-// backward step, tile t (rows r0 .. r0 + live): x_t = Linv_t^T y_t ; y_c -= sum_{i in t} L(i, c) x_i for every
-// column c to the LEFT of the tile. One warp per column (the 128 rows of a column are contiguous).
-__global__ void __launch_bounds__(TS_THREADS)
-    trsv_backward_step_kernel(const double* __restrict__ Lpack, const int64_t* __restrict__ panel_off,
-                              const int* __restrict__ panel_h, int NB, int r0, int live, int n_cols_left,
-                              const double* __restrict__ Linv, const double* __restrict__ yt /* y at row r0 */,
-                              double* __restrict__ y /* full vector */, double* __restrict__ xout /* at row r0 */) {
-  __shared__ double x[PT];
-  __shared__ double ys[PT];
-  const int tid = threadIdx.x;
-  if (tid < PT) ys[tid] = (tid < live) ? yt[tid] : 0.0;
-  __syncthreads();
-  {
-    // x_j = sum_{i >= j} Linv(i, j) y_i : 2 threads per entry (even / odd i)
-    const int j = tid & 127, half = tid >> 7;
-    const double acc = (j < live) ? tile_dot_contig(Linv, ys, j, j + half, live - 1) : 0.0;
-    if (half == 1) x[j] = acc;
-    __syncthreads();
-    if (half == 0) x[j] += acc;
-    __syncthreads();
-  }
-  if (blockIdx.x == 0 && tid < live) xout[tid] = x[tid];
-  const int warp = tid >> 5, lane = tid & 31;
-  const int c = blockIdx.x * (TS_THREADS / 32) + warp;
-  if (c >= n_cols_left) return;
-  const int k = c / NB;
-  const double* col = Lpack + panel_off[k] + static_cast<int64_t>(c - k * NB) * panel_h[k] + (r0 - k * NB);
-  double acc = 0.0;
-  for (int i = lane; i < live; i += 32) acc = fma(col[i], x[i], acc);
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-  if (lane == 0) y[c] -= acc;
-}
-
-// ------------------------------------------------------------------------------------------
-// triangular solves, second version: the tile product leaves the critical path of the other CTAs
-// ------------------------------------------------------------------------------------------
-// In the step kernels above EVERY CTA first repeats the 128 x 128 product with the inverted diagonal tile (out of
-// L2: 100-200 CTAs x 64-128 KB per launch) before it touches its rows, and every thread keeps only 8 loads in
-// flight. Here the tile's solution arrives through global memory: step t applies y_t to all rows below in 128-row
-// CTAs (32 independent loads per thread and batch), and CTA 0 -- which owns exactly the rows of tile t + 1 --
-// goes on to y_{t+1} = Linv_{t+1} b_{t+1} with the inverse prefetched into shared memory by cp.async while the
-// row update runs. One wave of at most 102 CTAs; nothing is computed twice.
+// The steps: the tile's solution arrives through global memory, so no CTA repeats the 128 x 128 product with the
+// inverted diagonal tile before it touches its rows. Forward step t applies y_t to all rows below in 128-row CTAs
+// (32 independent loads per thread and batch), and CTA 0 -- which owns exactly the rows of tile t + 1 -- goes on
+// to y_{t+1} = Linv_{t+1} b_{t+1} with the inverse prefetched into shared memory by cp.async while the row update
+// runs. One wave of at most 102 CTAs; nothing is computed twice.
 constexpr int TS2_THREADS = 256;
 constexpr int TS2_LD = PT + 2;  // pitch of the staged inverse (16-byte aligned columns)
 constexpr size_t kTs2Smem = static_cast<size_t>(PT) * TS2_LD * sizeof(double);
@@ -825,32 +512,6 @@ __global__ void __launch_bounds__(TS2_THREADS, 1)
 // ------------------------------------------------------------------------------------------
 // host side: blocked right-looking Cholesky with look-ahead, block-cyclic over the ranks
 // ------------------------------------------------------------------------------------------
-// B200BA_PANEL=2 (default): blocked tile kernel + out-of-place panel solves straight out of S; =1: the first
-// version (pack, register-window tile Cholesky, separate inverse launch, in-place solves)
-static int panel_version() {
-  static int v = -1;
-  if (v < 0) v = getenv("B200BA_PANEL") ? atoi(getenv("B200BA_PANEL")) : 2;
-  return v;
-}
-// B200BA_AUX=0 keeps the second look-ahead update of the single-GPU factorisation on the panel stream
-static bool aux_enabled() {
-  static const bool v = !(getenv("B200BA_AUX") && atoi(getenv("B200BA_AUX")) == 0);
-  return v;
-}
-// B200BA_TRSV=1: the first version of the triangular solves (one launch per tile, every CTA repeats the tile product)
-static int trsv_version() {
-  static int v = -1;
-  if (v < 0) v = getenv("B200BA_TRSV") ? atoi(getenv("B200BA_TRSV")) : 2;
-  return v;
-}
-
-void dense_variants(int* gemm, int* panel, int* trsv, int* aux) {
-  *gemm = gemm_variant();
-  *panel = panel_version();
-  *trsv = trsv_version();
-  *aux = aux_enabled() ? 1 : 0;
-}
-
 int dense_plan(DenseCtx* d, int n, int nb, int rank, int ranks) {
   d->n = n;
   d->rank = rank;
@@ -893,7 +554,7 @@ int dense_factor(DenseCtx* d) {
   const int sub_n = NB / PT;
   cudaStream_t sm = d->s_main, sp = d->s_panel;
   auto owner = [&](int k) { return k % R; };
-  const bool use_aux = aux_enabled() && R == 1 && d->s_aux != nullptr;
+  const bool use_aux = R == 1 && d->s_aux != nullptr;
   // S is ready when everything queued on s_main so far has run
   cudaEventRecord(d->ev_misc, sm);
   cudaStreamWaitEvent(sp, d->ev_misc, 0);
@@ -926,17 +587,17 @@ int dense_factor(DenseCtx* d) {
       g.C = d->S + d->map.col_offset(j0) + j0;
       g.ldc = d->map.ld;
     }
-    return launch_dgemm_nt(g, /*lower=*/true, /*scatter=*/false, st, /*leave_sms=*/false, /*one_tile_per_cta=*/true);
+    return launch_dgemm_nt(g, /*lower=*/true, /*scatter=*/false, st, /*one_tile_per_cta=*/true);
   };
 
   for (int k = 0; k < d->nblk; ++k) {
     const int k0 = k * NB, kw = std::min(NB, n - k0), hk = d->panel_h[k], hlive = n - k0;
     double* P = d->Lpack + d->panel_off[k];
-    if (owner(k) == me && panel_version() == 2) {
+    if (owner(k) == me) {
       // Panel factorisation straight out of S: every diagonal tile goes through the blocked factor + inverse launch
-      // (S -> P), the rows below it are solved OUT of place (S -> P, so the product may use the 128 x 64 tiles: a
-      // panel has fewer row blocks than the GPU has SMs and whole 128 x 128 x 128 tiles per SM made this step throughput-bound
-      // on a third of the machine), and the panel-internal update is applied to the remaining columns in S.
+      // (S -> P), the rows below it are solved OUT of place (S -> P: in place, the CTA of columns 0..63 of a row
+      // block would overwrite operand columns the CTA of columns 64..127 still reads), and the panel-internal
+      // update is applied to the remaining columns in S.
       const double* Sk = d->S + d->map.col_offset(k0) + k0;  // (i, c) of the block column at Sk[c * ld + i]
       double* Sk_w = d->S + d->map.col_offset(k0) + k0;
       const int64_t ld = d->map.ld;
@@ -963,7 +624,7 @@ int dense_factor(DenseCtx* d) {
           g.beta = 0.0;
           g.a_aligned = gemm_operand_aligned(g.A, g.lda);
           g.b_aligned = gemm_operand_aligned(g.B, g.ldb);
-          if (launch_dgemm_nt(g, false, false, sp, false, true)) return 1;
+          if (launch_dgemm_nt(g, false, false, sp, true)) return 1;
           const int rest = kw - c0 - PT;  // remaining columns of this panel
           if (rest > 0) {
             GemmArgs u{};
@@ -979,56 +640,7 @@ int dense_factor(DenseCtx* d) {
             u.alpha = -1.0;
             u.beta = 1.0;
             u.a_aligned = u.b_aligned = gemm_operand_aligned(u.A, u.lda);
-            if (launch_dgemm_nt(u, true, false, sp, false, true)) return 1;
-          }
-        }
-      }
-    } else if (owner(k) == me) {
-      // first version: pack the (fully updated) block column into its panel, then factor it in place
-      cudaMemcpy2DAsync(P, static_cast<size_t>(hk) * sizeof(double), d->S + d->map.col_offset(k0) + k0,
-                        static_cast<size_t>(d->map.ld) * sizeof(double), static_cast<size_t>(hlive) * sizeof(double), kw,
-                        cudaMemcpyDeviceToDevice, sp);
-      for (int sub = 0; sub < sub_n; ++sub) {
-        const int c0 = sub * PT;
-        if (c0 >= kw) break;
-        const int live = std::min(PT, kw - c0);
-        double* tile = P + static_cast<int64_t>(c0) * hk + c0;
-        double* Li = P + static_cast<int64_t>(hk) * NB + static_cast<int64_t>(sub) * PT * PT;
-        if (launch_potrf_tile(tile, hk, live, Li, d->info, sp)) return 1;
-        const int below = hlive - c0 - PT;
-        if (below > 0) {
-          GemmArgs g{};  // rows below: X <- X Linv^T
-          g.M = below;
-          g.N = PT;
-          g.K = PT;
-          g.A = tile + PT;
-          g.lda = hk;
-          g.B = Li;
-          g.ldb = PT;
-          g.C = tile + PT;
-          g.ldc = hk;
-          g.alpha = 1.0;
-          g.beta = 0.0;
-          g.in_place = true;
-          g.a_aligned = gemm_operand_aligned(g.A, g.lda);
-          g.b_aligned = gemm_operand_aligned(g.B, g.ldb);
-          if (launch_dgemm_nt(g, false, false, sp)) return 1;
-          const int rest = kw - c0 - PT;  // remaining columns of this panel
-          if (rest > 0) {
-            GemmArgs u{};
-            u.M = below;
-            u.N = rest;
-            u.K = PT;
-            u.A = tile + PT;
-            u.lda = hk;
-            u.B = u.A;
-            u.ldb = hk;
-            u.C = P + static_cast<int64_t>(c0 + PT) * hk + (c0 + PT);
-            u.ldc = hk;
-            u.alpha = -1.0;
-            u.beta = 1.0;
-            u.a_aligned = u.b_aligned = gemm_operand_aligned(u.A, u.lda);
-            if (launch_dgemm_nt(u, true, false, sp)) return 1;
+            if (launch_dgemm_nt(u, true, false, sp, true)) return 1;
           }
         }
       }
@@ -1075,66 +687,37 @@ int dense_solve(DenseCtx* d, double* b) {
   const int n = d->n, NB = d->NB;
   if (n == 0) return 0;
   cudaStream_t sm = d->s_main;
-  const int sub_n = NB / PT;
   auto linv_of = [&](int t) {
     const int k = (t * PT) / NB, sub = (t * PT - k * NB) / PT;
     return d->Lpack + d->panel_off[k] + static_cast<int64_t>(d->panel_h[k]) * NB + static_cast<int64_t>(sub) * PT * PT;
   };
-  if (trsv_version() == 2) {
-    static bool configured_dev[64] = {};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (!configured_dev[dev & 63]) {
-      cudaFuncSetAttribute(trsv_forward2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kTs2Smem));
-      cudaFuncSetAttribute(trsv_backward2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kTs2Smem));
-      configured_dev[dev & 63] = true;
-    }
-    const int T = d->ntiles;
-    // forward: y_0 = Linv_0 b_0, then one launch per tile that has rows below it
-    trsv_store_tile_kernel<<<1, PT, 0, sm>>>(linv_of(0), b, std::min(PT, n), d->tmp, false);
-    for (int t = 0; t + 1 < T; ++t) {
-      const int c0 = t * PT, k = c0 / NB, off = c0 - k * NB;
-      const int rows_below = n - c0 - PT;
-      const double* Lp = d->Lpack + d->panel_off[k] + static_cast<int64_t>(off) * d->panel_h[k] + off + PT;
-      trsv_forward2_kernel<<<(rows_below + PT - 1) / PT, TS2_THREADS, kTs2Smem, sm>>>(Lp, d->panel_h[k], rows_below, d->tmp + c0,
-                                                                                      b + c0 + PT, linv_of(t + 1), d->tmp + c0 + PT);
-    }
-    // backward: x_{T-1} = Linv^T y_{T-1}, then one launch per tile that has columns to its left
-    {
-      const int r0 = (T - 1) * PT;
-      trsv_store_tile_kernel<<<1, PT, 0, sm>>>(linv_of(T - 1), d->tmp + r0, std::min(PT, n - r0), b + r0, true);
-    }
-    for (int t = T - 1; t >= 1; --t) {
-      const int r0 = t * PT, live = std::min(PT, n - r0);
-      trsv_backward2_kernel<<<r0 / PT, TS2_THREADS, kTs2Smem, sm>>>(d->Lpack, d->d_panel_off, d->d_panel_h, NB, r0, live, b + r0,
-                                                                    d->tmp, linv_of(t - 1), b + r0 - PT);
-    }
-    return cudaGetLastError() == cudaSuccess ? 0 : 1;
+  static bool configured_dev[64] = {};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (!configured_dev[dev & 63]) {
+    cudaFuncSetAttribute(trsv_forward2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kTs2Smem));
+    cudaFuncSetAttribute(trsv_backward2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kTs2Smem));
+    configured_dev[dev & 63] = true;
   }
-  // forward: L y = b  (y is collected in d->tmp)
-  for (int t = 0; t < d->ntiles; ++t) {
-    const int c0 = t * PT, live = std::min(PT, n - c0), k = c0 / NB;
+  const int T = d->ntiles;
+  // forward: y_0 = Linv_0 b_0, then one launch per tile that has rows below it
+  trsv_store_tile_kernel<<<1, PT, 0, sm>>>(linv_of(0), b, std::min(PT, n), d->tmp, false);
+  for (int t = 0; t + 1 < T; ++t) {
+    const int c0 = t * PT, k = c0 / NB, off = c0 - k * NB;
     const int rows_below = n - c0 - PT;
-    const double* Li = linv_of(t);
-    if (rows_below > 0) {
-      const int grid = (rows_below + TS_ROWS - 1) / TS_ROWS;
-      trsv_forward_step_kernel<<<grid, TS_THREADS, 0, sm>>>(d->Lpack + d->panel_off[k], d->panel_h[k], c0 - k * NB, live,
-                                                              rows_below, Li, b + c0, d->tmp + c0);
-    } else {
-      trsv_store_tile_kernel<<<1, PT, 0, sm>>>(Li, b + c0, live, d->tmp + c0, false);
-    }
+    const double* Lp = d->Lpack + d->panel_off[k] + static_cast<int64_t>(off) * d->panel_h[k] + off + PT;
+    trsv_forward2_kernel<<<(rows_below + PT - 1) / PT, TS2_THREADS, kTs2Smem, sm>>>(Lp, d->panel_h[k], rows_below, d->tmp + c0,
+                                                                                    b + c0 + PT, linv_of(t + 1), d->tmp + c0 + PT);
   }
-  // backward: L^T x = y  (x lands in b)
-  for (int t = d->ntiles - 1; t >= 0; --t) {
+  // backward: x_{T-1} = Linv^T y_{T-1}, then one launch per tile that has columns to its left
+  {
+    const int r0 = (T - 1) * PT;
+    trsv_store_tile_kernel<<<1, PT, 0, sm>>>(linv_of(T - 1), d->tmp + r0, std::min(PT, n - r0), b + r0, true);
+  }
+  for (int t = T - 1; t >= 1; --t) {
     const int r0 = t * PT, live = std::min(PT, n - r0);
-    const double* Li = linv_of(t);
-    if (r0 > 0) {
-      const int grid = (r0 + TS_THREADS / 32 - 1) / (TS_THREADS / 32);
-      trsv_backward_step_kernel<<<grid, TS_THREADS, 0, sm>>>(d->Lpack, d->d_panel_off, d->d_panel_h, NB, r0, live, r0, Li,
-                                                               d->tmp + r0, d->tmp, b + r0);
-    } else {
-      trsv_store_tile_kernel<<<1, PT, 0, sm>>>(Li, d->tmp + r0, live, b + r0, true);
-    }
+    trsv_backward2_kernel<<<r0 / PT, TS2_THREADS, kTs2Smem, sm>>>(d->Lpack, d->d_panel_off, d->d_panel_h, NB, r0, live, b + r0,
+                                                                  d->tmp, linv_of(t - 1), b + r0 - PT);
   }
   return cudaGetLastError() == cudaSuccess ? 0 : 1;
 }

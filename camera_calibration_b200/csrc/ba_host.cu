@@ -82,8 +82,6 @@ bool load_nccl(std::string* err) {
   return true;
 }
 
-constexpr int kMaxCholPanels = 1024;
-
 enum Phase { PH_JAC = 0, PH_ACC, PH_SCHUR, PH_FACTOR, PH_TRIAL, PH_UPDATE, PH_ALLREDUCE, PH_STRAGGLER, PH_SOLVE, PH_COUNT };
 
 }  // namespace
@@ -128,8 +126,6 @@ struct b200ba_handle {
   int64_t reduce_count = 0;  // doubles of sys.base covered by the per-build all-reduce
   double* d_potrf_work = nullptr;
   int potrf_lwork = 0;
-  int chol_mode = -1;                     // B200BA_DIST_CHOL=0|1 overrides: 1 = column-block Cholesky (see factor_dense)
-  int chol_nb = 512;                      // its panel width (B200BA_CHOL_NB)
   int *d_info = nullptr, *d_fail = nullptr;
   // Static cell-major processing order: device position -> index in the caller's (reference)
   // observation order. Computed once at create time from the cell of the measured pixel.
@@ -170,7 +166,6 @@ struct b200ba_handle {
   std::vector<int32_t> lm_events;         // B200BA_LM_* per LM attempt of the last b200ba_optimize
   std::vector<double> grp_sums;           // [sx | sy | count] per Schur block (see build_groups)
   int force_grouped = -1;                 // B200BA_GROUPED=0|1 overrides the cost model
-  bool compact_j = true;                  // B200BA_COMPACT_J=0: expanded Jacobian buffer also for central-generic cameras
 
   // calibration report: allocated by the first b200ba_calibration_report
   ReportDev rep{};
@@ -558,8 +553,8 @@ int make_layout(b200ba_handle* h, const b200ba_options* opt) {
   const int64_t n = h->n_obs;
   if (dev_alloc(h, &h->out.residual, 2 * n)) return 1;
   if (dev_alloc(h, &h->out.cost, n)) return 1;
-  // compact Jacobian records when every camera is central-generic (B200BA_COMPACT_J=0 keeps the expanded buffer)
-  h->out.compact = (h->uniform_model == B200BA_MODEL_CENTRAL_GENERIC && h->compact_j) ? 1 : 0;
+  // compact Jacobian records when every camera is central-generic
+  h->out.compact = (h->uniform_model == B200BA_MODEL_CENTRAL_GENERIC) ? 1 : 0;
   if (h->out.compact) {
     if (h->out.jac) cudaFree(h->out.jac);
     h->out.jac = nullptr;
@@ -611,12 +606,6 @@ int make_layout(b200ba_handle* h, const b200ba_options* opt) {
   if (dev_alloc(h, &h->d_x, L.dof)) return 1;
   int lwork = 0;
   CUSOLVER_TRY(h, cusolverDnDpotrf_bufferSize(h->cusolver, CUBLAS_FILL_MODE_LOWER, L.nd, h->d_S, std::max(1, L.nd), &lwork));
-  {
-    int lw2 = 0;
-    const int nbp = std::max(1, std::min(L.nd, h->chol_nb));
-    CUSOLVER_TRY(h, cusolverDnDpotrf_bufferSize(h->cusolver, CUBLAS_FILL_MODE_LOWER, nbp, h->d_S, std::max(1, L.nd), &lw2));
-    lwork = std::max(lwork, lw2);
-  }
   h->potrf_lwork = lwork;
   if (dev_alloc(h, &h->d_potrf_work, std::max(1, lwork))) return 1;
 
@@ -764,76 +753,12 @@ int build_system(b200ba_handle* h, double huber, double* cost, double* n_valid, 
   return 0;
 }
 
-__global__ void fold_panel_info_kernel(const int* __restrict__ panel_info, int n, int* __restrict__ info) {
-  int worst = 0;
-  for (int i = threadIdx.x; i < n; i += 32) worst = max(worst, panel_info[i] != 0 ? 1 : 0);
-  for (int o = 16; o > 0; o >>= 1) worst = max(worst, __shfl_xor_sync(0xffffffffu, worst, o));
-  if (threadIdx.x == 0) info[0] = worst;
-}
-
-// Cholesky factorisation of the reduced system S (column-major, lower) in place; info[0] != 0
-// when a pivot was not positive.
-//   default: cusolverDnDpotrf on the whole matrix (replicated on every rank).
-//   B200BA_DIST_CHOL=1: right-looking factorisation over column blocks of width nb, dealt round-robin
-//   to the ranks. The owner of block k factors its diagonal tile and solves the tile column below
-//   it, broadcasts the finished column block (whole columns: contiguous in the column-major S),
-//   then every rank applies the rank-nb update to the column blocks IT owns. Each rank thereby
-//   does 1/N of the n^3/3 update flops instead of all of them, and ends with the complete L (its
-//   own blocks computed, the others received), so the triangular solves stay local.
+// Cholesky factorisation of the reduced system S (column-major, lower) in place with cusolverDnDpotrf on the whole
+// matrix (replicated on every rank); info[0] != 0 when a pivot was not positive.
 int factor_dense(b200ba_handle* h) {
-  const Layout& L = h->L;
-  const int nd = L.nd;
-  const int nb = h->chol_nb;
-  const int nblk = (nd + nb - 1) / nb;
-  // Opt-in (B200BA_DIST_CHOL=1): the panel chain (potrf(nb) + trsm + broadcast per column block) is
-  // serial without look-ahead, so the replicated potrf stays the default.
-  bool blocked = (h->chol_mode == 1) && nd > nb;
-  if (nblk > kMaxCholPanels) blocked = false;
-  if (!blocked) {
-    CUSOLVER_TRY(h, cusolverDnDpotrf(h->cusolver, CUBLAS_FILL_MODE_LOWER, nd, h->d_S, nd, h->d_potrf_work, h->potrf_lwork,
-                                     h->d_info));
-    return 0;
-  }
-  const double one = 1.0, minus_one = -1.0;
-  int* panel_info = h->d_info + 2;
-  CUDA_TRY(h, cudaMemsetAsync(panel_info, 0, nblk * sizeof(int), h->stream));
-  for (int k = 0; k < nblk; ++k) {
-    const int owner = k % h->n_ranks;
-    const int j0 = k * nb, w = std::min(nb, nd - j0), below = nd - j0 - w;
-    double* Akk = h->d_S + static_cast<size_t>(j0) * nd + j0;
-    if (h->rank == owner) {
-      CUSOLVER_TRY(h, cusolverDnDpotrf(h->cusolver, CUBLAS_FILL_MODE_LOWER, w, Akk, nd, h->d_potrf_work, h->potrf_lwork,
-                                       panel_info + k));
-      if (below > 0)  // L_below = A_below L_kk^-T
-        CUBLAS_TRY(h, cublasDtrsm(h->cublas, CUBLAS_SIDE_RIGHT, CUBLAS_FILL_MODE_LOWER, CUBLAS_OP_T, CUBLAS_DIAG_NON_UNIT, below,
-                                  w, &one, Akk, nd, Akk + w, nd));
-    }
-    if (h->n_ranks > 1 && h->comm) {
-      double* col = h->d_S + static_cast<size_t>(j0) * nd;
-      const int rc = g_nccl.Broadcast(col, col, static_cast<size_t>(nd) * w, kNcclDouble, owner, h->comm, h->stream);
-      if (rc != 0) {
-        h->error = std::string("ncclBroadcast: ") + (g_nccl.GetErrorString ? g_nccl.GetErrorString(rc) : "error");
-        return 1;
-      }
-    }
-    // trailing update of the column blocks this rank owns
-    for (int j = k + 1; j < nblk; ++j) {
-      if (j % h->n_ranks != h->rank) continue;
-      const int c0 = j * nb, wj = std::min(nb, nd - c0);
-      const double* Lj = h->d_S + static_cast<size_t>(j0) * nd + c0;  // rows c0.. of column block k
-      CUBLAS_TRY(h, cublasDgemm(h->cublas, CUBLAS_OP_N, CUBLAS_OP_T, nd - c0, wj, w, &minus_one, Lj, nd, Lj, nd, &one,
-                                h->d_S + static_cast<size_t>(c0) * nd + c0, nd));
-    }
-  }
-  fold_panel_info_kernel<<<1, 32, 0, h->stream>>>(panel_info, nblk, h->d_info);
-  if (h->n_ranks > 1 && h->comm) {
-    // every rank must take the same branch of the LM loop
-    const int rc = g_nccl.AllReduce(h->d_info, h->d_info, 1, kNcclInt32, kNcclMax, h->comm, h->stream);
-    if (rc != 0) {
-      h->error = "ncclAllReduce (factorisation status) failed";
-      return 1;
-    }
-  }
+  const int nd = h->L.nd;
+  CUSOLVER_TRY(h, cusolverDnDpotrf(h->cusolver, CUBLAS_FILL_MODE_LOWER, nd, h->d_S, nd, h->d_potrf_work, h->potrf_lwork,
+                                   h->d_info));
   return 0;
 }
 
@@ -1673,7 +1598,6 @@ int b200ba_create(const b200ba_problem* p, int device, b200ba_handle** out) {
   }
   if (const char* e = getenv("B200BA_DENSE")) h->own_dense = !(strcmp(e, "lib") == 0 || strcmp(e, "0") == 0);
   if (const char* e = getenv("B200BA_DENSE_NB")) h->dense_nb = std::max(128, atoi(e) / 128 * 128);
-  set_gemm_sm_reserve(getenv("B200BA_PANEL_SMS") ? atoi(getenv("B200BA_PANEL_SMS")) : 8);
   {
     int lo = 0, hi = 0;
     cudaDeviceGetStreamPriorityRange(&lo, &hi);
@@ -1681,9 +1605,6 @@ int b200ba_create(const b200ba_problem* p, int device, b200ba_handle** out) {
     TRYC(cuda_ok(cudaStreamCreateWithPriority(&h->aux_stream, cudaStreamNonBlocking, hi), "cudaStreamCreate"));
   }
   if (const char* e = getenv("B200BA_GROUPED")) h->force_grouped = atoi(e);
-  if (const char* e = getenv("B200BA_COMPACT_J")) h->compact_j = atoi(e) != 0;
-  if (const char* e = getenv("B200BA_DIST_CHOL")) h->chol_mode = atoi(e);
-  if (const char* e = getenv("B200BA_CHOL_NB")) h->chol_nb = std::max(32, atoi(e));
   h->pb.n_obs = n;
   h->pb.obs_imageset = h->d_obs_imageset;
   h->pb.obs_camera = h->d_obs_camera;
@@ -1701,7 +1622,7 @@ int b200ba_create(const b200ba_problem* p, int device, b200ba_handle** out) {
   TRYC(cuda_ok(cudaMemset(h->d_last_projection, 0, std::max<int64_t>(1, n) * sizeof(double2)), "memset"));
   TRYC(dev_alloc(h, &h->d_straggler_list, n));
   TRYC(dev_alloc(h, &h->d_straggler_count, 1));
-  TRYC(dev_alloc(h, &h->d_info, 2 + kMaxCholPanels));
+  TRYC(dev_alloc(h, &h->d_info, 2));
   TRYC(dev_alloc(h, &h->d_fail, 1));
   TRYC(dev_alloc(h, &h->d_partial, cost_reduce_partial_size()));
   TRYC(dev_alloc(h, &h->d_scal, 16));
@@ -2401,7 +2322,7 @@ int b200ba_debug_solve_step(b200ba_handle* h, const b200ba_options* opt, double 
   info[0] = spd;
   info[1] = h->use_grouped ? 1 : 0;
   info[2] = h->n_groups;
-  dense_variants(&info[3], &info[4], &info[5], &info[6]);
+  info[3] = info[4] = info[5] = info[6] = 0;  // reserved
   info[7] = h->own_dense ? h->dn.NB : 0;
   return 0;
 }
@@ -2514,7 +2435,6 @@ int b200ba_dense_cholesky_solve(int device, int32_t n, int32_t nb, const double*
   }
   CallScope cs(&g_create_error);
   if (int rc = cs.use_device(device)) return rc;
-  set_gemm_sm_reserve(getenv("B200BA_PANEL_SMS") ? atoi(getenv("B200BA_PANEL_SMS")) : 8);
   DenseCtx d;
   dense_plan(&d, n, nb, 0, 1);
   double* dA = nullptr;

@@ -568,37 +568,9 @@ __global__ void __launch_bounds__(128, MINB)
   }
 }
 
-// Resident blocks per SM the kernel is compiled for (register budget 65536 / (128 * MINB)).
-// 4 (128 registers, 16 warps / SM) is the default; B200BA_JAC_MINB=2|3|4|5|6 overrides it for tuning runs.
-static int jac_minb() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("B200BA_JAC_MINB");
-    v = e ? atoi(e) : 4;
-    if (v < 2 || v > 6) v = 4;
-  }
-  return v;
-}
-
-// Threads per block of the main pass (tuning knob B200BA_JAC_THREADS=32|64|128; the kernel is
-// compiled for at most 128) and its evaluation budget (B200BA_EVAL_BUDGET, default 16).
-static int jac_threads() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("B200BA_JAC_THREADS");
-    v = e ? atoi(e) : 128;
-    if (v != 32 && v != 64 && v != 128) v = 128;
-  }
-  return v;
-}
-static int main_eval_budget() {
-  static bool read = false;
-  if (!read) {
-    read = true;
-    if (const char* e = getenv("B200BA_EVAL_BUDGET")) g_main_eval_budget = atoi(e) < 1 ? 1 : atoi(e);
-  }
-  return g_main_eval_budget;
-}
+// Main pass: 128 threads per block; MINB = resident blocks per SM the kernel is compiled for (register budget
+// 65536 / (128 * MINB)).
+constexpr int kMainThreads = 128;
 
 // Straggler pass geometry: a fixed grid that loops over the device-side list (its length is not
 // known on the host without a sync); 2 lanes per listed observation.
@@ -609,14 +581,10 @@ template <int MODEL, bool JAC, int MINB>
 static void launch_rj_model(const ProblemDev& pb, const Layout& L, const StateDev& st, double2* lp,
                             const ObsOut& out, double huber, uint32_t* list, int* count, cudaStream_t s,
                             cudaEvent_t main_done) {
-  const int threads = jac_threads();
-  const unsigned blocks = static_cast<unsigned>((pb.n_obs + threads - 1) / threads);
-  if (MODEL == B200BA_MODEL_CENTRAL_GENERIC && JAC && out.compact)
-    residual_jacobian_kernel<MODEL, JAC, MINB, false, (MODEL == B200BA_MODEL_CENTRAL_GENERIC && JAC)>
-        <<<blocks, threads, 0, s>>>(pb, L, st, lp, out, huber, list, count, main_eval_budget());
-  else
-    residual_jacobian_kernel<MODEL, JAC, MINB, false, false><<<blocks, threads, 0, s>>>(pb, L, st, lp, out, huber, list, count,
-                                                                                        main_eval_budget());
+  const unsigned blocks = static_cast<unsigned>((pb.n_obs + kMainThreads - 1) / kMainThreads);
+  // central-generic Jacobians go to the compact records (out.compact is set for exactly these rigs)
+  residual_jacobian_kernel<MODEL, JAC, MINB, false, (MODEL == B200BA_MODEL_CENTRAL_GENERIC && JAC)>
+      <<<blocks, kMainThreads, 0, s>>>(pb, L, st, lp, out, huber, list, count, g_main_eval_budget);
   if (main_done) cudaEventRecord(main_done, s);  // between the main and the straggler pass
 }
 
@@ -628,13 +596,7 @@ static void launch_rj(int model, const ProblemDev& pb, const Layout& L, const St
   cudaMemsetAsync(count, 0, sizeof(int), s);
   switch (model) {
     case B200BA_MODEL_CENTRAL_GENERIC:
-      switch (jac_minb()) {
-        case 2: launch_rj_model<B200BA_MODEL_CENTRAL_GENERIC, JAC, 2>(pb, L, st, lp, out, huber, list, count, s, main_done); break;
-        case 3: launch_rj_model<B200BA_MODEL_CENTRAL_GENERIC, JAC, 3>(pb, L, st, lp, out, huber, list, count, s, main_done); break;
-        case 5: launch_rj_model<B200BA_MODEL_CENTRAL_GENERIC, JAC, 5>(pb, L, st, lp, out, huber, list, count, s, main_done); break;
-        case 6: launch_rj_model<B200BA_MODEL_CENTRAL_GENERIC, JAC, 6>(pb, L, st, lp, out, huber, list, count, s, main_done); break;
-        default: launch_rj_model<B200BA_MODEL_CENTRAL_GENERIC, JAC, 4>(pb, L, st, lp, out, huber, list, count, s, main_done);
-      }
+      launch_rj_model<B200BA_MODEL_CENTRAL_GENERIC, JAC, 4>(pb, L, st, lp, out, huber, list, count, s, main_done);
       break;
     case B200BA_MODEL_NONCENTRAL_GENERIC:
       launch_rj_model<B200BA_MODEL_NONCENTRAL_GENERIC, JAC, 3>(pb, L, st, lp, out, huber, list, count, s, main_done);
@@ -653,12 +615,8 @@ static void launch_stragglers(int model, const ProblemDev& pb, const Layout& L, 
   if (pb.n_obs == 0) return;
   switch (model) {
     case B200BA_MODEL_CENTRAL_GENERIC:
-      if (JAC && out.compact)
-        residual_jacobian_kernel<B200BA_MODEL_CENTRAL_GENERIC, JAC, 2, true, JAC>
-            <<<kStragglerBlocks, kStragglerThreads, 0, s>>>(pb, L, st, lp, out, huber, list, count, 0);
-      else
-        residual_jacobian_kernel<B200BA_MODEL_CENTRAL_GENERIC, JAC, 2, true, false>
-            <<<kStragglerBlocks, kStragglerThreads, 0, s>>>(pb, L, st, lp, out, huber, list, count, 0);
+      residual_jacobian_kernel<B200BA_MODEL_CENTRAL_GENERIC, JAC, 2, true, JAC>
+          <<<kStragglerBlocks, kStragglerThreads, 0, s>>>(pb, L, st, lp, out, huber, list, count, 0);
       break;
     case B200BA_MODEL_NONCENTRAL_GENERIC:
       residual_jacobian_kernel<B200BA_MODEL_NONCENTRAL_GENERIC, JAC, 2, true, false>

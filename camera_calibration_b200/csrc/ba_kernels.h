@@ -200,19 +200,13 @@ struct GemmArgs {
   // global column col_base + n (rows likewise); tiles of column blocks owned by other ranks are skipped
   bool owned_only;
   int rank, col_base;
-  bool in_place;  // C aliases A (N = K <= 128): forces one 128-wide tile per row block
 };
 inline bool gemm_operand_aligned(const double* p, int64_t ld) {
   return (reinterpret_cast<uintptr_t>(p) % 16 == 0) && (ld % 2 == 0);
 }
 // lower: only tiles / entries with i >= j (M == N); scatter: the scatter-subtract epilogue (implies lower).
-// leave_sms: cap the persistent grid at (SM count - reserve) so that concurrently running panel kernels find
-// a free SM at once (set_gemm_sm_reserve; used for the trailing updates of the factorisation).
-int launch_dgemm_nt(const GemmArgs& g, bool lower, bool scatter, cudaStream_t s, bool leave_sms = false,
-                    bool one_tile_per_cta = false);
-void set_gemm_sm_reserve(int n);
-// Cholesky of a 128 x 128 (live size n) column-major diagonal tile in place + Linv [128 x 128, ld 128].
-int launch_potrf_tile(double* A, int64_t lda, int n, double* Linv, int* info, cudaStream_t s);
+// one_tile_per_cta: an ordinary grid instead of persistent CTAs (the factorisation's updates).
+int launch_dgemm_nt(const GemmArgs& g, bool lower, bool scatter, cudaStream_t s, bool one_tile_per_cta = false);
 
 // y += alpha B^T u (two stages, fixed order; partial: gemv_t_partial_size doubles) and t = B x for row-major B
 int gemv_t_partial_size(int rows, int cols);
@@ -245,7 +239,5 @@ struct DenseCtx {
 int dense_plan(DenseCtx* d, int n, int nb, int rank, int ranks);
 int dense_factor(DenseCtx* d);
 int dense_solve(DenseCtx* d, double* b);
-// the process-wide variants of the dense phase in effect (B200BA_GEMM, B200BA_PANEL, B200BA_TRSV, B200BA_AUX)
-void dense_variants(int* gemm, int* panel, int* trsv, int* aux);
 
 }  // namespace b200ba

@@ -923,9 +923,8 @@ B200BA_API int b200ba_debug_eval_counts(b200ba_handle* h, uint16_t* counts);
  *   rhs [n_d]        the reduced right-hand side b_d - B^T (D + lambda I)^-1 b_p
  *   x [n]            the update, in b200ba_build_system's variable order
  *   lambda_used      nullable
- *   info [8]         positive definite (1 / 0), grouped contraction used, number of groups, and the
- *                    dense-phase variants in effect: GEMM tile (64 | 128 | 12816), panel version,
- *                    triangular-solve version, aux stream (1 / 0), block width (0 on the library path)
+ *   info [8]         positive definite (1 / 0), grouped contraction used, number of groups, info[3..6]
+ *                    reserved (written as 0), block width of the dense phase (0 on the library path)
  * n_d = n minus the unknowns of the eliminated blocks (points, or poses without eliminate_points).
  * Returns 2 for a handle joined to a communicator. */
 B200BA_API int b200ba_debug_solve_step(b200ba_handle* h, const b200ba_options* opt, double lambda, int32_t n,

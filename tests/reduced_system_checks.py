@@ -193,7 +193,7 @@ def solve_step(adj, opt, lam=-1.0):
     return out
 
 
-# ---- cases shared by tests/test_reduced_system.py and tests/dense_variant_check.py -------------------------
+# ---- cases of tests/test_reduced_system.py ----------------------------------------------------------------
 def small_problem(cfg):
     """The small problems of the parity tests (n_d from about 70 to about 1 700)."""
     from camera_calibration_b200 import synthetic

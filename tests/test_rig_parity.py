@@ -335,32 +335,6 @@ def test_debug_switches_match_oracle(oracle_lib, fix):
 
 
 @pytest.mark.gpu
-def test_expanded_jacobian_records_equal_compact(monkeypatch):
-    """B200BA_COMPACT_J=0 (read when the handle is created) keeps the expanded per-observation Jacobian
-    records for central-generic cameras: same H, b and LM trajectory as the compact default."""
-    sp = _fx("central_uneven")
-    out = []
-    for compact in (None, "0"):
-        if compact is None:
-            monkeypatch.delenv("B200BA_COMPACT_J", raising=False)
-        else:
-            monkeypatch.setenv("B200BA_COMPACT_J", compact)
-        with api.BundleAdjuster(sp.problem) as adj:
-            adj.set_state(sp.init_state)
-            H, b, c = adj.build_system(cabi.default_options())
-            st = sp.init_state.copy()
-            rep = adj.optimize_host(st, cabi.default_options(max_iteration_count=5))
-        out.append((H, b, c, rep, st))
-    (H0, b0, c0, r0, s0), (H1, b1, c1, r1, s1) = out
-    assert np.abs(H1 - H0).max() <= 1e-12 * np.abs(H0).max()
-    assert np.abs(b1 - b0).max() <= 1e-12 * np.abs(b0).max()
-    assert abs(c1 - c0) <= 1e-12 * c0
-    assert r0.trace()[2] == r1.trace()[2] and np.allclose(r0.trace()[0], r1.trace()[0], rtol=1e-10)
-    assert np.abs(s0.points - s1.points).max() < 1e-9
-    assert max(np.abs(x - y).max() for x, y in zip(s0.intrinsics, s1.intrinsics)) < 1e-9
-
-
-@pytest.mark.gpu
 def test_structured_contraction_equals_dense(oracle_lib, monkeypatch):
     """The grouped Schur contraction (B200BA_GROUPED=1, several uneven groups) gives the LM loop of the
     dense one (=0) and of the oracle on the mixed rig."""

@@ -153,7 +153,9 @@ struct b200ba_handle {
   int* d_cols = nullptr;
   int* d_count = nullptr;
   int* h_count = nullptr;                 // pinned
-  double* d_Wc = nullptr;                 // 2 panels (double-buffered)
+  double* d_Wc = nullptr;                 // in-tree dense path: every group's panel; library path: 2 (double-buffered)
+  ContractGroup* h_contract = nullptr;    // pinned: the grouped contraction's table of one attempt
+  ContractGroup* d_contract = nullptr;
   double* d_P = nullptr;                  // 2 result buffers (double-buffered)
   size_t wc_stride = 0, p_stride = 0;
   cudaEvent_t ev_syrk[2] = {nullptr, nullptr}, ev_scatter[2] = {nullptr, nullptr}, ev_s_ready = nullptr;
@@ -403,7 +405,12 @@ int build_groups(b200ba_handle* h, bool allocate) {
     CUDA_TRY(h, cudaMallocHost(reinterpret_cast<void**>(&h->h_count), std::max(1, h->n_groups) * sizeof(int)));
     h->wc_stride = static_cast<size_t>(gb) * L.bs * (std::max(1, L.nd) + 1);
     h->p_stride = static_cast<size_t>(std::max(1, L.nd)) * std::max(1, L.nd);
-    if (dev_alloc(h, &h->d_Wc, 2 * h->wc_stride)) return 1;
+    // in-tree dense path: all groups' panels at once (sum_g k_g = nbd rows of at most nd + 1 columns)
+    const size_t wc_n = h->own_dense ? static_cast<size_t>(std::max(1, L.nbd)) * (std::max(1, L.nd) + 1) : 2 * h->wc_stride;
+    if (dev_alloc(h, &h->d_Wc, wc_n)) return 1;
+    if (dev_alloc(h, &h->d_contract, std::max(1, h->n_groups))) return 1;
+    if (h->h_contract) cudaFreeHost(h->h_contract);
+    CUDA_TRY(h, cudaMallocHost(reinterpret_cast<void**>(&h->h_contract), std::max(1, h->n_groups) * sizeof(ContractGroup)));
     if (!h->own_dense && dev_alloc(h, &h->d_P, 2 * h->p_stride)) return 1;
     for (int i = 0; i < 2; ++i) {
       if (!h->ev_syrk[i]) CUDA_TRY(h, cudaEventCreateWithFlags(&h->ev_syrk[i], cudaEventDisableTiming));
@@ -971,36 +978,51 @@ int solve_system_own(b200ba_handle* h, double lambda, int* spd) {
       joined = true;
     };
     if (h->use_grouped) {
-      // structured contraction: per group gather -> DMMA rank-k update with the scatter epilogue
-      int it = 0;
+      // structured contraction: every group's compact panel W_g is gathered, then ONE DMMA launch runs the rank-k
+      // updates of all groups with the scatter epilogue (one persistent grid: no tail and no gather between groups)
+      int n_tab = 0;
+      int64_t w_off = 0, tiles = 0;
       for (int g = h->rank; g < h->n_groups; g += R) {
         const int nblk = h->group_start[g + 1] - h->group_start[g];
         const int kg = nblk * L.bs, mg = h->group_count[g];
         if (mg == 0 || kg == 0) continue;
         const int ldw = (mg + 1) / 2 * 2;
-        double* Wc = h->d_Wc + (it & 1) * h->wc_stride;
-        const int* cols = h->d_cols + static_cast<size_t>(g) * nd;
-        launch_gather_scale(L.bs, nblk, nd, mg, ldw, h->sys.B, h->d_Linv, h->d_group_blocks + h->group_start[g], cols, Wc,
-                            h->stream);
+        ContractGroup& cg = h->h_contract[n_tab++];
+        cg.w_off = w_off;
+        cg.cols_off = static_cast<int64_t>(g) * nd;
+        cg.tile0 = tiles;
+        cg.m = mg;
+        cg.k = kg;
+        cg.ld = ldw;
+        cg.aligned = gemm_operand_aligned(h->d_Wc + w_off, ldw);
+        launch_gather_scale(L.bs, nblk, nd, mg, ldw, h->sys.B, h->d_Linv, h->d_group_blocks + h->group_start[g],
+                            h->d_cols + cg.cols_off, h->d_Wc + w_off, h->stream);
+        w_off += static_cast<int64_t>(kg) * ldw;
+        tiles += dgemm_lower_tiles(mg, mg);
+        h->timings.contraction_flops += static_cast<double>(mg) * mg * kg;
+        h->timings.kernel_launches += 1;
+      }
+      if (n_tab > 0) {
+        // the pinned table is rewritten only by the next attempt, after this one has synchronised
+        CUDA_TRY(h, cudaMemcpyAsync(h->d_contract, h->h_contract, n_tab * sizeof(ContractGroup), cudaMemcpyHostToDevice,
+                                    h->stream));
         join_copy();
         GemmArgs ga{};
-        ga.M = ga.N = mg;
-        ga.K = kg;
-        ga.A = ga.B = Wc;
-        ga.lda = ga.ldb = ldw;
+        ga.A = h->d_Wc;
         ga.C = h->d_S;
         ga.alpha = -1.0;
         ga.beta = 1.0;
-        ga.a_aligned = ga.b_aligned = gemm_operand_aligned(Wc, ldw);
-        ga.cols = cols;
+        ga.cols = h->d_cols;
         ga.map = d.map;
+        ga.groups = h->d_contract;
+        ga.n_groups = n_tab;
+        ga.n_tiles_lower = tiles;
+        ga.M = ga.N = ga.K = 1;  // unused in the grouped mode (the launcher skips empty products)
         if (launch_dgemm_nt(ga, true, true, h->stream)) {
           h->error = "dgemm_nt (contraction) launch failed";
           return 1;
         }
-        h->timings.contraction_flops += static_cast<double>(mg) * mg * kg;
-        h->timings.kernel_launches += 2;
-        ++it;
+        h->timings.kernel_launches += 1;
       }
     } else if (L.nbd > 0 && nd > 0) {
       // dense contraction over this rank's slice of the Schur blocks: S_r -= W_r^T W_r
@@ -1123,8 +1145,11 @@ void free_handle_buffers(b200ba_handle* h) {
   F(h->sys.base); F(h->d_W); F(h->d_S); F(h->d_Linv); F(h->d_v); F(h->d_y); F(h->d_x); F(h->d_potrf_work);
   F(h->d_info); F(h->d_fail); F(h->d_straggler_list); F(h->d_straggler_count); F(h->d_perm); F(h->d_lp_stage);
   F(h->d_group_of_block); F(h->d_group_blocks); F(h->d_flags); F(h->d_cols); F(h->d_count); F(h->d_Wc); F(h->d_P); F(h->d_u);
+  F(h->d_contract);
   if (h->h_count) cudaFreeHost(h->h_count);
   h->h_count = nullptr;
+  if (h->h_contract) cudaFreeHost(h->h_contract);
+  h->h_contract = nullptr;
   F(h->d_partial); F(h->d_scal); F(h->d_rot);
   F(h->rep.err); F(h->rep.mag); F(h->rep.cam_off); F(h->rep.cell_off); F(h->rep.cell_order); F(h->rep.Q);
   F(h->rep.partial); F(h->rep.select_hist); F(h->rep.hist); F(h->rep.kl); F(h->rep.cams); F(h->d_rep_stage);

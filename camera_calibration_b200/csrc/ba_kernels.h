@@ -181,6 +181,14 @@ struct DenseMap {
   }
 };
 
+// One group of the grouped contraction (GemmArgs::groups): its compact panel W_g (k x m, row-major, leading
+// dimension ld) at A + w_off, its column list at cols + cols_off, and the index of its first tile in the launch.
+struct ContractGroup {
+  int64_t w_off, cols_off, tile0;
+  int m, k, ld;
+  bool aligned;  // W_g is 16-byte aligned (even w_off and ld)
+};
+
 // C (+)= alpha * A B^T; A(i, k) at A[k * lda + i], B(j, k) at B[k * ldb + j], C(i, j) at C[j * ldc + i].
 struct GemmArgs {
   int M, N, K;
@@ -200,6 +208,11 @@ struct GemmArgs {
   // global column col_base + n (rows likewise); tiles of column blocks owned by other ranks are skipped
   bool owned_only;
   int rank, col_base;
+  // grouped contraction: C += alpha * W_g^T W_g (lower, scatter through each group's columns) for n_groups groups
+  // in one launch; A = base of the panels, cols = base of the column lists, n_tiles_lower = total tile count.
+  // Groups share entries of S, so the epilogue adds with FP64 reductions; beta, B, M, N, K are not used.
+  const ContractGroup* groups;
+  int n_groups;
 };
 inline bool gemm_operand_aligned(const double* p, int64_t ld) {
   return (reinterpret_cast<uintptr_t>(p) % 16 == 0) && (ld % 2 == 0);
@@ -207,6 +220,8 @@ inline bool gemm_operand_aligned(const double* p, int64_t ld) {
 // lower: only tiles / entries with i >= j (M == N); scatter: the scatter-subtract epilogue (implies lower).
 // one_tile_per_cta: an ordinary grid instead of persistent CTAs (the factorisation's updates).
 int launch_dgemm_nt(const GemmArgs& g, bool lower, bool scatter, cudaStream_t s, bool one_tile_per_cta = false);
+// tiles of the LOWER enumeration of an M x N product (ContractGroup::tile0)
+int64_t dgemm_lower_tiles(int M, int N);
 
 // y += alpha B^T u (two stages, fixed order; partial: gemv_t_partial_size doubles) and t = B x for row-major B
 int gemv_t_partial_size(int rows, int cols);

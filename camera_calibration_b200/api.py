@@ -494,6 +494,15 @@ def debug_cost_compare(trial, base=None, residual=None, device: int = -1) -> np.
     return out
 
 
+def debug_live_allocations() -> Tuple[int, int, int]:
+    """(count, device bytes, pinned host bytes) of the allocations the library holds right now
+    (``b200ba_debug_live_allocations``)."""
+    lib = cabi.load_library()
+    dev, pinned = C.c_int64(0), C.c_int64(0)
+    n = lib.b200ba_debug_live_allocations(C.byref(dev), C.byref(pinned))
+    return int(n), dev.value, pinned.value
+
+
 def schur_solve(block_size: int, D, B, Cm, b1, b2, device: int = -1) -> np.ndarray:
     """SolveWithSchurComplementDenseOffDiag (libvis lm_optimizer.h:1246-1369) on the device."""
     lib = cabi.load_library()

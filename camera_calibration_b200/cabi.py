@@ -554,6 +554,7 @@ SYMBOLS = {
     "b200ba_debug_cost_compare": (C.c_int, [C.c_int, C.c_int64, _D, _D, _D, _D]),
     "b200ba_debug_nice_orientation": (C.c_int, [C.c_void_p, _D]),
     "b200ba_debug_lm_events": (C.c_int32, [C.c_void_p, _I32, C.c_int32]),
+    "b200ba_debug_live_allocations": (C.c_int64, [C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
 }
 
 # b200ba_debug_lm_events codes (the oracle reports a NaN update as LM_REFUSED_PIVOT)

@@ -16,6 +16,7 @@
 #include <dlfcn.h>
 
 #include <algorithm>
+#include <atomic>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -84,6 +85,44 @@ bool load_nccl(std::string* err) {
 
 enum Phase { PH_JAC = 0, PH_ACC, PH_SCHUR, PH_FACTOR, PH_TRIAL, PH_UPDATE, PH_ALLREDUCE, PH_STRAGGLER, PH_SOLVE, PH_COUNT };
 
+// Number and bytes ([0] device, [1] pinned host) of the allocations all owners hold (b200ba_debug_live_allocations).
+std::atomic<int64_t> g_live_count{0}, g_live_bytes[2] = {};
+
+// Device and pinned host allocations that share one lifetime: release() or the destructor frees them all.
+struct Allocations {
+  struct Block {
+    void* p;
+    size_t bytes;
+    bool pinned;
+  };
+  std::vector<Block> blocks;
+
+  Allocations() = default;
+  Allocations(const Allocations&) = delete;
+  Allocations& operator=(const Allocations&) = delete;
+  ~Allocations() { release(); }
+  template <class T>
+  cudaError_t alloc(T** p, size_t count, bool pinned = false) {
+    const size_t bytes = count * sizeof(T);
+    void** q = reinterpret_cast<void**>(p);
+    const cudaError_t e = pinned ? cudaMallocHost(q, bytes) : cudaMalloc(q, bytes);
+    if (e == cudaSuccess && *p) {
+      blocks.push_back({*p, bytes, pinned});
+      g_live_count += 1;
+      g_live_bytes[pinned] += static_cast<int64_t>(bytes);
+    }
+    return e;
+  }
+  void release() {
+    for (const Block& b : blocks) {
+      b.pinned ? cudaFreeHost(b.p) : cudaFree(b.p);
+      g_live_count -= 1;
+      g_live_bytes[b.pinned] -= static_cast<int64_t>(b.bytes);
+    }
+    blocks.clear();
+  }
+};
+
 }  // namespace
 
 struct b200ba_handle {
@@ -94,6 +133,11 @@ struct b200ba_handle {
   cublasHandle_t cublas = nullptr;
   cusolverDnHandle_t cusolver = nullptr;
   std::string error;
+  // The owners of every buffer below: problem_mem until destroy (b200ba_create, and the snapshot, rotations, report
+  // and report images on first use), layout_mem until the layout changes (make_layout), dense_mem until the layout or
+  // the rank count changes (plan_dense). The destructor releases everything the handle holds.
+  Allocations problem_mem, layout_mem, dense_mem;
+  ~b200ba_handle();
 
   // problem
   std::vector<b200ba_camera> cams_host;
@@ -233,13 +277,8 @@ namespace {
   } while (0)
 
 template <class T>
-int dev_alloc(b200ba_handle* h, T** p, size_t count) {
-  if (*p) {
-    cudaFree(*p);
-    *p = nullptr;
-  }
-  if (count == 0) count = 1;
-  CUDA_TRY(h, cudaMalloc(reinterpret_cast<void**>(p), count * sizeof(T)));
+int dev_alloc(b200ba_handle* h, Allocations& owner, T** p, size_t count) {
+  CUDA_TRY(h, owner.alloc(p, std::max<size_t>(1, count)));
   return 0;
 }
 
@@ -343,25 +382,23 @@ void resolve_timings(b200ba_handle* h) {
 int reduce_group_sums(b200ba_handle* h) {
   if (h->n_ranks <= 1 || !h->comm || h->grp_sums.empty()) return 0;
   const size_t n = h->grp_sums.size();
+  Allocations scratch;
   double* d = nullptr;
-  CUDA_TRY(h, cudaMalloc(reinterpret_cast<void**>(&d), n * sizeof(double)));
-  cudaMemcpy(d, h->grp_sums.data(), n * sizeof(double), cudaMemcpyHostToDevice);
-  const int rc = g_nccl.AllReduce(d, d, n, kNcclDouble, kNcclSum, h->comm, h->stream);
-  const cudaError_t ce = cudaStreamSynchronize(h->stream);
-  if (rc == 0 && ce == cudaSuccess) cudaMemcpy(h->grp_sums.data(), d, n * sizeof(double), cudaMemcpyDeviceToHost);
-  cudaFree(d);
-  if (rc != 0 || ce != cudaSuccess) {
+  CUDA_TRY(h, scratch.alloc(&d, n));
+  CUDA_TRY(h, cudaMemcpy(d, h->grp_sums.data(), n * sizeof(double), cudaMemcpyHostToDevice));
+  if (g_nccl.AllReduce(d, d, n, kNcclDouble, kNcclSum, h->comm, h->stream) != 0) {
     h->error = "all-reduce of the group centroids failed";
     return 1;
   }
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  CUDA_TRY(h, cudaMemcpy(h->grp_sums.data(), d, n * sizeof(double), cudaMemcpyDeviceToHost));
   return 0;
 }
 
 // Groups of Schur blocks for the structured contraction, from the centroid sums in h->grp_sums
 // ([sx | sy | count] per block). Must produce the same grouping on every rank: the ranks split
 // the GROUPS among themselves (solve_system), so a rank-dependent order would drop / repeat blocks.
-int build_groups(b200ba_handle* h, bool allocate) {
-  const Layout& L = h->L;
+int build_groups(b200ba_handle* h, const Layout& L, bool allocate) {
   const int nb = L.nblocks;
   int gb = (L.bs == 3) ? 96 : 48;  // ~288 rows per group
   if (const char* e = getenv("B200BA_GROUP_BLOCKS")) gb = std::max(1, atoi(e));
@@ -396,28 +433,24 @@ int build_groups(b200ba_handle* h, bool allocate) {
   h->group_start[h->n_groups] = nb;
   h->group_count.assign(std::max(1, h->n_groups), 0);
   if (allocate) {
-    if (dev_alloc(h, &h->d_group_of_block, std::max(1, nb))) return 1;
-    if (dev_alloc(h, &h->d_group_blocks, std::max(1, nb))) return 1;
-    if (dev_alloc(h, &h->d_flags, static_cast<size_t>(std::max(1, h->n_groups)) * std::max(1, L.nd))) return 1;
-    if (dev_alloc(h, &h->d_cols, static_cast<size_t>(std::max(1, h->n_groups)) * std::max(1, L.nd))) return 1;
-    if (dev_alloc(h, &h->d_count, std::max(1, h->n_groups))) return 1;
-    if (h->h_count) cudaFreeHost(h->h_count);
-    CUDA_TRY(h, cudaMallocHost(reinterpret_cast<void**>(&h->h_count), std::max(1, h->n_groups) * sizeof(int)));
+    Allocations& m = h->layout_mem;
+    if (dev_alloc(h, m, &h->d_group_of_block, std::max(1, nb))) return 1;
+    if (dev_alloc(h, m, &h->d_group_blocks, std::max(1, nb))) return 1;
+    if (dev_alloc(h, m, &h->d_flags, static_cast<size_t>(std::max(1, h->n_groups)) * std::max(1, L.nd))) return 1;
+    if (dev_alloc(h, m, &h->d_cols, static_cast<size_t>(std::max(1, h->n_groups)) * std::max(1, L.nd))) return 1;
+    if (dev_alloc(h, m, &h->d_count, std::max(1, h->n_groups))) return 1;
+    CUDA_TRY(h, m.alloc(&h->h_count, std::max(1, h->n_groups), /*pinned=*/true));
     h->wc_stride = static_cast<size_t>(gb) * L.bs * (std::max(1, L.nd) + 1);
     h->p_stride = static_cast<size_t>(std::max(1, L.nd)) * std::max(1, L.nd);
     // in-tree dense path: all groups' panels at once (sum_g k_g = nbd rows of at most nd + 1 columns)
     const size_t wc_n = h->own_dense ? static_cast<size_t>(std::max(1, L.nbd)) * (std::max(1, L.nd) + 1) : 2 * h->wc_stride;
-    if (dev_alloc(h, &h->d_Wc, wc_n)) return 1;
-    if (dev_alloc(h, &h->d_contract, std::max(1, h->n_groups))) return 1;
-    if (h->h_contract) cudaFreeHost(h->h_contract);
-    CUDA_TRY(h, cudaMallocHost(reinterpret_cast<void**>(&h->h_contract), std::max(1, h->n_groups) * sizeof(ContractGroup)));
-    if (!h->own_dense && dev_alloc(h, &h->d_P, 2 * h->p_stride)) return 1;
-    for (int i = 0; i < 2; ++i) {
-      if (!h->ev_syrk[i]) CUDA_TRY(h, cudaEventCreateWithFlags(&h->ev_syrk[i], cudaEventDisableTiming));
-      if (!h->ev_scatter[i]) CUDA_TRY(h, cudaEventCreateWithFlags(&h->ev_scatter[i], cudaEventDisableTiming));
-    }
-    if (!h->ev_s_ready) CUDA_TRY(h, cudaEventCreateWithFlags(&h->ev_s_ready, cudaEventDisableTiming));
-    if (dev_alloc(h, &h->d_u, std::max(1, L.nbd))) return 1;
+    if (dev_alloc(h, m, &h->d_Wc, wc_n)) return 1;
+    if (dev_alloc(h, m, &h->d_contract, std::max(1, h->n_groups))) return 1;
+    CUDA_TRY(h, m.alloc(&h->h_contract, std::max(1, h->n_groups), /*pinned=*/true));
+    if (!h->own_dense && dev_alloc(h, m, &h->d_P, 2 * h->p_stride)) return 1;
+    for (cudaEvent_t* e : {&h->ev_syrk[0], &h->ev_syrk[1], &h->ev_scatter[0], &h->ev_scatter[1], &h->ev_s_ready})
+      if (!*e) CUDA_TRY(h, cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+    if (dev_alloc(h, m, &h->d_u, std::max(1, L.nbd))) return 1;
   }
   CUDA_TRY(h, cudaMemcpy(h->d_group_of_block, gob.data(), std::max(1, nb) * sizeof(int), cudaMemcpyHostToDevice));
   if (nb > 0) CUDA_TRY(h, cudaMemcpy(h->d_group_blocks, order.data(), nb * sizeof(int), cudaMemcpyHostToDevice));
@@ -460,30 +493,32 @@ void dense_release(DenseCtx* d, bool own_streams) {
       if (s) cudaStreamDestroy(s);
 }
 
-// (Re)plans the storage of S / the packed factor for the current (n_d, rank count).
-int plan_dense(b200ba_handle* h) {
-  if (!h->own_dense || !h->have_layout) return 0;
-  const int nd = h->L.nd;
-  if (h->dense_planned_n == nd && h->dense_planned_ranks == h->n_ranks) return 0;
+// (Re)plans the storage of S / the packed factor for L.nd and the current rank count, in place of the previous plan.
+int plan_dense(b200ba_handle* h, const Layout& L) {
+  const int nd = L.nd;
+  if (!h->own_dense || (h->dense_planned_n == nd && h->dense_planned_ranks == h->n_ranks)) return 0;
+  h->dense_planned_n = -1;
+  h->dense_mem.release();
   DenseCtx& d = h->dn;
+  Allocations& m = h->dense_mem;
   // one GPU: 512-wide block columns (fewer, longer panels); several ranks: 256, so that the block-cyclic distribution has enough blocks per rank and the broadcasts stay short
   const int nb = h->dense_nb > 0 ? h->dense_nb : (h->n_ranks == 1 ? 512 : 256);
   dense_plan(&d, nd, nb, h->rank, h->n_ranks);
-  if (dev_alloc(h, &h->d_S, static_cast<size_t>(std::max<int64_t>(1, d.chunk * h->n_ranks)))) return 1;
+  if (dev_alloc(h, m, &h->d_S, static_cast<size_t>(std::max<int64_t>(1, d.chunk * h->n_ranks)))) return 1;
   d.S = h->d_S;
-  if (dev_alloc(h, &d.Lpack, static_cast<size_t>(std::max<int64_t>(1, d.panel_off[d.nblk])))) return 1;
-  if (dev_alloc(h, &d.tmp, std::max(1, nd))) return 1;
-  if (dev_alloc(h, &d.d_panel_off, d.panel_off.size())) return 1;
-  if (dev_alloc(h, &d.d_panel_h, d.panel_h.size())) return 1;
+  if (dev_alloc(h, m, &d.Lpack, static_cast<size_t>(std::max<int64_t>(1, d.panel_off[d.nblk])))) return 1;
+  if (dev_alloc(h, m, &d.tmp, std::max(1, nd))) return 1;
+  if (dev_alloc(h, m, &d.d_panel_off, d.panel_off.size())) return 1;
+  if (dev_alloc(h, m, &d.d_panel_h, d.panel_h.size())) return 1;
   CUDA_TRY(h, cudaMemcpy(d.d_panel_off, d.panel_off.data(), d.panel_off.size() * sizeof(int64_t), cudaMemcpyHostToDevice));
   CUDA_TRY(h, cudaMemcpy(d.d_panel_h, d.panel_h.data(), d.panel_h.size() * sizeof(int), cudaMemcpyHostToDevice));
   {
     std::vector<int> ident(std::max(1, nd));
     for (int i = 0; i < nd; ++i) ident[i] = i;
-    if (dev_alloc(h, &h->d_ident_cols, ident.size())) return 1;
+    if (dev_alloc(h, m, &h->d_ident_cols, ident.size())) return 1;
     CUDA_TRY(h, cudaMemcpy(h->d_ident_cols, ident.data(), ident.size() * sizeof(int), cudaMemcpyHostToDevice));
   }
-  if (dev_alloc(h, &h->d_gemv_partial, static_cast<size_t>(gemv_t_partial_size(h->L.nbd, std::max(1, nd))))) return 1;
+  if (dev_alloc(h, m, &h->d_gemv_partial, static_cast<size_t>(gemv_t_partial_size(L.nbd, std::max(1, nd))))) return 1;
   // the un-owned chunks of S are never written by the contraction of a single rank but are read by nobody either;
   // zero once so that partial sums start clean
   CUDA_TRY(h, cudaMemset(h->d_S, 0, static_cast<size_t>(std::max<int64_t>(1, d.chunk * h->n_ranks)) * sizeof(double)));
@@ -499,7 +534,16 @@ int plan_dense(b200ba_handle* h) {
   return 0;
 }
 
+// Frees the layout's and the dense plan's buffers, also after a failure to make them, so that the next call starts over.
+void drop_layout(b200ba_handle* h) {
+  h->have_layout = false;
+  h->dense_planned_n = -1;
+  h->layout_mem.release();
+  h->dense_mem.release();
+}
+
 // ---- layout / buffers ----------------------------------------------------------------------
+// The layout for opt, and its buffers. h->L and have_layout change only once every buffer exists.
 int make_layout(b200ba_handle* h, const b200ba_options* opt) {
   if (opt->regularization_weight != 0) {
     // the reference logs an error and carries on without the term (joint_optimization.cc:299-305)
@@ -551,35 +595,21 @@ int make_layout(b200ba_handle* h, const b200ba_options* opt) {
   L.jc_rig = 9;
   L.jc_intr = 9 + (L.rig_in_state ? 6 : 0);
   L.n_jcols = L.jc_intr + kmax;
-  const bool same = h->have_layout && memcmp(&L, &h->L, sizeof(Layout)) == 0;
-  if (same) return plan_dense(h);
-  h->L = L;
-  h->have_layout = true;
-  h->dense_planned_n = -1;
-
+  if (h->have_layout && memcmp(&L, &h->L, sizeof(Layout)) == 0) return plan_dense(h, L);
+  drop_layout(h);
+  Allocations& m = h->layout_mem;
   const int64_t n = h->n_obs;
-  if (dev_alloc(h, &h->out.residual, 2 * n)) return 1;
-  if (dev_alloc(h, &h->out.cost, n)) return 1;
+  if (dev_alloc(h, m, &h->out.residual, 2 * n)) return 1;
+  if (dev_alloc(h, m, &h->out.cost, n)) return 1;
   // compact Jacobian records when every camera is central-generic
   h->out.compact = (h->uniform_model == B200BA_MODEL_CENTRAL_GENERIC) ? 1 : 0;
-  if (h->out.compact) {
-    if (h->out.jac) cudaFree(h->out.jac);
-    h->out.jac = nullptr;
-    if (dev_alloc(h, &h->out.cjac, 14 * static_cast<size_t>(n))) return 1;
-  } else {
-    if (dev_alloc(h, &h->out.jac, 2 * static_cast<size_t>(L.n_jcols) * n)) return 1;
-  }
-  if (dev_alloc(h, &h->out.cell, n)) return 1;
-  if (dev_alloc(h, &h->out.has_jac, n)) return 1;
-  if (dev_alloc(h, &h->out.evals, n)) return 1;
-  h->out_trial.evals = nullptr;
-  if (dev_alloc(h, &h->out_trial.residual, 2 * n)) return 1;
-  if (dev_alloc(h, &h->out_trial.cost, n)) return 1;
-  h->out_trial.jac = nullptr;
-  h->out_trial.cjac = nullptr;
-  h->out_trial.compact = 0;
-  h->out_trial.cell = nullptr;
-  h->out_trial.has_jac = nullptr;
+  if (h->out.compact && dev_alloc(h, m, &h->out.cjac, 14 * static_cast<size_t>(n))) return 1;
+  if (!h->out.compact && dev_alloc(h, m, &h->out.jac, 2 * static_cast<size_t>(L.n_jcols) * n)) return 1;
+  if (dev_alloc(h, m, &h->out.cell, n)) return 1;
+  if (dev_alloc(h, m, &h->out.has_jac, n)) return 1;
+  if (dev_alloc(h, m, &h->out.evals, n)) return 1;
+  if (dev_alloc(h, m, &h->out_trial.residual, 2 * n)) return 1;
+  if (dev_alloc(h, m, &h->out_trial.cost, n)) return 1;
 
   // the normal equations: one allocation (one all-reduce)
   SystemDev& s = h->sys;
@@ -594,27 +624,27 @@ int make_layout(b200ba_handle* h, const b200ba_options* opt) {
   const int64_t oC = osc + 32;
   s.total = oC + align32(static_cast<int64_t>(L.nd) * L.nd);
   h->reduce_count = oC;
-  if (dev_alloc(h, &s.base, s.total)) return 1;
+  if (dev_alloc(h, m, &s.base, s.total)) return 1;
   s.Dblk = s.base + oD;
   s.bp = s.base + obp;
   s.B = s.base + oB;
   s.C = s.base + oC;
   s.bd = s.base + obd;
   s.scalars = s.base + osc;
-  if (dev_alloc(h, &h->d_W, static_cast<size_t>(L.nbd) * L.nd)) return 1;
+  if (dev_alloc(h, m, &h->d_W, static_cast<size_t>(L.nbd) * L.nd)) return 1;
   if (!h->own_dense) {
-    if (dev_alloc(h, &h->d_S, static_cast<size_t>(L.nd) * L.nd + L.nd)) return 1;  // + partial rhs tail
-  } else if (plan_dense(h)) {
+    if (dev_alloc(h, m, &h->d_S, static_cast<size_t>(L.nd) * L.nd + L.nd)) return 1;  // + partial rhs tail
+  } else if (plan_dense(h, L)) {
     return 1;
   }
-  if (dev_alloc(h, &h->d_Linv, static_cast<size_t>(L.dsz) * L.nblocks)) return 1;
-  if (dev_alloc(h, &h->d_v, L.nbd)) return 1;
-  if (dev_alloc(h, &h->d_y, L.nbd)) return 1;
-  if (dev_alloc(h, &h->d_x, L.dof)) return 1;
+  if (dev_alloc(h, m, &h->d_Linv, static_cast<size_t>(L.dsz) * L.nblocks)) return 1;
+  if (dev_alloc(h, m, &h->d_v, L.nbd)) return 1;
+  if (dev_alloc(h, m, &h->d_y, L.nbd)) return 1;
+  if (dev_alloc(h, m, &h->d_x, L.dof)) return 1;
   int lwork = 0;
   CUSOLVER_TRY(h, cusolverDnDpotrf_bufferSize(h->cusolver, CUBLAS_FILL_MODE_LOWER, L.nd, h->d_S, std::max(1, L.nd), &lwork));
   h->potrf_lwork = lwork;
-  if (dev_alloc(h, &h->d_potrf_work, std::max(1, lwork))) return 1;
+  if (dev_alloc(h, m, &h->d_potrf_work, std::max(1, lwork))) return 1;
 
   // ---- groups of Schur blocks for the structured contraction ------------------------------------
   {
@@ -631,8 +661,10 @@ int make_layout(b200ba_handle* h, const b200ba_options* opt) {
       }
     }
     if (reduce_group_sums(h)) return 1;
-    if (build_groups(h, true)) return 1;
+    if (build_groups(h, L, true)) return 1;
   }
+  h->L = L;
+  h->have_layout = true;
   return 0;
 }
 
@@ -1124,45 +1156,9 @@ int check_ready(b200ba_handle* h, const b200ba_options* opt) {
     return 2;
   }
   CUDA_TRY(h, cudaSetDevice(h->device));
-  return make_layout(h, opt);
-}
-
-void free_handle_buffers(b200ba_handle* h) {
-  auto F = [](auto*& p) {
-    if (p) cudaFree(p);
-    p = nullptr;
-  };
-  F(h->d_obs_imageset); F(h->d_obs_camera); F(h->d_obs_point); F(h->d_obs_xy);
-  for (int i = 0; i < 2; ++i) {
-    F(h->st[i].points); F(h->st[i].rig_tr_global); F(h->st[i].camera_tr_rig); F(h->st[i].intrinsics);
-    F(h->st[i].image_tr_global); F(h->st[i].tangents);
-  }
-  F(h->d_last_projection);
-  F(h->snap.points); F(h->snap.rig_tr_global); F(h->snap.camera_tr_rig); F(h->snap.intrinsics); F(h->d_snap_lp);
-  h->have_snapshot = false;
-  F(h->out.residual); F(h->out.cost); F(h->out.jac); F(h->out.cjac); F(h->out.cell); F(h->out.has_jac); F(h->out.evals);
-  F(h->out_trial.residual); F(h->out_trial.cost);
-  F(h->sys.base); F(h->d_W); F(h->d_S); F(h->d_Linv); F(h->d_v); F(h->d_y); F(h->d_x); F(h->d_potrf_work);
-  F(h->d_info); F(h->d_fail); F(h->d_straggler_list); F(h->d_straggler_count); F(h->d_perm); F(h->d_lp_stage);
-  F(h->d_group_of_block); F(h->d_group_blocks); F(h->d_flags); F(h->d_cols); F(h->d_count); F(h->d_Wc); F(h->d_P); F(h->d_u);
-  F(h->d_contract);
-  if (h->h_count) cudaFreeHost(h->h_count);
-  h->h_count = nullptr;
-  if (h->h_contract) cudaFreeHost(h->h_contract);
-  h->h_contract = nullptr;
-  F(h->d_partial); F(h->d_scal); F(h->d_rot);
-  F(h->rep.err); F(h->rep.mag); F(h->rep.cam_off); F(h->rep.cell_off); F(h->rep.cell_order); F(h->rep.Q);
-  F(h->rep.partial); F(h->rep.select_hist); F(h->rep.hist); F(h->rep.kl); F(h->rep.cams); F(h->d_rep_stage);
-  h->have_report = false;
-  F(h->d_img_group_off); F(h->d_img_group_obs);
-  h->have_images = false;
-  F(h->dn.Lpack); F(h->dn.tmp); F(h->dn.d_panel_off); F(h->dn.d_panel_h); F(h->d_ident_cols); F(h->d_gemv_partial);
-  h->dn.S = nullptr;
-  h->dense_planned_n = -1;
-  if (h->h_scal) cudaFreeHost(h->h_scal);
-  if (h->h_flags) cudaFreeHost(h->h_flags);
-  h->h_scal = nullptr;
-  h->h_flags = nullptr;
+  if (make_layout(h, opt) == 0) return 0;
+  drop_layout(h);
+  return 1;
 }
 
 // First b200ba_calibration_report: allocates the report's buffers and uploads what depends on the problem
@@ -1213,11 +1209,12 @@ int setup_report(b200ba_handle* h) {
     }
   for (double& q : Q) q /= q_sum;
   ReportDev& r = h->rep;
-  if (dev_alloc(h, &r.err, n) || dev_alloc(h, &r.mag, n) || dev_alloc(h, &r.cam_off, nc + 1) ||
-      dev_alloc(h, &r.cell_off, cell_off.size()) || dev_alloc(h, &r.cell_order, n) || dev_alloc(h, &r.Q, 64) ||
-      dev_alloc(h, &r.partial, report_partial_size(nc)) || dev_alloc(h, &r.select_hist, 256 * nc) ||
-      dev_alloc(h, &r.hist, static_cast<size_t>(nc) * B200BA_REPORT_HIST * B200BA_REPORT_HIST) ||
-      dev_alloc(h, &r.kl, static_cast<size_t>(nc) * kCells) || dev_alloc(h, &r.cams, nc) || dev_alloc(h, &h->d_rep_stage, n))
+  Allocations& m = h->problem_mem;
+  if (dev_alloc(h, m, &r.err, n) || dev_alloc(h, m, &r.mag, n) || dev_alloc(h, m, &r.cam_off, nc + 1) ||
+      dev_alloc(h, m, &r.cell_off, cell_off.size()) || dev_alloc(h, m, &r.cell_order, n) || dev_alloc(h, m, &r.Q, 64) ||
+      dev_alloc(h, m, &r.partial, report_partial_size(nc)) || dev_alloc(h, m, &r.select_hist, 256 * nc) ||
+      dev_alloc(h, m, &r.hist, static_cast<size_t>(nc) * B200BA_REPORT_HIST * B200BA_REPORT_HIST) ||
+      dev_alloc(h, m, &r.kl, static_cast<size_t>(nc) * kCells) || dev_alloc(h, m, &r.cams, nc) || dev_alloc(h, m, &h->d_rep_stage, n))
     return 1;
   CUDA_TRY(h, cudaMemcpy(r.cam_off, cam_off.data(), cam_off.size() * sizeof(int64_t), cudaMemcpyHostToDevice));
   CUDA_TRY(h, cudaMemcpy(r.cell_off, cell_off.data(), cell_off.size() * sizeof(int), cudaMemcpyHostToDevice));
@@ -1262,7 +1259,8 @@ int setup_images(b200ba_handle* h) {
   }
   group_off.push_back(static_cast<int>(keyed.size()));
   for (int c = 0; c < nc; ++c) h->img_cam_groups[c + 1] += h->img_cam_groups[c];
-  if (dev_alloc(h, &h->d_img_group_off, group_off.size()) || dev_alloc(h, &h->d_img_group_obs, group_obs.size())) return 1;
+  Allocations& m = h->problem_mem;
+  if (dev_alloc(h, m, &h->d_img_group_off, group_off.size()) || dev_alloc(h, m, &h->d_img_group_obs, group_obs.size())) return 1;
   CUDA_TRY(h, cudaMemcpy(h->d_img_group_off, group_off.data(), group_off.size() * sizeof(int), cudaMemcpyHostToDevice));
   if (!group_obs.empty())
     CUDA_TRY(h, cudaMemcpy(h->d_img_group_obs, group_obs.data(), group_obs.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
@@ -1275,16 +1273,13 @@ int setup_images(b200ba_handle* h) {
 struct CallScope {
   std::string* error;  // receives the first error message
   int rc = 0;          // 1 after the first error
-  std::vector<void*> buffers;
+  Allocations buffers;
   cudaEvent_t events[3] = {};
   cublasHandle_t cublas = nullptr;
   cusolverDnHandle_t cusolver = nullptr;
 
   explicit CallScope(std::string* error_sink) : error(error_sink) {}
-  CallScope(const CallScope&) = delete;
-  CallScope& operator=(const CallScope&) = delete;
   ~CallScope() {
-    for (void* p : buffers) cudaFree(p);
     for (cudaEvent_t e : events)
       if (e) cudaEventDestroy(e);
     if (cublas) cublasDestroy(cublas);
@@ -1311,9 +1306,7 @@ struct CallScope {
     return e == cudaSuccess;
   }
   template <class T>
-  void alloc(T** p, size_t count) {
-    if (ok(cudaMalloc(p, sizeof(T) * count))) buffers.push_back(*p);
-  }
+  void alloc(T** p, size_t count) { ok(buffers.alloc(p, count)); }
   // records timing event k on stream s; all events are created on the first call, so none is created inside a window
   void record(int k, cudaStream_t s) {
     for (cudaEvent_t& e : events)
@@ -1444,6 +1437,18 @@ int download_system(b200ba_handle* h, double* H, double* b) {
 
 }  // namespace
 
+b200ba_handle::~b200ba_handle() {
+  for (cudaEvent_t e : event_pool) cudaEventDestroy(e);
+  for (cudaEvent_t e : {ev_syrk[0], ev_syrk[1], ev_scatter[0], ev_scatter[1], ev_s_ready})
+    if (e) cudaEventDestroy(e);
+  dense_release(&dn, /*own_streams=*/false);
+  for (Allocations* m : {&dense_mem, &layout_mem, &problem_mem}) m->release();
+  if (cublas) cublasDestroy(cublas);
+  if (cusolver) cusolverDnDestroy(cusolver);
+  for (cudaStream_t s : {stream, side_stream, panel_stream, aux_stream})
+    if (s) cudaStreamDestroy(s);
+}
+
 // ==============================================================================================
 // C ABI
 // ==============================================================================================
@@ -1514,11 +1519,6 @@ int b200ba_create(const b200ba_problem* p, int device, b200ba_handle** out) {
   b200ba_handle* h = new b200ba_handle();
   auto fail = [&](int rc) {
     g_create_error = h->error;
-    free_handle_buffers(h);
-    if (h->cublas) cublasDestroy(h->cublas);
-    if (h->cusolver) cusolverDnDestroy(h->cusolver);
-    if (h->stream) cudaStreamDestroy(h->stream);
-    if (h->side_stream) cudaStreamDestroy(h->side_stream);
     delete h;
     return rc;
   };
@@ -1571,10 +1571,11 @@ int b200ba_create(const b200ba_problem* p, int device, b200ba_handle** out) {
     if (h->cams_host[c].model_type != h->uniform_model) h->uniform_model = -1;
   }
   const int64_t n = p->n_obs;
-  TRYC(dev_alloc(h, &h->d_obs_imageset, n));
-  TRYC(dev_alloc(h, &h->d_obs_camera, n));
-  TRYC(dev_alloc(h, &h->d_obs_point, n));
-  TRYC(dev_alloc(h, &h->d_obs_xy, n));
+  Allocations& m = h->problem_mem;
+  TRYC(dev_alloc(h, m, &h->d_obs_imageset, n));
+  TRYC(dev_alloc(h, m, &h->d_obs_camera, n));
+  TRYC(dev_alloc(h, m, &h->d_obs_point, n));
+  TRYC(dev_alloc(h, m, &h->d_obs_xy, n));
   if (n > 0) {
     // Static cell-major order: sort the observations ONCE by (camera, B-spline cell of the
     // measured pixel). Lanes of a warp then gather the same 4x4 control points (broadcast loads
@@ -1611,10 +1612,10 @@ int b200ba_create(const b200ba_problem* p, int device, b200ba_handle** out) {
       txy[2 * i + 1] = p->obs_xy[2 * h->perm[i] + 1];
     }
     TRYC(cuda_ok(cudaMemcpy(h->d_obs_xy, txy.data(), n * sizeof(float2), cudaMemcpyHostToDevice), "H2D"));
-    TRYC(dev_alloc(h, &h->d_perm, n));
+    TRYC(dev_alloc(h, m, &h->d_perm, n));
     TRYC(cuda_ok(cudaMemcpy(h->d_perm, h->perm.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice), "H2D"));
   }
-  TRYC(dev_alloc(h, &h->d_lp_stage, n));
+  TRYC(dev_alloc(h, m, &h->d_lp_stage, n));
   if (n > 0) {
     h->h_obs_imageset.assign(p->obs_imageset, p->obs_imageset + n);
     h->h_obs_camera.assign(p->obs_camera, p->obs_camera + n);
@@ -1636,23 +1637,23 @@ int b200ba_create(const b200ba_problem* p, int device, b200ba_handle** out) {
   h->pb.obs_point = h->d_obs_point;
   h->pb.obs_xy = h->d_obs_xy;
   for (int i = 0; i < 2; ++i) {
-    TRYC(dev_alloc(h, &h->st[i].points, 3 * static_cast<size_t>(h->n_points)));
-    TRYC(dev_alloc(h, &h->st[i].rig_tr_global, 7 * static_cast<size_t>(h->n_imagesets)));
-    TRYC(dev_alloc(h, &h->st[i].camera_tr_rig, 7 * static_cast<size_t>(h->n_cameras)));
-    TRYC(dev_alloc(h, &h->st[i].intrinsics, h->intr_total));
-    TRYC(dev_alloc(h, &h->st[i].image_tr_global, 12 * static_cast<size_t>(h->n_imagesets) * h->n_cameras));
-    TRYC(dev_alloc(h, &h->st[i].tangents, h->tan_total));
+    TRYC(dev_alloc(h, m, &h->st[i].points, 3 * static_cast<size_t>(h->n_points)));
+    TRYC(dev_alloc(h, m, &h->st[i].rig_tr_global, 7 * static_cast<size_t>(h->n_imagesets)));
+    TRYC(dev_alloc(h, m, &h->st[i].camera_tr_rig, 7 * static_cast<size_t>(h->n_cameras)));
+    TRYC(dev_alloc(h, m, &h->st[i].intrinsics, h->intr_total));
+    TRYC(dev_alloc(h, m, &h->st[i].image_tr_global, 12 * static_cast<size_t>(h->n_imagesets) * h->n_cameras));
+    TRYC(dev_alloc(h, m, &h->st[i].tangents, h->tan_total));
   }
-  TRYC(dev_alloc(h, &h->d_last_projection, n));
+  TRYC(dev_alloc(h, m, &h->d_last_projection, n));
   TRYC(cuda_ok(cudaMemset(h->d_last_projection, 0, std::max<int64_t>(1, n) * sizeof(double2)), "memset"));
-  TRYC(dev_alloc(h, &h->d_straggler_list, n));
-  TRYC(dev_alloc(h, &h->d_straggler_count, 1));
-  TRYC(dev_alloc(h, &h->d_info, 2));
-  TRYC(dev_alloc(h, &h->d_fail, 1));
-  TRYC(dev_alloc(h, &h->d_partial, cost_reduce_partial_size()));
-  TRYC(dev_alloc(h, &h->d_scal, 16));
-  TRYC(cuda_ok(cudaMallocHost(reinterpret_cast<void**>(&h->h_scal), 16 * sizeof(double)), "cudaMallocHost"));
-  TRYC(cuda_ok(cudaMallocHost(reinterpret_cast<void**>(&h->h_flags), 4 * sizeof(int)), "cudaMallocHost"));
+  TRYC(dev_alloc(h, m, &h->d_straggler_list, n));
+  TRYC(dev_alloc(h, m, &h->d_straggler_count, 1));
+  TRYC(dev_alloc(h, m, &h->d_info, 2));
+  TRYC(dev_alloc(h, m, &h->d_fail, 1));
+  TRYC(dev_alloc(h, m, &h->d_partial, cost_reduce_partial_size()));
+  TRYC(dev_alloc(h, m, &h->d_scal, 16));
+  TRYC(cuda_ok(m.alloc(&h->h_scal, 16, /*pinned=*/true), "cudaMallocHost"));
+  TRYC(cuda_ok(m.alloc(&h->h_flags, 4, /*pinned=*/true), "cudaMallocHost"));
 #undef TRYC
   *out = h;
   return 0;
@@ -1664,20 +1665,6 @@ void b200ba_destroy(b200ba_handle* h) {
   if (h->stream) cudaStreamSynchronize(h->stream);
   if (h->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(h->comm);
   resolve_timings(h);
-  for (auto e : h->event_pool) cudaEventDestroy(e);
-  for (int i = 0; i < 2; ++i) {
-    if (h->ev_syrk[i]) cudaEventDestroy(h->ev_syrk[i]);
-    if (h->ev_scatter[i]) cudaEventDestroy(h->ev_scatter[i]);
-  }
-  if (h->ev_s_ready) cudaEventDestroy(h->ev_s_ready);
-  free_handle_buffers(h);
-  if (h->cublas) cublasDestroy(h->cublas);
-  if (h->cusolver) cusolverDnDestroy(h->cusolver);
-  if (h->stream) cudaStreamDestroy(h->stream);
-  if (h->side_stream) cudaStreamDestroy(h->side_stream);
-  if (h->panel_stream) cudaStreamDestroy(h->panel_stream);
-  if (h->aux_stream) cudaStreamDestroy(h->aux_stream);
-  dense_release(&h->dn, /*own_streams=*/false);
   delete h;
 }
 
@@ -1748,12 +1735,12 @@ int b200ba_snapshot_state(b200ba_handle* h) {
     return 2;
   }
   CUDA_TRY(h, cudaSetDevice(h->device));
-  if (!h->snap.points) {
-    if (dev_alloc(h, &h->snap.points, 3 * static_cast<size_t>(h->n_points))) return 1;
-    if (dev_alloc(h, &h->snap.rig_tr_global, 7 * static_cast<size_t>(h->n_imagesets))) return 1;
-    if (dev_alloc(h, &h->snap.camera_tr_rig, 7 * static_cast<size_t>(h->n_cameras))) return 1;
-    if (dev_alloc(h, &h->snap.intrinsics, h->intr_total)) return 1;
-    if (dev_alloc(h, &h->d_snap_lp, h->n_obs)) return 1;
+  if (!h->d_snap_lp) {
+    if (dev_alloc(h, h->problem_mem, &h->snap.points, 3 * static_cast<size_t>(h->n_points))) return 1;
+    if (dev_alloc(h, h->problem_mem, &h->snap.rig_tr_global, 7 * static_cast<size_t>(h->n_imagesets))) return 1;
+    if (dev_alloc(h, h->problem_mem, &h->snap.camera_tr_rig, 7 * static_cast<size_t>(h->n_cameras))) return 1;
+    if (dev_alloc(h, h->problem_mem, &h->snap.intrinsics, h->intr_total)) return 1;
+    if (dev_alloc(h, h->problem_mem, &h->d_snap_lp, h->n_obs)) return 1;
   }
   if (copy_state_dev(h, h->st[h->cur], h->d_last_projection, h->snap, h->d_snap_lp)) return 1;
   h->have_snapshot = true;
@@ -2196,7 +2183,7 @@ int b200ba_run_bundle_adjustment(b200ba_handle* h, const b200ba_options* opt_in,
     acc.total_ms += h->timings.total_ms;
     if (!opt.localize_only) {
       // beautify all camera orientations (calibration.cc:245-252)
-      if (!h->d_rot && dev_alloc(h, &h->d_rot, 9 * static_cast<size_t>(h->n_cameras))) return 1;
+      if (!h->d_rot && dev_alloc(h, h->problem_mem, &h->d_rot, 9 * static_cast<size_t>(h->n_cameras))) return 1;
       launch_nice_orientation(h->pb, h->st[h->cur], h->n_cameras, h->d_rot, h->stream);
       CUDA_TRY(h, cudaGetLastError());
     }
@@ -2254,13 +2241,12 @@ int b200ba_get_jacobians(b200ba_handle* h, double* j_point, double* j_pose, doub
   std::vector<uint8_t> has(n);
   if (h->out.compact) {
     // rebuild the expanded buffer from the compact records (state of the evaluation = current state)
+    Allocations scratch;
     double* tmp = nullptr;
-    CUDA_TRY(h, cudaMalloc(reinterpret_cast<void**>(&tmp), std::max<size_t>(1, jac.size()) * sizeof(double)));
+    CUDA_TRY(h, scratch.alloc(&tmp, std::max<size_t>(1, jac.size())));
     launch_expand_jacobian(h->pb, L, h->st[h->cur], h->out, tmp, h->stream);
-    cudaError_t e = cudaStreamSynchronize(h->stream);
-    if (e == cudaSuccess) e = cudaMemcpy(jac.data(), tmp, jac.size() * sizeof(double), cudaMemcpyDeviceToHost);
-    cudaFree(tmp);
-    CUDA_TRY(h, e);
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    CUDA_TRY(h, cudaMemcpy(jac.data(), tmp, jac.size() * sizeof(double), cudaMemcpyDeviceToHost));
   } else
     CUDA_TRY(h, cudaMemcpy(jac.data(), h->out.jac, jac.size() * sizeof(double), cudaMemcpyDeviceToHost));
   CUDA_TRY(h, cudaMemcpy(cell.data(), h->out.cell, n * sizeof(int32_t), cudaMemcpyDeviceToHost));
@@ -2413,7 +2399,7 @@ int b200ba_debug_nice_orientation(b200ba_handle* h, double* rot) {
     return 2;
   }
   CUDA_TRY(h, cudaSetDevice(h->device));
-  if (!h->d_rot && dev_alloc(h, &h->d_rot, 9 * static_cast<size_t>(h->n_cameras))) return 1;
+  if (!h->d_rot && dev_alloc(h, h->problem_mem, &h->d_rot, 9 * static_cast<size_t>(h->n_cameras))) return 1;
   launch_nice_orientation(h->pb, h->st[h->cur], h->n_cameras, h->d_rot, h->stream);
   CUDA_TRY(h, cudaGetLastError());
   CUDA_TRY(h, cudaMemcpyAsync(rot, h->d_rot, 9 * sizeof(double) * h->n_cameras, cudaMemcpyDeviceToHost, h->stream));
@@ -2441,6 +2427,13 @@ B200BA_API int b200ba_debug_eval_counts(b200ba_handle* h, uint16_t* counts) {
   CUDA_TRY(h, cudaMemcpy(tmp.data(), h->out.evals, h->n_obs * sizeof(uint16_t), cudaMemcpyDeviceToHost));
   for (int64_t i = 0; i < h->n_obs; ++i) counts[h->perm[i]] = tmp[i];
   return 0;
+}
+
+// Diagnostics / tests: the device and pinned host allocations held by every handle and running call.
+int64_t b200ba_debug_live_allocations(int64_t* device_bytes, int64_t* pinned_bytes) {
+  if (device_bytes) *device_bytes = g_live_bytes[0];
+  if (pinned_bytes) *pinned_bytes = g_live_bytes[1];
+  return g_live_count;
 }
 
 int b200ba_get_timings(const b200ba_handle* h, b200ba_timings* t) {
@@ -4146,11 +4139,15 @@ int b200ba_comm_init(b200ba_handle* h, const uint8_t id[B200BA_NCCL_UNIQUE_ID_BY
   }
   h->rank = rank;
   h->n_ranks = n_ranks;
-  if (plan_dense(h)) return 1;
+  if (!h->have_layout) return 0;
+  if (plan_dense(h, h->L)) {
+    drop_layout(h);
+    return 1;
+  }
   // every rank must derive the same groups of Schur blocks: reduce the centroid sums
   if (h->L.eliminate_points && h->L.nblocks > 0 && !h->grp_sums.empty()) {
     if (reduce_group_sums(h)) return 1;
-    if (build_groups(h, false)) return 1;
+    if (build_groups(h, h->L, false)) return 1;
   }
   return 0;
 }

@@ -953,6 +953,10 @@ B200BA_API int b200ba_debug_nice_orientation(b200ba_handle* h, double* rot);
 #define B200BA_LM_REFUSED_PIVOT 3  /* factorisation met a non-positive pivot; the update was not evaluated */
 /* Copies up to cap codes; returns the number of attempts (-1 for a NULL handle). */
 B200BA_API int32_t b200ba_debug_lm_events(const b200ba_handle* h, int32_t* codes, int32_t cap);
+/* Allocations the library holds right now, over every handle and every running stand-alone call: returns
+ * their number; device_bytes and pinned_bytes (nullable) receive the bytes of device memory and of pinned
+ * host memory. */
+B200BA_API int64_t b200ba_debug_live_allocations(int64_t* device_bytes, int64_t* pinned_bytes);
 
 #ifdef __cplusplus
 }
